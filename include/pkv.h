@@ -7,7 +7,8 @@
  * Conventions
  *  - All tensors hold 16-bit elements of `dtype` (PKV_BF16 / PKV_FP16); strides are in ELEMENTS.
  *    The innermost (head_dim) axis is contiguous; base pointers and row strides are 16-byte aligned.
- *  - Batch size is 1 (as in the reference: README.md:47, batch inference unsupported).
+ *  - Batch size is 1 (as in the reference: README.md:47, batch inference unsupported), except for
+ *    pkv_decode_attn_batch, which decodes the compacted caches of several prompts in one launch.
  *  - Q is [num_q_heads, seq_len, head_dim]; K/V are [num_kv_heads, seq_len, head_dim] and are NOT
  *    repeated: query head h reads kv head h / (num_q_heads / num_kv_heads). Passing
  *    num_kv_heads == num_q_heads reproduces the reference's post-`repeat_kv` call exactly
@@ -230,6 +231,23 @@ int pkv_decode_attn(const pkv_decode_desc* d, void* stream);
  * the same workspace as pkv_decode_attn. Results are those of pkv_decode_attn with length + *step_dev up to the
  * summation order across splits. */
 int pkv_decode_attn_graph(const pkv_decode_desc* d, const int32_t* step_dev, int64_t max_length, void* stream);
+/* The decode step of num_seqs sequences in ONE launch (grid: split x q head x sequence). Replaces, for a batch, the
+ * per-layer torch.cat of the whole batched cache (cache_utils_think.py:383-384, llama_model.py:170) and the attention call
+ * llama_model.py:174-183 / :291-313 / :411-445 — batch inference, which the reference lists as unsupported (README.md:47).
+ * Sequence s, query head h: cache at k_cache + s*cache_stride_b + h*cache_stride_h, query q[s][h], output out[s][h]
+ * (q, out: [num_seqs, num_q_heads, head_dim] contiguous); it appends k_new[s][h / group] / v_new[s][h / group]
+ * (k_new, v_new: [num_seqs, num_kv_heads, head_dim] contiguous, optional) as its last row and attends
+ *     rows = d->length (+ *step_dev when step_dev != NULL) (+ rows[s*num_q_heads + h] when rows != NULL)
+ * rows; `rows` is DEVICE int32 [num_seqs*num_q_heads] (prompts whose compacted caches differ in length, AdaKV / HeadKV
+ * heads). Graph-replayable like pkv_decode_attn_graph: the launch is sized for `max_length` rows (cache_stride_h >=
+ * max_length*head_dim), row counts are read on the device, and each (sequence, head) divides its rows among the splits a
+ * one-sequence launch uses, so every sequence's output and appended row are bit-identical to pkv_decode_attn_graph /
+ * pkv_decode_attn_ragged on that sequence alone. A (sequence, head) whose row count falls outside [1, max_length] reads
+ * and writes no row; its output is NaN. Workspace: pkv_decode_workspace_bytes with num_q_heads = num_seqs*num_q_heads.
+ * PKV_ERR_INVALID_ARG: num_seqs outside [1, 65535], cache_stride_b < num_q_heads*cache_stride_h, max_length < length or
+ * above the capacity, misaligned rows / step_dev. */
+int pkv_decode_attn_batch(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
+                          const int32_t* step_dev, int64_t max_length, void* stream);
 /* Append only (no attention): writes k_new/v_new as row length-1. */
 int pkv_cache_append(const pkv_decode_desc* d, void* stream);
 

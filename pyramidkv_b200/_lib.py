@@ -20,7 +20,7 @@ EXPORTS = [
     "pkv_evict_workspace_bytes", "pkv_evict_prefill", "pkv_stage_scores", "pkv_stage_pool", "pkv_stage_topk",
     "pkv_stage_gather", "pkv_decode_workspace_bytes", "pkv_decode_attn", "pkv_decode_attn_graph", "pkv_cache_append", "pkv_host_pick_rows", "pkv_debug_read_stamps", "pkv_rope_inplace", "pkv_update_flatten_view", "pkv_adakv_scratch_bytes", "pkv_adakv_counts",
     "pkv_ragged_place_window", "pkv_decode_attn_ragged", "pkv_evict_single_launch", "pkv_stage_scan_pool",
-    "pkv_evict_prefill_batch", "pkv_evict_batch_supported", "pkv_stage_batch",
+    "pkv_evict_prefill_batch", "pkv_evict_batch_supported", "pkv_stage_batch", "pkv_decode_attn_batch",
 ]
 
 
@@ -133,6 +133,8 @@ def lib() -> C.CDLL:
     L.pkv_rope_inplace.restype = i32
     L.pkv_decode_attn_graph.argtypes = [C.POINTER(DecodeDesc), p, i64, p]
     L.pkv_decode_attn_graph.restype = i32
+    L.pkv_decode_attn_batch.argtypes = [C.POINTER(DecodeDesc), C.c_int32, i64, p, p, i64, p]
+    L.pkv_decode_attn_batch.restype = i32
     if L.pkv_version() != 3:
         raise RuntimeError(f"libpkv ABI version {L.pkv_version()} != 3; rebuild with `python -m pyramidkv_b200.build --force`")
     _lib = L

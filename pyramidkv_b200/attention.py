@@ -22,7 +22,7 @@ from typing import Callable, Optional
 import torch
 from transformers.modeling_utils import ALL_ATTENTION_FUNCTIONS
 
-from .cache import PkvCacheLayer, PkvRaggedCacheLayer, install_layer, layer_is_empty
+from .cache import PkvBatchCacheLayer, PkvCacheLayer, PkvRaggedCacheLayer, install_layer, layer_is_empty
 from .kv_cluster import INIT_BY_METHOD, flush_pending
 
 DEFAULT_DECODE_RESERVE = 256   # rows of head-room behind the compacted prompt (grows by doubling)
@@ -77,8 +77,14 @@ def make_forward(method: str, modeling, original_forward):
         if getattr(self.config, "pkv_fused_rope", False) and not torch.is_grad_enabled():
             # SURVEY.md §8 f2: one in-place launch (pkv_rope_inplace) instead of HF's ten elementwise launches and four
             # full-size temporaries; bit-identical results. Opt-in knob on the shared config, like the reference's knobs.
-            for b in range(bsz):
-                cluster.backend.rope_inplace(query_states[b], key_states[b], cos[b if cos.shape[0] > 1 else 0], sin[b if sin.shape[0] > 1 else 0])
+            if q_len == 1 and bsz > 1:
+                # a batched decode step: one launch with the batch axis as the token axis (q [Hq, B, D], cos / sin [B, D])
+                cs = (cos, sin) if cos.shape[0] == bsz else (cos.expand(bsz, -1, -1).contiguous(), sin.expand(bsz, -1, -1).contiguous())
+                cluster.backend.rope_inplace(query_states[:, :, 0, :].transpose(0, 1), key_states[:, :, 0, :].transpose(0, 1),
+                                             cs[0][:, 0, :], cs[1][:, 0, :])
+            else:
+                for b in range(bsz):
+                    cluster.backend.rope_inplace(query_states[b], key_states[b], cos[b if cos.shape[0] > 1 else 0], sin[b if sin.shape[0] > 1 else 0])
         else:
             query_states, key_states = modeling.apply_rotary_pos_emb(query_states, key_states, cos, sin)
         num_q_heads = query_states.shape[1]
@@ -131,10 +137,24 @@ def make_forward(method: str, modeling, original_forward):
             attn_weights = None
             static = getattr(past_key_values, "_pkv_static", None)
             ragged = isinstance(layer, PkvRaggedCacheLayer)
+            joined = isinstance(layer, PkvBatchCacheLayer)
             # rows = `rows_arg` (+ head_rows[h] for ragged caches, + the device step counter in static mode)
             rows_arg = (layer.appended if ragged else layer.length) + 1
             head_rows = {"head_rows": layer.head_rows} if ragged else {}
-            if q_len == 1 and static is not None:
+            if q_len == 1 and (bsz > 1 or joined):
+                # several sequences: ONE launch for the batch. Rows = layer.length + 1 (equal-length batched prefill) or
+                # layer.rows[b, h] + 1 (joined prompts), + the device step counter in static mode
+                if static is None:
+                    layer.reserve(1)
+                out = cluster.backend.decode_attn_batch(
+                    query_states[:, :, 0, :], layer.k_buf, layer.v_buf, 1 if joined else layer.length + 1,
+                    key_states[:, :, 0, :], value_states[:, :, 0, :], rows=layer.rows if joined else None,
+                    step=static.step if static is not None else None, max_length=layer.capacity,
+                    workspace=static.workspace if static is not None else None, softmax_scale=self.scaling)
+                if static is None:
+                    layer.advance(1)
+                attn_output = out[:, None]
+            elif q_len == 1 and static is not None:
                 # graph-replayable step (generate.StaticDecoder): the row count is layer.length + 1 + *static.step on the
                 # device, the buffers were reserved up front and the Python bookkeeping is settled by StaticDecoder.finish()
                 out = torch.empty(bsz, 1, num_q_heads, self.head_dim, dtype=query_states.dtype, device=query_states.device)

@@ -135,6 +135,91 @@ class PkvRaggedCacheLayer(PkvCacheLayer):
         raise NotImplementedError("ragged caches are batch size 1 (pyramidkv_utils.py:723)")
 
 
+class PkvBatchCacheLayer(PkvCacheLayer):
+    """The compacted caches of B prompts, prefilled one at a time and joined (`join_caches`), decoded together: buffers
+    [B, Hq, capacity, D], `rows_host[b][h]` the rows sequence b keeps for head h (prompts shorter than the budget keep
+    every row; AdaKV / HeadKV heads differ) and `rows` the same counts on the device (int32 [B*Hq], what
+    `pkv_decode_attn_batch` adds to its row count). Decode appends one row to every sequence per step; `settle` books the
+    rows each sequence really kept (a sequence that stopped at its EOS keeps fewer). `length` is the longest (sequence,
+    head)'s row count (what the buffers must hold); `seq_seen[b]` the tokens sequence b has seen."""
+
+    def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, rows_host, seq_seen):
+        self.rows_host = [[int(r) for r in row] for row in rows_host]
+        self.seq_seen = [int(s) for s in seq_seen]
+        assert len(self.rows_host) == len(self.seq_seen) == k_buf.shape[0] and all(len(r) == k_buf.shape[1] for r in self.rows_host)
+        self.rows = self._device_rows(k_buf.device)
+        super().__init__(k_buf, v_buf, max(max(r) for r in self.rows_host), max(self.seq_seen))
+
+    def _device_rows(self, device) -> torch.Tensor:
+        return torch.tensor([r for row in self.rows_host for r in row], dtype=torch.int32, device=device)
+
+    def settle(self, appended) -> None:
+        """Sequence b appended `appended[b]` rows to every head (in place, by the decode kernel)."""
+        assert len(appended) == len(self.rows_host)
+        for b, n in enumerate(appended):
+            self.rows_host[b] = [r + int(n) for r in self.rows_host[b]]
+            self.seq_seen[b] += int(n)
+        self.rows = self._device_rows(self.device)     # a new tensor: launches already queued keep reading the old one
+        self.length = max(max(r) for r in self.rows_host)
+        self.seen_tokens = max(self.seq_seen)
+        self._refresh_views()
+
+    def advance(self, rows: int) -> None:
+        self.settle([rows] * len(self.rows_host))
+
+    def head_view(self, b: int, h: int):
+        """Valid rows of sequence b, head h: ([rows, D] keys, values)."""
+        r = self.rows_host[b][h]
+        return self.k_buf[b, h, :r], self.v_buf[b, h, :r]
+
+    def update(self, key_states, value_states, *args, **kwargs):
+        raise NotImplementedError("multi-token append to a joined batch is not defined: its sequences hold different row counts "
+                                  "(decode it one token per step: generate.StaticDecoder / greedy_generate_batch)")
+
+    def batch_repeat_interleave(self, repeats: int) -> None:
+        raise NotImplementedError("a joined batch holds one row count per sequence and head; repeat the prompts before joining")
+
+    def batch_select_indices(self, indices: torch.Tensor) -> None:
+        raise NotImplementedError("a joined batch holds one row count per sequence and head; join the selected prompts instead")
+
+
+def join_caches(caches, reserve: int = 0):
+    """One batched cache from B single-prompt caches filled by the patched prefill (every layer a batch-1 `PkvCacheLayer` or
+    `PkvRaggedCacheLayer`): layer by layer the valid rows are copied once into [B, Hq, longest + reserve, D] buffers
+    (`PkvBatchCacheLayer`). A cache may be passed several times. Stock / FullKV caches raise."""
+    from transformers import DynamicCache
+    if not caches:
+        raise ValueError("join_caches: no caches")
+    n_layers = len(caches[0].layers)
+    for c in caches:
+        if len(c.layers) != n_layers or not all(isinstance(l, PkvCacheLayer) and not isinstance(l, PkvBatchCacheLayer) for l in c.layers):
+            raise RuntimeError("join_caches needs caches prefilled by the patched forward on every layer "
+                               "(method 'fullkv' and stock caches are not compacted)")
+        if any(l.k_buf.shape[0] != 1 for l in c.layers):
+            raise ValueError("join_caches joins single-prompt (batch 1) caches")
+    out = DynamicCache()
+    out.layers = []
+    for i in range(n_layers):
+        src = [c.layers[i] for c in caches]
+        rows = []
+        for l in src:
+            if isinstance(l, PkvRaggedCacheLayer):
+                rows.append([r + l.appended for r in l.head_rows_host])
+            else:
+                rows.append([l.length] * l.k_buf.shape[1])
+        _, hq, _, d = src[0].k_buf.shape
+        if any(l.k_buf.shape[1] != hq or l.k_buf.shape[3] != d or l.dtype != src[0].dtype or l.device != src[0].device for l in src):
+            raise ValueError(f"join_caches: layer {i}: head counts, head_dim, dtype or device differ between the caches")
+        cap = max(max(r) for r in rows) + int(reserve)
+        k = torch.empty(len(src), hq, cap, d, dtype=src[0].dtype, device=src[0].device)
+        v = torch.empty_like(k)
+        for b, l in enumerate(src):
+            k[b, :, : l.length] = l.k_buf[0, :, : l.length]
+            v[b, :, : l.length] = l.v_buf[0, :, : l.length]
+        out.layers.append(PkvBatchCacheLayer(k, v, rows, [l.seen_tokens for l in src]))
+    return out
+
+
 def layer_is_empty(past_key_values, layer_idx: int) -> bool:
     """Prefill detection = "this layer's cache is empty" (the reference compares key length with the
     per-module `kv_seq_len` counter that `prepare_inputs_for_generation` resets — llama_model.py:165, :2609-2612)."""

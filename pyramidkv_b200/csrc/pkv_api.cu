@@ -482,8 +482,8 @@ extern "C" int pkv_stage_batch(const pkv_evict_desc* descs, int n_layers, int st
 extern "C" int pkv_evict_prefill_batch(const pkv_evict_desc* descs, int n_layers, void* stream) { return pkv_stage_batch(descs, n_layers, 0, stream); }
 
 // max_length > 0: graph-replayable launch — `length` is the row count at step 0 and the launch (split count, workspace,
-// capacity check) is sized for max_length rows.
-static int resolve_decode(const pkv_decode_desc* d, DecodeArgs* a, bool need_q, int64_t max_length = 0) {
+// capacity check) is sized for max_length rows. num_seqs sequences: q / out / k_new / v_new hold num_seqs blocks back to back.
+static int resolve_decode(const pkv_decode_desc* d, DecodeArgs* a, bool need_q, int64_t max_length = 0, int num_seqs = 1) {
     if (!d) return fail(PKV_ERR_INVALID_ARG, "null descriptor");
     if (d->struct_bytes != sizeof(pkv_decode_desc))
         return fail(PKV_ERR_INVALID_ARG, "pkv_decode_desc.struct_bytes=%u, library expects %zu (ABI mismatch)", d->struct_bytes, sizeof(pkv_decode_desc));
@@ -510,8 +510,11 @@ static int resolve_decode(const pkv_decode_desc* d, DecodeArgs* a, bool need_q, 
     a->num_sms = di->sms;
     a->nsplit = decode_num_splits(a->Hq, rows_bound, a->num_sms);
     a->ws = static_cast<float*>(d->workspace);
+    a->num_seqs = num_seqs;
+    a->cache_sb = int64_t(a->Hq) * a->cache_sh;
+    a->max_rows = rows_bound;
     if (need_q && a->nsplit > 1) {
-        const uint64_t need = uint64_t(a->Hq) * a->nsplit * (2 + a->D) * sizeof(float);
+        const uint64_t need = uint64_t(num_seqs) * a->Hq * a->nsplit * (2 + a->D) * sizeof(float);
         if (!d->workspace || d->workspace_bytes < need) return fail(PKV_ERR_WORKSPACE, "decode workspace of %llu bytes required", (unsigned long long)need);
     }
     return PKV_OK;
@@ -532,17 +535,36 @@ int pkv_decode_attn(const pkv_decode_desc* d, void* stream) {
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "decode launch");
 }
 
-int pkv_decode_attn_graph(const pkv_decode_desc* d, const int32_t* step_dev, int64_t max_length, void* stream) {
-    if (!step_dev) return fail(PKV_ERR_INVALID_ARG, "pkv_decode_attn_graph: null step counter");
-    if ((reinterpret_cast<uintptr_t>(step_dev) & 3u) != 0) return fail(PKV_ERR_INVALID_ARG, "pkv_decode_attn_graph: step counter must be 4-byte aligned");
-    if (max_length < 1) return fail(PKV_ERR_INVALID_ARG, "pkv_decode_attn_graph: max_length must be >= 1");
+// The device-length decode of num_seqs sequences: pkv_decode_attn_batch, and pkv_decode_attn_graph / pkv_decode_attn_ragged
+// as its one-sequence calls.
+static int decode_devlen(const char* fn, const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
+                         const int32_t* step_dev, int64_t max_length, void* stream) {
+    if ((reinterpret_cast<uintptr_t>(rows) & 3u) || (reinterpret_cast<uintptr_t>(step_dev) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned int32 pointer", fn);
+    if (max_length < 1) return fail(PKV_ERR_INVALID_ARG, "%s: max_length must be >= 1", fn);
+    if (num_seqs < 1 || num_seqs > 65535) return fail(PKV_ERR_INVALID_ARG, "%s: num_seqs=%d outside [1, 65535]", fn, num_seqs);
     DecodeArgs a;
-    int rc = resolve_decode(d, &a, true, max_length);
+    int rc = resolve_decode(d, &a, true, max_length, num_seqs);
     if (rc) return rc;
+    if (num_seqs > 1 && (cache_stride_b < int64_t(a.Hq) * a.cache_sh || cache_stride_b % 8))
+        return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_b=%lld is below num_q_heads*cache_stride_h=%lld or not a multiple of 8", fn,
+                    (long long)cache_stride_b, (long long)(int64_t(a.Hq) * a.cache_sh));
+    if (num_seqs > 1) a.cache_sb = cache_stride_b;
+    a.devlen = true;
+    a.rows = rows;
     a.step_dev = step_dev;
     DeviceGuard guard(d->device);
     const cudaError_t e = launch_decode(a, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "decode launch");
+}
+
+int pkv_decode_attn_batch(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
+                          const int32_t* step_dev, int64_t max_length, void* stream) {
+    return decode_devlen("pkv_decode_attn_batch", d, num_seqs, cache_stride_b, rows, step_dev, max_length, stream);
+}
+
+int pkv_decode_attn_graph(const pkv_decode_desc* d, const int32_t* step_dev, int64_t max_length, void* stream) {
+    if (!step_dev) return fail(PKV_ERR_INVALID_ARG, "pkv_decode_attn_graph: null step counter");
+    return decode_devlen("pkv_decode_attn_graph", d, 1, 0, nullptr, step_dev, max_length, stream);
 }
 
 int pkv_rope_inplace(const pkv_rope_desc* d, void* stream) {
@@ -597,16 +619,7 @@ int pkv_ragged_place_window(const pkv_evict_desc* d, const int32_t* caps, void* 
 
 int pkv_decode_attn_ragged(const pkv_decode_desc* d, const int32_t* head_rows, const int32_t* step_dev, int64_t max_length, void* stream) {
     if (!head_rows) return fail(PKV_ERR_INVALID_ARG, "pkv_decode_attn_ragged: null head_rows");
-    if ((reinterpret_cast<uintptr_t>(head_rows) & 3u) || (reinterpret_cast<uintptr_t>(step_dev) & 3u)) return fail(PKV_ERR_INVALID_ARG, "pkv_decode_attn_ragged: misaligned int32 pointer");
-    if (max_length < 1) return fail(PKV_ERR_INVALID_ARG, "pkv_decode_attn_ragged: max_length must be >= 1");
-    DecodeArgs a;
-    int rc = resolve_decode(d, &a, true, max_length);
-    if (rc) return rc;
-    a.head_rows = head_rows;
-    a.step_dev = step_dev;
-    DeviceGuard guard(d->device);
-    const cudaError_t e = launch_decode(a, static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "decode launch");
+    return decode_devlen("pkv_decode_attn_ragged", d, 1, 0, head_rows, step_dev, max_length, stream);
 }
 
 int pkv_update_flatten_view(void* dst, const void* src, const void* state, const int32_t* head_lens, const int32_t* cu_lens,

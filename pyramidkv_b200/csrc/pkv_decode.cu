@@ -5,7 +5,9 @@
 // attention launch (eager llama_model.py:174-183, sdpa :291-313, flash :411-445 -> flash_attn_func :77).
 // q_len == 1 and every cached row is visible, so there is no mask. One launch for T <= 256 rows per
 // head; longer caches are split along T (flash-decoding) and merged by a second small kernel.
-// HBM-bound: reads 2*Hq*T*D*2 bytes; each row is fetched with 128-bit loads, D/8 lanes per row.
+// Several sequences decoded in lock-step share one launch: the grid is (split, q head, sequence), and every
+// (sequence, head) divides its own rows among the splits a one-sequence launch would use.
+// HBM-bound: reads 2*Hq*T*D*2 bytes per sequence; each row is fetched with 128-bit loads, D/8 lanes per row.
 #include "pkv_common.cuh"
 #include "pkv_internal.h"
 
@@ -27,14 +29,14 @@ __host__ __device__ inline int64_t splits_for(int64_t Hq, int64_t T, int64_t num
 }
 
 struct DecodeParams {
-    const uint16_t *q, *k_new, *v_new;
-    uint16_t *k_cache, *v_cache, *out;
-    int64_t cache_sh, T, chunk;
+    const uint16_t *q, *k_new, *v_new;   // q [num_seqs][Hq][D], k_new / v_new [num_seqs][Hkv][D]
+    uint16_t *k_cache, *v_cache, *out;   // caches at + s*cache_sb + h*cache_sh; out [num_seqs][Hq][D]
+    int64_t cache_sh, cache_sb, T, chunk, max_rows;
     int G, nsplit, num_sms;
     float scale;
-    float* ws;  // [Hq][nsplit][2 + D] partial (m, l, acc) when nsplit > 1
+    float* ws;  // [num_seqs*Hq][nsplit][2 + D] partial (m, l, acc) when nsplit > 1
     const int32_t* step_dev;  // DEVLEN kernels: rows = T + *step_dev (graph-replayable decode; the grid is sized for the maximum)
-    const int32_t* head_rows; // DEVLEN kernels: + head_rows[h] (ragged AdaKV / HeadKV caches: every head has its own row count)
+    const int32_t* rows;      // DEVLEN kernels: + rows[s*Hq + h] (rows of each sequence and head: joined prompts, AdaKV / HeadKV)
 };
 
 template <typename T>
@@ -51,6 +53,9 @@ __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
 // current step is read from device memory, so that ONE captured launch (CUDA graph) serves every decode step; the grid
 // is sized for the cache capacity, and the rows are divided in-kernel among the splits a host launch for the current row
 // count would use (the others stay empty), so both forms add the same terms in the same order: the same output bits.
+// The split count comes from the per-sequence head count gridDim.y, so a sequence gets the same bits in a batch as alone.
+// A row count outside [1, max_rows] (the capacity the launch was checked against) is treated as 0: nothing is read or
+// written but the output, which becomes NaN.
 template <typename T, int D, bool DEVLEN>
 __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodeParams p) {
     constexpr int LPR = D / 8;     // lanes per cached row
@@ -60,13 +65,18 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int split = blockIdx.x, h = blockIdx.y, g = h / p.G;
+    const int64_t sh = int64_t(blockIdx.z) * gridDim.y + h;            // (sequence, head) index
+    const int64_t sg = int64_t(blockIdx.z) * (gridDim.y / p.G) + g;    // (sequence, kv head) index
     const int sub = lane / LPR, piece = lane % LPR;
-    uint16_t* kc = p.k_cache + int64_t(h) * p.cache_sh;
-    uint16_t* vc = p.v_cache + int64_t(h) * p.cache_sh;
+    uint16_t* kc = p.k_cache + int64_t(blockIdx.z) * p.cache_sb + int64_t(h) * p.cache_sh;
+    uint16_t* vc = p.v_cache + int64_t(blockIdx.z) * p.cache_sb + int64_t(h) * p.cache_sh;
+    const uint16_t* k_new = p.k_new + sg * D;
+    const uint16_t* v_new = p.v_new + sg * D;
     int64_t rows = p.T, chunk = p.chunk;
     if constexpr (DEVLEN) {
         if (p.step_dev) rows += int64_t(__ldg(p.step_dev));
-        if (p.head_rows) rows += int64_t(__ldg(p.head_rows + blockIdx.y));
+        if (p.rows) rows += int64_t(__ldg(p.rows + sh));
+        if (rows < 1 || rows > p.max_rows) rows = 0;
         const int64_t ns = min(int64_t(p.nsplit), splits_for(gridDim.y, rows, p.num_sms));
         chunk = (rows + ns - 1) / ns;
     }
@@ -77,12 +87,12 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
 
     // fused append: the CTA that owns the last row stores the new token's K/V (this head's copy)
     if (has_new && new_row >= r_begin && new_row < r_end && warp == 0 && lane < LPR) {
-        *reinterpret_cast<uint4*>(kc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(p.k_new + int64_t(g) * D + lane * 8);
-        *reinterpret_cast<uint4*>(vc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(p.v_new + int64_t(g) * D + lane * 8);
+        *reinterpret_cast<uint4*>(kc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(k_new + lane * 8);
+        *reinterpret_cast<uint4*>(vc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(v_new + lane * 8);
     }
 
     float qf[8];
-    unpack8<T>(*reinterpret_cast<const uint4*>(p.q + int64_t(h) * D + piece * 8), qf);
+    unpack8<T>(*reinterpret_cast<const uint4*>(p.q + sh * D + piece * 8), qf);
 
     float m = -INFINITY, l = 0.f, acc[8];
 #pragma unroll
@@ -100,8 +110,8 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
             ok[u] = r < r_end;
             if (ok[u]) {
                 const bool is_new = has_new && r == new_row;   // read the appended row from its source
-                const uint16_t* kr = is_new ? p.k_new + int64_t(g) * D : kc + r * D;
-                const uint16_t* vr = is_new ? p.v_new + int64_t(g) * D : vc + r * D;
+                const uint16_t* kr = is_new ? k_new : kc + r * D;
+                const uint16_t* vr = is_new ? v_new : vc + r * D;
                 kv[u] = *reinterpret_cast<const uint4*>(kr + piece * 8);
                 vv[u] = *reinterpret_cast<const uint4*>(vr + piece * 8);
             }
@@ -161,9 +171,9 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
             at += s_acc[w][tid] * c;
         }
         if (p.nsplit == 1) {
-            p.out[int64_t(h) * D + tid] = DT<T>::from_f32(at / lt);
+            p.out[sh * D + tid] = DT<T>::from_f32(at / lt);
         } else {
-            float* w = p.ws + (int64_t(h) * p.nsplit + split) * (2 + D);
+            float* w = p.ws + (sh * p.nsplit + split) * (2 + D);
             if (tid == 0) { w[0] = mn; w[1] = lt; }
             w[2 + tid] = at;
         }
@@ -171,8 +181,9 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
 }
 
 template <typename T, int D>
-__global__ void decode_combine_kernel(const DecodeParams p) {
-    const int h = blockIdx.x, d = threadIdx.x;
+__global__ void decode_combine_kernel(const DecodeParams p) {   // one CTA per (sequence, head)
+    const int64_t h = blockIdx.x;
+    const int d = threadIdx.x;
     const float* w = p.ws + int64_t(h) * p.nsplit * (2 + D);
     float mn = -INFINITY;
     for (int s = 0; s < p.nsplit; ++s) mn = fmaxf(mn, w[s * (2 + D)]);
@@ -183,7 +194,7 @@ __global__ void decode_combine_kernel(const DecodeParams p) {
         lt += w[s * (2 + D) + 1] * c;
         at += w[s * (2 + D) + 2 + d] * c;
     }
-    p.out[int64_t(h) * D + d] = DT<T>::from_f32(at / lt);
+    p.out[h * D + d] = DT<T>::from_f32(at / lt);
 }
 
 template <int D>
@@ -202,24 +213,25 @@ DecodeParams make_params(const DecodeArgs& a) {
     DecodeParams p;
     p.q = a.q; p.k_new = a.k_new; p.v_new = a.v_new;
     p.k_cache = a.k_cache; p.v_cache = a.v_cache; p.out = a.out;
-    p.cache_sh = a.cache_sh; p.T = a.T;
+    p.cache_sh = a.cache_sh; p.cache_sb = a.cache_sb; p.T = a.T; p.max_rows = a.max_rows;
     p.G = a.G; p.nsplit = a.nsplit; p.num_sms = a.num_sms;
     p.chunk = (a.T + a.nsplit - 1) / a.nsplit;
     p.scale = a.scale;
     p.ws = a.ws;
     p.step_dev = a.step_dev;
-    p.head_rows = a.head_rows;
+    p.rows = a.rows;
     return p;
 }
 
 template <typename T, int D>
 cudaError_t launch_decode_t(const DecodeArgs& a, cudaStream_t st) {
     const DecodeParams p = make_params(a);
-    if (a.step_dev || a.head_rows) decode_kernel<T, D, true><<<dim3(unsigned(a.nsplit), unsigned(a.Hq)), kDecodeThreads, 0, st>>>(p);
-    else decode_kernel<T, D, false><<<dim3(unsigned(a.nsplit), unsigned(a.Hq)), kDecodeThreads, 0, st>>>(p);
+    const dim3 grid(unsigned(a.nsplit), unsigned(a.Hq), unsigned(a.num_seqs));
+    if (a.devlen) decode_kernel<T, D, true><<<grid, kDecodeThreads, 0, st>>>(p);
+    else decode_kernel<T, D, false><<<grid, kDecodeThreads, 0, st>>>(p);
     count_launch();
     if (a.nsplit > 1) {
-        decode_combine_kernel<T, D><<<unsigned(a.Hq), D, 0, st>>>(p);
+        decode_combine_kernel<T, D><<<unsigned(int64_t(a.num_seqs) * a.Hq), D, 0, st>>>(p);
         count_launch();
     }
     return cudaGetLastError();

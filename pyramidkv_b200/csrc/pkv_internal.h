@@ -107,12 +107,16 @@ struct DecodeArgs {
     const uint16_t *q, *k_new, *v_new;
     uint16_t *k_cache, *v_cache, *out;
     int64_t cache_sh;
+    int64_t cache_sb = 0;   // elements between the caches of consecutive sequences
+    int num_seqs = 1;
+    int64_t max_rows = 0;   // devlen: row counts outside [1, max_rows] are not attended (NaN output, nothing written)
+    bool devlen = false;    // row counts are read on the device (graph-replayable form): T (+ *step_dev) (+ rows[s*Hq + h])
     float* ws;
     float scale;
     int nsplit;
     int num_sms;
-    const int32_t* step_dev = nullptr;  // pkv_decode_attn_graph: device step counter added to T inside the kernel
-    const int32_t* head_rows = nullptr; // pkv_decode_attn_ragged: per-head row counts added to T inside the kernel
+    const int32_t* step_dev = nullptr;  // device step counter added to T inside the kernel
+    const int32_t* rows = nullptr;      // [num_seqs*Hq] per (sequence, head) row counts added to T inside the kernel
 };
 int decode_num_splits(int Hq, int64_t T, int num_sms);
 cudaError_t launch_decode(const DecodeArgs& a, cudaStream_t st);

@@ -65,6 +65,10 @@ class CudaBackend:
                     max_length=0, workspace=None, head_rows=None):
         return ops.decode_attn(q, k_cache, v_cache, length, k_new, v_new, out, softmax_scale, step, max_length, workspace, head_rows)
 
+    def decode_attn_batch(self, q, k_buf, v_buf, length, k_new, v_new, rows=None, step=None, max_length=0, workspace=None,
+                          out=None, softmax_scale=0.0):
+        return ops.decode_attn_batch(q, k_buf, v_buf, length, k_new, v_new, rows, step, max_length, workspace, out, softmax_scale)
+
     def rope_inplace(self, q, k, cos, sin):
         ops.rope_inplace(q, k, cos, sin)
 

@@ -398,6 +398,73 @@ def decode_attn(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, l
     return out
 
 
+def decode_attn_batch(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor, length: int,
+                      k_new: Optional[torch.Tensor] = None, v_new: Optional[torch.Tensor] = None,
+                      rows: Optional[torch.Tensor] = None, step: Optional[torch.Tensor] = None, max_length: int = 0,
+                      workspace: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                      softmax_scale: float = 0.0) -> torch.Tensor:
+    """The decode step of B sequences in ONE launch (`pkv_decode_attn_batch`). q [B, Hq, D] (e.g. HF's
+    `query_states[:, :, 0, :]`); buffers [B, Hq, capacity, D]; k_new / v_new [B, Hkv, D] appended as each sequence's last
+    row. Sequence b, head h attends `length` (+ `*step`) (+ `rows[b*Hq + h]`) rows: `rows` is an int32 device tensor
+    [B*Hq] (or [B, Hq]) or None (every sequence holds `length` rows). The launch is sized for `max_length` rows (default:
+    the capacity) and is graph-replayable; every sequence's output and appended row are bit-identical to `decode_attn` in
+    the graph form (or the ragged form, for per-head rows) on that sequence alone. Returns out [B, Hq, D]."""
+    _require_cuda(q, k_buf, v_buf, k_new, v_new, rows, step, workspace, out)
+    if k_buf.dim() != 4 or k_buf.shape != v_buf.shape or k_buf.stride() != v_buf.stride():
+        raise ValueError("k_buf / v_buf must be [B, Hq, capacity, D] tensors of equal shape and strides")
+    B, Hq, cap, D = k_buf.shape
+    if k_buf.stride(3) != 1 or k_buf.stride(2) != D:
+        raise ValueError("k_buf / v_buf: every head's rows must be contiguous [capacity, D]")
+    if q.shape != (B, Hq, D):
+        raise ValueError(f"q must be [B, Hq, D] = {(B, Hq, D)}, got {tuple(q.shape)}")
+    if not q.is_contiguous():
+        q = q.contiguous()
+    if out is None:
+        out = torch.empty(B, Hq, D, dtype=q.dtype, device=q.device)
+    elif out.shape != (B, Hq, D) or not out.is_contiguous() or out.dtype != q.dtype:
+        raise ValueError("out must be a contiguous [B, Hq, D] tensor of q's dtype")
+    max_length = int(max_length) or cap
+    if not 1 <= length <= max_length <= cap:
+        raise ValueError(f"cache capacity {cap} exceeded or bad row counts (length {length}, max_length {max_length})")
+    if step is not None and (step.dtype != torch.int32 or step.numel() != 1):
+        raise ValueError("step must be an int32 device tensor with one element")
+    if rows is not None:
+        if rows.dtype != torch.int32 or rows.numel() != B * Hq or not rows.is_contiguous():
+            raise ValueError(f"rows must be a contiguous int32 device tensor of B*Hq = {B * Hq} elements")
+        if not torch.cuda.is_current_stream_capturing():
+            # (one device read; a captured launch relies on the caller, and the kernel reads and writes no row of a
+            # (sequence, head) whose count exceeds max_length)
+            most = int(rows.max()) + int(length) + (int(step) if step is not None else 0)
+            if most > max_length:
+                raise ValueError(f"cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
+    d = DecodeDesc()
+    d.struct_bytes = C.sizeof(DecodeDesc)
+    d.dtype, d.num_q_heads, d.head_dim = _dtype_code(q), Hq, D
+    d.device = q.device.index if q.device.index is not None else torch.cuda.current_device()
+    d.length = int(length)
+    d.q, d.k_cache, d.v_cache, d.cache_stride_h, d.out = q.data_ptr(), k_buf.data_ptr(), v_buf.data_ptr(), k_buf.stride(1), out.data_ptr()
+    keep = [q, out]
+    if k_new is not None:
+        if k_new.dim() != 3 or k_new.shape[0] != B or k_new.shape[2] != D or v_new is None or v_new.shape != k_new.shape:
+            raise ValueError("k_new / v_new must be [B, Hkv, D]")
+        k_new, v_new = k_new.contiguous(), v_new.contiguous()
+        d.num_kv_heads = k_new.shape[1]
+        d.k_new, d.v_new = k_new.data_ptr(), v_new.data_ptr()
+        keep += [k_new, v_new]
+    else:
+        d.num_kv_heads = Hq
+    d.num_q_heads = B * Hq                 # workspace query: one set of split partials per (sequence, head)
+    nbytes = int(_lib.lib().pkv_decode_workspace_bytes(C.byref(d)))
+    d.num_q_heads = Hq
+    ws = workspace if workspace is not None else _workspace(q.device, nbytes)
+    d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel() * ws.element_size()
+    d.softmax_scale = float(softmax_scale)
+    _lib.check(_lib.lib().pkv_decode_attn_batch(C.byref(d), B, k_buf.stride(0), rows.data_ptr() if rows is not None else None,
+                                                step.data_ptr() if step is not None else None, max_length,
+                                                torch.cuda.current_stream(q.device).cuda_stream))
+    return out
+
+
 def decode_workspace_bytes(num_q_heads: int, head_dim: int) -> int:
     """Upper bound of the decode workspace for any cache length (`pkv_decode_workspace_bytes`)."""
     d = DecodeDesc()

@@ -211,6 +211,48 @@ def _run_prompt_static(model, ids: torch.Tensor, max_new_tokens: int, use_graph:
                         [rows[0], rows[-1]] if rows else [], torch.cat(toks, dim=1)[0].tolist())
 
 
+def _run_batch_static(model, prompts: List[torch.Tensor], max_new_tokens: int, use_graph: Optional[bool]):
+    """Several prompts through greedy_generate_batch's flow: each prefilled alone (timed alone, after an untimed warm-up at
+    its length), the caches joined, then one static decode of all of them. Returns (one PromptResult per prompt, the
+    batch's aggregate decode tok/s = sequences * steps / decode time)."""
+    from .cache import join_caches
+    from .generate import StaticDecoder, _prefill
+    dev = prompts[0].device
+    firsts, caches, prefill_ms = [], [], []
+    with torch.no_grad():
+        for ids in prompts:
+            _prefill(model, ids)
+            _sync(dev)
+            t0 = time.perf_counter()
+            f, c = _prefill(model, ids)
+            _sync(dev)
+            prefill_ms.append((time.perf_counter() - t0) * 1e3)
+            firsts.append(f)
+            caches.append(c)
+        first = torch.cat(firsts)
+        cache = join_caches(caches, reserve=max(0, max_new_tokens - 1))
+        del caches
+        gen, decode_s = torch.empty(len(prompts), 0, dtype=torch.long, device=dev), 0.0
+        if max_new_tokens > 1:
+            dec = StaticDecoder(model, cache, first, max_new_tokens - 1, use_graph=use_graph)
+            if dec.use_graph:
+                dec._capture()                       # graph capture is a one-off cost per batch shape, not decode time
+            _sync(dev)
+            t0 = time.perf_counter()
+            gen = dec.run(max_new_tokens - 1).clone()
+            _sync(dev)
+            decode_s = time.perf_counter() - t0
+            dec.finish()
+    steps = max_new_tokens - 1
+    per_seq = steps / max(decode_s, 1e-9) if steps > 0 else 0.0
+    res = []
+    for b, ids in enumerate(prompts):
+        rows = [max(l.rows_host[b]) for l in cache.layers]
+        res.append(PromptResult(int(ids.shape[1]), max_new_tokens, prefill_ms[b], per_seq, [rows[0], rows[-1]],
+                                torch.cat([first[b], gen[b]]).tolist()))
+    return res, per_seq * len(prompts)
+
+
 def run_prompt(model, ids: torch.Tensor, max_new_tokens: int, decode_loop: str = "hf") -> PromptResult:
     """Greedy generate exactly as the reference runner does. One untimed warm-up call at this prompt length (allocator,
     cuBLAS heuristics, lazy module init), then two timed calls: one new token (prefill + eviction of all layers) and the
@@ -250,8 +292,17 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
               dtype: torch.dtype = torch.float16, attn_implementation: str = "sdpa", merge=None, seed: int = 42,
               backend_factory: Optional[Callable] = None, out_path: Optional[str] = None, tag: Optional[dict] = None,
               decode_loop: str = "hf", floor: float = 0.2, head_beta: float = 1.01, head_path: str = "",
-              capacity_ratio: float = -1) -> List[dict]:
-    """prompts: iterable of (name, prompt_tokens, max_new_tokens). One JSON record per prompt (also appended to out_path)."""
+              capacity_ratio: float = -1, eval_batch_size: int = 1) -> List[dict]:
+    """prompts: iterable of (name, prompt_tokens, max_new_tokens). One JSON record per prompt (also appended to out_path).
+    eval_batch_size N > 1: consecutive prompts with the same max_new_tokens are decoded N at a time (static loops only;
+    each prompt is still prefilled alone, so its prefill_ms, cache rows and tokens are its own)."""
+    if eval_batch_size < 1:
+        raise ValueError(f"eval_batch_size must be >= 1, got {eval_batch_size}")
+    if eval_batch_size > 1 and (decode_loop == "hf" or canonical_method(method) == "fullkv"):
+        raise NotImplementedError("eval_batch_size > 1 decodes the joined compacted caches of the prompts with the static loop: "
+                                  "use --decode_loop static or static-eager with an eviction method (padded HF batches are not supported)")
+    if decode_loop not in ("hf", "static", "static-eager"):
+        raise ValueError(f"decode_loop must be hf, static or static-eager, got {decode_loop!r}")
     if device is None:
         if not torch.cuda.is_available():
             raise RuntimeError("the runners need a CUDA device (H100, sm_90a); there is no CPU fallback")
@@ -266,25 +317,39 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
         elif method != "fullkv" and capacity_ratio == -1:
             raise ValueError("either max_capacity_prompts or max_capacity_prompts_ratio must be given")
         records = []
-        for i, (name, length, new) in enumerate(prompts):
+        prompts = list(prompts)
+        if eval_batch_size > 1 and max_capacity_prompt == -1 and capacity_ratio != -1 and len({p[1] for p in prompts}) > 1:
+            raise NotImplementedError("--max_capacity_prompts_ratio sets a budget per prompt length; batch prompts of one length")
+        i = 0
+        while i < len(prompts):
+            group = [i]                                   # consecutive prompts decoded together: same max_new_tokens
+            while len(group) < eval_batch_size and group[-1] + 1 < len(prompts) and prompts[group[-1] + 1][2] == prompts[i][2]:
+                group.append(group[-1] + 1)
             if method != "fullkv" and max_capacity_prompt == -1 and capacity_ratio != -1:
                 # run_longbench.py:213-216: with --max_capacity_prompts -1 the budget is a fraction of EACH prompt's length
-                cap_i = round(length * capacity_ratio)
+                cap_i = round(prompts[i][1] * capacity_ratio)
                 window = set_knobs(model, method, cap_i, merge, backend_factory, floor, head_beta, head_path)
-            ids = synthetic_prompt(model.config.vocab_size, length, seed + i, device)
-            r = run_prompt(model, ids, new, decode_loop if method != "fullkv" else "hf")
-            rec = {"task": name, "arch": arch, "method": method,
-                   "max_capacity_prompt": model.config.max_capacity_prompt if method != "fullkv" else max_capacity_prompt, "window": window,
-                   "decode_loop": decode_loop if method != "fullkv" else "hf",
-                   "dtype": str(dtype).replace("torch.", ""), "data": "synthetic token ids, random-init weights", **(tag or {}),
-                   "prompt_tokens": r.prompt_tokens, "new_tokens": r.new_tokens, "prefill_ms": r.prefill_ms,
-                   "decode_tok_per_s": r.decode_tok_per_s, "cache_rows_first_last": r.cache_rows_first_last, "pred_ids": r.pred_ids}
-            records.append(rec)
-            print(json.dumps({k: v for k, v in rec.items() if k != "pred_ids"}), flush=True)
-            if out_path:
-                os.makedirs(os.path.dirname(os.path.abspath(out_path)), exist_ok=True)
-                with open(out_path, "a") as f:
-                    f.write(json.dumps(rec) + "\n")
+            ids = [synthetic_prompt(model.config.vocab_size, prompts[j][1], seed + j, device) for j in group]
+            batch = {}
+            if eval_batch_size > 1:
+                rs, agg = _run_batch_static(model, ids, prompts[i][2], None if decode_loop == "static" else False)
+                batch = {"eval_batch_size": eval_batch_size, "batch_size": len(group), "batch_decode_tok_per_s_aggregate": agg}
+            else:
+                rs = [run_prompt(model, ids[0], prompts[i][2], decode_loop if method != "fullkv" else "hf")]
+            for j, r in zip(group, rs):
+                rec = {"task": prompts[j][0], "arch": arch, "method": method,
+                       "max_capacity_prompt": model.config.max_capacity_prompt if method != "fullkv" else max_capacity_prompt, "window": window,
+                       "decode_loop": decode_loop if method != "fullkv" else "hf",
+                       "dtype": str(dtype).replace("torch.", ""), "data": "synthetic token ids, random-init weights", **(tag or {}),
+                       "prompt_tokens": r.prompt_tokens, "new_tokens": r.new_tokens, "prefill_ms": r.prefill_ms,
+                       "decode_tok_per_s": r.decode_tok_per_s, **batch, "cache_rows_first_last": r.cache_rows_first_last, "pred_ids": r.pred_ids}
+                records.append(rec)
+                print(json.dumps({k: v for k, v in rec.items() if k != "pred_ids"}), flush=True)
+                if out_path:
+                    os.makedirs(os.path.dirname(os.path.abspath(out_path)), exist_ok=True)
+                    with open(out_path, "a") as f:
+                        f.write(json.dumps(rec) + "\n")
+            i = group[-1] + 1
         return records
     finally:
         from pyramidkv.monkeypatch import restore

@@ -33,7 +33,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--max_num_examples", type=int, default=2)
     p.add_argument("--sample_method", type=str, default="topk", choices=["random", "topk"])
     p.add_argument("--max_new_tokens", type=int, default=None)
-    p.add_argument("--eval_batch_size", type=int, default=1)
+    p.add_argument("--eval_batch_size", type=int, default=1,
+                   help="N > 1 (static decode loops): prompts are prefilled one at a time and decoded N at a time")
     p.add_argument("--use_cache", type=bool, default=True)
     p.add_argument("--attn_implementation", type=str, default="flash_attention_2", choices=["flash_attention_2", "sdpa", "eager"])
     p.add_argument("--method", type=str, default=None)
@@ -63,8 +64,9 @@ def main(argv=None, backend_factory=None, device=None):
         raise SystemExit("--method is required (FullKV, PyramidKV, SnapKV, H2O, StreamingLLM)")
     if args.quant_method is not None:
         raise NotImplementedError("quantised caches (--quant_method) are outside the eviction hot path built here")
-    if args.eval_batch_size != 1:
-        raise NotImplementedError("the reference path is batch size 1 (README: batch inference unsupported)")
+    if args.eval_batch_size != 1 and args.decode_loop == "hf":
+        raise NotImplementedError("--eval_batch_size > 1 needs --decode_loop static or static-eager (the prompts are prefilled one at "
+                                  "a time and their compacted caches decoded together); padded HF batches are not supported")
     method = runner.canonical_method(args.method)
     arch = runner.resolve_arch(args.model_path, args.model_name)
     tasks = sorted(runner.LONGBENCH_SHAPES) if args.dataset in ("all", "") else [args.dataset]
@@ -85,7 +87,7 @@ def main(argv=None, backend_factory=None, device=None):
                             attn_implementation=args.attn_implementation, merge=args.merge, seed=args.seed,
                             backend_factory=backend_factory, out_path=out, decode_loop=args.decode_loop,
                             floor=args.floor, head_beta=args.head_beta, head_path=args.head_path,
-                            capacity_ratio=args.max_capacity_prompts_ratio)
+                            capacity_ratio=args.max_capacity_prompts_ratio, eval_batch_size=args.eval_batch_size)
     n = len(recs)
     print(json.dumps({"summary": True, "arch": arch, "method": method, "max_capacity_prompts": capacity, "examples": n,
                       "mean_prefill_ms": sum(r["prefill_ms"] for r in recs) / n,
