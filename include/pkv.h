@@ -248,6 +248,37 @@ int pkv_decode_attn_graph(const pkv_decode_desc* d, const int32_t* step_dev, int
  * above the capacity, misaligned rows / step_dev. */
 int pkv_decode_attn_batch(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
                           const int32_t* step_dev, int64_t max_length, void* stream);
+/* The opt-in FP8 compacted cache. K and V are stored as E4M3 bytes ([num_seqs, num_q_heads, capacity, head_dim], one byte
+ * per element) with one fp32 scale per (sequence, head, row) for each: [num_seqs, num_q_heads, capacity]. A 16-bit row x
+ * is stored as amax = max|x_e| (fp32); amax == 0: scale 0 and every byte 0; otherwise inv = rn_f32(448 / amax),
+ * q_e = E4M3(rn_f32(x_e * inv)) rounded to nearest even and saturated to +-448 (cvt.rn.satfinite.e4m3x2.f32), scale =
+ * rn_f32(amax / 448). Row e stands for float(q_e) * scale. (The reference's --quant_method caches are HQQ-based and are
+ * not built here.)
+ *
+ * pkv_decode_attn_batch_fp8 = pkv_decode_attn_batch over such a cache, with the same row count rule, split rule,
+ * out-of-range behaviour (NaN output, nothing read or written), workspace (pkv_decode_workspace_bytes with num_q_heads =
+ * num_seqs*num_q_heads) and graph replayability: every sequence's output and appended row are bit-identical to a
+ * num_seqs = 1 launch on that sequence alone. It is the only FP8 decode entry point: a single sequence (host-launched or
+ * in a graph) is num_seqs = 1, with step_dev = NULL and rows = NULL for a host launch of `length` rows. d->dtype is the
+ * dtype of q, k_new, v_new and out; d->k_cache / d->v_cache point at the E4M3 bytes and cache_stride_h counts bytes
+ * (a multiple of 16, >= max_length*head_dim; cache_stride_b likewise). Sequence s, head h reads its scales at
+ * k_scale / v_scale + s*scale_stride_b + h*scale_stride_h (floats; scale_stride_h >= max_length). The CTA that owns the
+ * last row quantises k_new[s][h / group] / v_new[s][h / group] with the rule above, stores its bytes and scale, and attends
+ * that quantised row: the output is the attention (fp32 online softmax, as pkv_decode_attn) over exactly the rows the
+ * cache holds. PKV_ERR_INVALID_ARG additionally for null or misaligned scale pointers and too small scale strides. */
+int pkv_decode_attn_batch_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
+                              const int32_t* step_dev, int64_t max_length, float* k_scale, float* v_scale, int64_t scale_stride_h,
+                              int64_t scale_stride_b, void* stream);
+/* Conversion of the compacted 16-bit caches of num_layers layers (one prompt, or one equal-length batch of num_seqs
+ * sequences) to the FP8 format above, in one launch per 32 layers; the per-layer tables travel as kernel parameters.
+ * Layer l: src[2l] / src[2l+1] = K / V, 16-bit contiguous [num_seqs, num_heads, src_capacity[l], head_dim]; dst[2l] /
+ * dst[2l+1] = E4M3 [num_seqs, num_heads, dst_capacity[l], head_dim]; scales[2l] / scales[2l+1] = fp32 [num_seqs,
+ * num_heads, dst_capacity[l]]. Every (sequence, head) converts rows[l] rows, or, when rows_dev != NULL and rows_dev[l] !=
+ * NULL, the DEVICE int32 count rows_dev[l][s*num_heads + h] (AdaKV / HeadKV heads), which must not exceed rows[l]. Rows
+ * past the count are neither read nor written. Pointers to 16-bit / E4M3 data are 16-byte aligned. */
+int pkv_cache_quantize_fp8(int32_t dtype, int32_t num_seqs, int32_t num_heads, int32_t head_dim, int32_t device, int32_t num_layers,
+                           const void* const* src, void* const* dst, float* const* scales, const int64_t* src_capacity,
+                           const int64_t* dst_capacity, const int64_t* rows, const int32_t* const* rows_dev, void* stream);
 /* Append only (no attention): writes k_new/v_new as row length-1. */
 int pkv_cache_append(const pkv_decode_desc* d, void* stream);
 

@@ -21,6 +21,7 @@ EXPORTS = [
     "pkv_stage_gather", "pkv_decode_workspace_bytes", "pkv_decode_attn", "pkv_decode_attn_graph", "pkv_cache_append", "pkv_host_pick_rows", "pkv_debug_read_stamps", "pkv_rope_inplace", "pkv_update_flatten_view", "pkv_adakv_scratch_bytes", "pkv_adakv_counts",
     "pkv_ragged_place_window", "pkv_decode_attn_ragged", "pkv_evict_single_launch", "pkv_stage_scan_pool",
     "pkv_evict_prefill_batch", "pkv_evict_batch_supported", "pkv_stage_batch", "pkv_decode_attn_batch",
+    "pkv_decode_attn_batch_fp8", "pkv_cache_quantize_fp8",
 ]
 
 
@@ -135,6 +136,11 @@ def lib() -> C.CDLL:
     L.pkv_decode_attn_graph.restype = i32
     L.pkv_decode_attn_batch.argtypes = [C.POINTER(DecodeDesc), C.c_int32, i64, p, p, i64, p]
     L.pkv_decode_attn_batch.restype = i32
+    L.pkv_decode_attn_batch_fp8.argtypes = [C.POINTER(DecodeDesc), C.c_int32, i64, p, p, i64, p, p, i64, i64, p]
+    L.pkv_decode_attn_batch_fp8.restype = i32
+    # tables: src / dst / scales [2*layers] pointers, capacities and rows [layers] int64, rows_dev [layers] pointers or NULL
+    L.pkv_cache_quantize_fp8.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p, p, p, p, p, p, p, p]
+    L.pkv_cache_quantize_fp8.restype = i32
     if L.pkv_version() != 3:
         raise RuntimeError(f"libpkv ABI version {L.pkv_version()} != 3; rebuild with `python -m pyramidkv_b200.build --force`")
     _lib = L

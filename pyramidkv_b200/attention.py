@@ -22,7 +22,8 @@ from typing import Callable, Optional
 import torch
 from transformers.modeling_utils import ALL_ATTENTION_FUNCTIONS
 
-from .cache import PkvBatchCacheLayer, PkvCacheLayer, PkvRaggedCacheLayer, install_layer, layer_is_empty
+from .cache import (PkvBatchCacheLayer, PkvCacheLayer, PkvFp8CacheLayer, PkvRaggedCacheLayer, install_layer, kv_cache_dtype,
+                    layer_is_empty, quantize_caches_fp8)
 from .kv_cluster import INIT_BY_METHOD, flush_pending
 
 DEFAULT_DECODE_RESERVE = 256   # rows of head-room behind the compacted prompt (grows by doubling)
@@ -54,6 +55,17 @@ def _has_padding(attention_mask) -> bool:
         return False
     row = attention_mask[:, 0, -1, :]
     return bool((~row).any()) if row.dtype == torch.bool else bool((row < 0).any())
+
+
+def _maybe_quantize(module, past_key_values, cluster) -> None:
+    """Knob pkv_kv_cache_dtype = "fp8_e4m3": once the LAST layer's prefill has filled its cache (and the parked evictions
+    are flushed), every layer's compacted cache becomes a PkvFp8CacheLayer in one launch. The conversion runs after the
+    eviction, so it covers every compacting method."""
+    if kv_cache_dtype(module.config) is None or module.layer_idx != last_layer_idx(module):
+        return
+    if getattr(past_key_values, "_pkv_pending", None):
+        flush_pending(past_key_values._pkv_pending, cluster.backend)
+    quantize_caches_fp8(past_key_values, cluster.backend)
 
 
 def make_forward(method: str, modeling, original_forward):
@@ -105,6 +117,7 @@ def make_forward(method: str, modeling, original_forward):
                     raise NotImplementedError("AdaKV / HeadKV are batch size 1 (pyramidkv_utils.py:723)")
                 k_buf, v_buf, head_rows = cluster.evict_ragged(query_states[0], key_states[0], value_states[0], reserve=reserve)
                 install_layer(past_key_values, self.layer_idx, PkvRaggedCacheLayer(k_buf[None], v_buf[None], head_rows, seen_tokens=q_len))
+                _maybe_quantize(self, past_key_values, cluster)
                 attn_output = attn_output.reshape(*input_shape, -1).contiguous()
                 return self.o_proj(attn_output), attn_weights
             # Deferred eviction (knob pkv_defer_eviction, default on): a layer's eviction reads only this layer's q / k / v and
@@ -125,6 +138,7 @@ def make_forward(method: str, modeling, original_forward):
             else:
                 k_buf, v_buf = torch.stack([t[0] for t in bufs]), torch.stack([t[1] for t in bufs])
             install_layer(past_key_values, self.layer_idx, PkvCacheLayer(k_buf, v_buf, rows, seen_tokens=q_len))
+            _maybe_quantize(self, past_key_values, cluster)
         else:
             # ---------------- decode (llama_model.py:169-170) ----------------
             if getattr(past_key_values, "_pkv_pending", None):      # a prefill that stopped before its last layer (never with generate())
@@ -141,7 +155,21 @@ def make_forward(method: str, modeling, original_forward):
             # rows = `rows_arg` (+ head_rows[h] for ragged caches, + the device step counter in static mode)
             rows_arg = (layer.appended if ragged else layer.length) + 1
             head_rows = {"head_rows": layer.head_rows} if ragged else {}
-            if q_len == 1 and (bsz > 1 or joined):
+            if q_len == 1 and isinstance(layer, PkvFp8CacheLayer):
+                # FP8 cache (knob pkv_kv_cache_dtype): one launch for any batch size, host-launched or in the static loop's
+                # graph; rows = layer.rows[b, h] + 1 (+ the device step counter in static mode). The kernel quantises the new
+                # K / V row and attends it as stored.
+                if static is None:
+                    layer.reserve(1)
+                out = cluster.backend.decode_attn_batch_fp8(
+                    query_states[:, :, 0, :], layer.k_buf, layer.v_buf, layer.k_scale, layer.v_scale, 1,
+                    key_states[:, :, 0, :], value_states[:, :, 0, :], rows=layer.rows,
+                    step=static.step if static is not None else None, max_length=layer.capacity,
+                    workspace=static.workspace if static is not None else None, softmax_scale=self.scaling)
+                if static is None:
+                    layer.advance(1)
+                attn_output = out[:, None]
+            elif q_len == 1 and (bsz > 1 or joined):
                 # several sequences: ONE launch for the batch. Rows = layer.length + 1 (equal-length batched prefill) or
                 # layer.rows[b, h] + 1 (joined prompts), + the device step counter in static mode
                 if static is None:

@@ -183,14 +183,143 @@ class PkvBatchCacheLayer(PkvCacheLayer):
         raise NotImplementedError("a joined batch holds one row count per sequence and head; join the selected prompts instead")
 
 
+KV_CACHE_DTYPES = (None, "fp8_e4m3")   # model.config.pkv_kv_cache_dtype
+
+
+def kv_cache_dtype(config) -> Optional[str]:
+    """The knob `pkv_kv_cache_dtype` of a model config: None (the default: the 16-bit cache) or "fp8_e4m3"."""
+    v = getattr(config, "pkv_kv_cache_dtype", None)
+    v = None if v == "auto" else v
+    if v not in KV_CACHE_DTYPES:
+        raise ValueError(f"pkv_kv_cache_dtype={v!r}: expected None or 'fp8_e4m3'")
+    return v
+
+
+class PkvFp8CacheLayer(PkvBatchCacheLayer):
+    """The compacted cache in FP8 (knob `pkv_kv_cache_dtype = "fp8_e4m3"`): `k_buf` / `v_buf` hold E4M3 bytes
+    (torch.float8_e4m3fn [B, Hq, capacity, D]) and `k_scale` / `v_scale` one fp32 scale per (sequence, head, row)
+    ([B, Hq, capacity]); row x of the 16-bit cache is stored as round(x * 448 / max|x|) and stands for its bytes times
+    the scale max|x| / 448 (include/pkv.h, pkv_cache_quantize_fp8). Half the bytes of the 16-bit cache plus 8 bytes per
+    row and head. Always in the per-(sequence, head) row-count form of `PkvBatchCacheLayer`, so one class holds a single
+    prompt, an equal-length batch, AdaKV / HeadKV heads of different lengths and joined prompts. Decode appends one
+    quantised row per sequence and step (`pkv_decode_attn_batch_fp8`)."""
+
+    def __init__(self, k_q: torch.Tensor, v_q: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor, rows_host, seq_seen):
+        assert k_q.dtype == torch.float8_e4m3fn and k_scale.shape == k_q.shape[:3] and v_scale.shape == k_scale.shape
+        self.k_scale, self.v_scale = k_scale, v_scale
+        super().__init__(k_q, v_q, rows_host, seq_seen)
+
+    def reserve(self, extra_rows: int) -> None:
+        need = self.length + extra_rows
+        if need <= self.capacity:
+            return
+        new_cap = max(need, self.capacity + max(64, self.capacity // 2))
+        b, h, _, d = self.k_buf.shape
+        n = self.length
+        bufs = []
+        for t in (self.k_buf, self.v_buf, self.k_scale, self.v_scale):
+            nt = torch.empty((b, h, new_cap) + tuple(t.shape[3:]), dtype=t.dtype, device=t.device)
+            nt[:, :, :n] = t[:, :, :n]
+            bufs.append(nt)
+        self.k_buf, self.v_buf, self.k_scale, self.v_scale = bufs
+        self._refresh_views()
+
+    @staticmethod
+    def dequantize(q: torch.Tensor, scale: torch.Tensor) -> torch.Tensor:
+        """float32 rows: bytes times the row scale."""
+        return q.float() * scale[..., None]
+
+    def head_view(self, b: int, h: int):
+        """Dequantised valid rows of sequence b, head h: ([rows, D] float32 keys, values)."""
+        r = self.rows_host[b][h]
+        return (self.dequantize(self.k_buf[b, h, :r], self.k_scale[b, h, :r]),
+                self.dequantize(self.v_buf[b, h, :r], self.v_scale[b, h, :r]))
+
+    def update(self, key_states, value_states, *args, **kwargs):
+        raise NotImplementedError("multi-token append to an FP8 cache is not built: decode it one token per step (the FP8 "
+                                  "cache covers the decode path; prefill and the multi-token path stay 16-bit)")
+
+    def crop(self, max_length: int) -> None:
+        raise NotImplementedError("cropping a compacted cache is undefined (rows are in score order, not position order)")
+
+    def batch_repeat_interleave(self, repeats: int) -> None:
+        raise NotImplementedError("an FP8 cache holds one row count per sequence and head (beam search over FP8 caches is "
+                                  "not built); repeat the prompts before joining")
+
+    def batch_select_indices(self, indices: torch.Tensor) -> None:
+        raise NotImplementedError("an FP8 cache holds one row count per sequence and head; join the selected prompts instead")
+
+
+def quantize_caches_fp8(past_key_values, backend) -> int:
+    """Convert every compacted layer of `past_key_values` (`PkvCacheLayer` / `PkvRaggedCacheLayer`, filled by the patched
+    prefill) to a `PkvFp8CacheLayer` with ONE backend call (`pkv_cache_quantize_fp8`: one launch per 32 layers) and drop
+    the 16-bit buffers. The FP8 buffers keep each layer's capacity (the decode head-room included). Returns the number of
+    layers converted."""
+    idx, items, metas = [], [], []
+    for i, l in enumerate(past_key_values.layers):
+        if not isinstance(l, PkvCacheLayer) or isinstance(l, PkvBatchCacheLayer):
+            continue
+        B, Hq, cap, D = l.k_buf.shape
+        kq = torch.empty(B, Hq, cap, D, dtype=torch.float8_e4m3fn, device=l.device)
+        vq = torch.empty_like(kq)
+        ks = torch.empty(B, Hq, cap, dtype=torch.float32, device=l.device)
+        vs = torch.empty_like(ks)
+        if isinstance(l, PkvRaggedCacheLayer):
+            rows_host = [[r + l.appended for r in l.head_rows_host]] * B
+            rows_dev = l.head_rows + l.appended if l.appended else l.head_rows
+        else:
+            rows_host, rows_dev = [[l.length] * Hq] * B, None
+        items.append((l.k_buf, l.v_buf, kq, vq, ks, vs, l.length, rows_dev))
+        metas.append((kq, vq, ks, vs, rows_host, [l.seen_tokens] * B))
+        idx.append(i)
+    if items:
+        backend.cache_quantize_fp8(items)
+    for i, m in zip(idx, metas):
+        past_key_values.layers[i] = PkvFp8CacheLayer(*m)
+    return len(idx)
+
+
+def _join_fp8(caches, reserve: int):
+    from transformers import DynamicCache
+    out = DynamicCache()
+    out.layers = []
+    for i in range(len(caches[0].layers)):
+        src = [c.layers[i] for c in caches]
+        _, hq, _, d = src[0].k_buf.shape
+        if any(l.k_buf.shape[1] != hq or l.k_buf.shape[3] != d or l.device != src[0].device for l in src):
+            raise ValueError(f"join_caches: layer {i}: head counts, head_dim or device differ between the caches")
+        rows = [list(l.rows_host[0]) for l in src]
+        cap = max(max(r) for r in rows) + int(reserve)
+        k = torch.empty(len(src), hq, cap, d, dtype=torch.float8_e4m3fn, device=src[0].device)
+        v = torch.empty_like(k)
+        ks = torch.empty(len(src), hq, cap, dtype=torch.float32, device=src[0].device)
+        vs = torch.empty_like(ks)
+        for b, l in enumerate(src):
+            n = l.length
+            k[b, :, :n], v[b, :, :n] = l.k_buf[0, :, :n], l.v_buf[0, :, :n]
+            ks[b, :, :n], vs[b, :, :n] = l.k_scale[0, :, :n], l.v_scale[0, :, :n]
+        out.layers.append(PkvFp8CacheLayer(k, v, ks, vs, rows, [l.seq_seen[0] for l in src]))
+    return out
+
+
 def join_caches(caches, reserve: int = 0):
     """One batched cache from B single-prompt caches filled by the patched prefill (every layer a batch-1 `PkvCacheLayer` or
     `PkvRaggedCacheLayer`): layer by layer the valid rows are copied once into [B, Hq, longest + reserve, D] buffers
-    (`PkvBatchCacheLayer`). A cache may be passed several times. Stock / FullKV caches raise."""
+    (`PkvBatchCacheLayer`). A cache may be passed several times. Stock / FullKV caches raise. Single-prompt FP8 caches
+    (`PkvFp8CacheLayer`) join the same way, bytes and scales copied once, into a `PkvFp8CacheLayer`; FP8 and 16-bit
+    caches do not mix."""
     from transformers import DynamicCache
     if not caches:
         raise ValueError("join_caches: no caches")
     n_layers = len(caches[0].layers)
+    fp8 = [isinstance(l, PkvFp8CacheLayer) for c in caches for l in c.layers]
+    if any(fp8):
+        if not all(fp8) or any(len(c.layers) != n_layers for c in caches):
+            raise ValueError("join_caches: FP8 and 16-bit caches cannot be joined together (set pkv_kv_cache_dtype the same "
+                             "for every prompt)")
+        if any(l.k_buf.shape[0] != 1 for c in caches for l in c.layers):
+            raise ValueError("join_caches joins single-prompt (batch 1) caches")
+        return _join_fp8(caches, reserve)
     for c in caches:
         if len(c.layers) != n_layers or not all(isinstance(l, PkvCacheLayer) and not isinstance(l, PkvBatchCacheLayer) for l in c.layers):
             raise RuntimeError("join_caches needs caches prefilled by the patched forward on every layer "

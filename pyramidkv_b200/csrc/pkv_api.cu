@@ -1,4 +1,5 @@
 // pkv_api.cu — the extern "C" boundary declared in include/pkv.h: validation, workspace layout, dispatch.
+#include <algorithm>
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
@@ -560,6 +561,86 @@ static int decode_devlen(const char* fn, const pkv_decode_desc* d, int32_t num_s
 int pkv_decode_attn_batch(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
                           const int32_t* step_dev, int64_t max_length, void* stream) {
     return decode_devlen("pkv_decode_attn_batch", d, num_seqs, cache_stride_b, rows, step_dev, max_length, stream);
+}
+
+int pkv_decode_attn_batch_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
+                              const int32_t* step_dev, int64_t max_length, float* k_scale, float* v_scale, int64_t scale_stride_h,
+                              int64_t scale_stride_b, void* stream) {
+    const char* fn = "pkv_decode_attn_batch_fp8";
+    if ((reinterpret_cast<uintptr_t>(rows) & 3u) || (reinterpret_cast<uintptr_t>(step_dev) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned int32 pointer", fn);
+    if (max_length < 1) return fail(PKV_ERR_INVALID_ARG, "%s: max_length must be >= 1", fn);
+    if (num_seqs < 1 || num_seqs > 65535) return fail(PKV_ERR_INVALID_ARG, "%s: num_seqs=%d outside [1, 65535]", fn, num_seqs);
+    if (!k_scale || !v_scale) return fail(PKV_ERR_INVALID_ARG, "%s: null scale pointer", fn);
+    if ((reinterpret_cast<uintptr_t>(k_scale) & 3u) || (reinterpret_cast<uintptr_t>(v_scale) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned scale pointer", fn);
+    DecodeArgs a;
+    int rc = resolve_decode(d, &a, true, max_length, num_seqs);
+    if (rc) return rc;
+    if (a.cache_sh % 16) return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_h=%lld bytes is not a multiple of 16", fn, (long long)a.cache_sh);
+    if (num_seqs > 1 && (cache_stride_b < int64_t(a.Hq) * a.cache_sh || cache_stride_b % 16))
+        return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_b=%lld is below num_q_heads*cache_stride_h=%lld or not a multiple of 16", fn,
+                    (long long)cache_stride_b, (long long)(int64_t(a.Hq) * a.cache_sh));
+    if (scale_stride_h < max_length || (num_seqs > 1 && scale_stride_b < int64_t(a.Hq) * scale_stride_h))
+        return fail(PKV_ERR_INVALID_ARG, "%s: scale strides (%lld, %lld) hold fewer than max_length=%lld rows per head", fn,
+                    (long long)scale_stride_h, (long long)scale_stride_b, (long long)max_length);
+    if (num_seqs > 1) a.cache_sb = cache_stride_b;
+    a.devlen = true;
+    a.rows = rows;
+    a.step_dev = step_dev;
+    a.k_scale = k_scale;
+    a.v_scale = v_scale;
+    a.scale_sh = scale_stride_h;
+    a.scale_sb = num_seqs > 1 ? scale_stride_b : int64_t(a.Hq) * scale_stride_h;
+    DeviceGuard guard(d->device);
+    const cudaError_t e = launch_decode_fp8(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "fp8 decode launch");
+}
+
+int pkv_cache_quantize_fp8(int32_t dtype, int32_t num_seqs, int32_t num_heads, int32_t head_dim, int32_t device, int32_t num_layers,
+                           const void* const* src, void* const* dst, float* const* scales, const int64_t* src_capacity,
+                           const int64_t* dst_capacity, const int64_t* rows, const int32_t* const* rows_dev, void* stream) {
+    const char* fn = "pkv_cache_quantize_fp8";
+    if (dtype != PKV_BF16 && dtype != PKV_FP16) return fail(PKV_ERR_UNSUPPORTED_DTYPE, "%s: dtype %d: only bf16 (0) and fp16 (1) are supported", fn, dtype);
+    if (head_dim != 64 && head_dim != 128) return fail(PKV_ERR_UNSUPPORTED, "%s: head_dim=%d: only 64 and 128 are built", fn, head_dim);
+    if (num_seqs < 1 || num_heads < 1 || num_layers < 1) return fail(PKV_ERR_INVALID_ARG, "%s: need num_seqs, num_heads, num_layers >= 1", fn);
+    if (!src || !dst || !scales || !src_capacity || !dst_capacity || !rows) return fail(PKV_ERR_INVALID_ARG, "%s: null table", fn);
+    for (int l = 0; l < num_layers; ++l) {
+        for (int kv = 0; kv < 2; ++kv) {
+            const void* s = src[2 * l + kv];
+            const void* t = dst[2 * l + kv];
+            const float* c = scales[2 * l + kv];
+            if (!s || !t || !c) return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: null tensor pointer", fn, l);
+            if (!aligned16(s) || !aligned16(t) || (reinterpret_cast<uintptr_t>(c) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: misaligned tensor pointer", fn, l);
+        }
+        if (rows[l] < 0 || rows[l] > src_capacity[l] || rows[l] > dst_capacity[l])
+            return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: rows=%lld outside [0, capacity] (source %lld, destination %lld)", fn, l,
+                        (long long)rows[l], (long long)src_capacity[l], (long long)dst_capacity[l]);
+        if (rows_dev && (reinterpret_cast<uintptr_t>(rows_dev[l]) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: misaligned row counts", fn, l);
+    }
+    const DevInfo* di = nullptr;
+    int rc = device_info(device, &di);
+    if (rc) return rc;
+    DeviceGuard guard(device);
+    for (int l0 = 0; l0 < num_layers; l0 += kMaxLayerBatch) {
+        QuantArgs a;
+        a.dtype = dtype; a.num_seqs = num_seqs; a.H = num_heads; a.D = head_dim;
+        a.n_layers = std::min(kMaxLayerBatch, num_layers - l0);
+        for (int i = 0; i < a.n_layers; ++i) {
+            const int l = l0 + i;
+            QuantLayer& q = a.layer[i];
+            for (int kv = 0; kv < 2; ++kv) {
+                q.src[kv] = static_cast<const uint16_t*>(src[2 * l + kv]);
+                q.dst[kv] = static_cast<uint8_t*>(dst[2 * l + kv]);
+                q.scale[kv] = scales[2 * l + kv];
+            }
+            q.src_cap = src_capacity[l];
+            q.dst_cap = dst_capacity[l];
+            q.rows = rows[l];
+            q.rows_dev = rows_dev ? rows_dev[l] : nullptr;
+        }
+        const cudaError_t e = launch_quantize_fp8(a, di->sms, static_cast<cudaStream_t>(stream));
+        if (e != cudaSuccess) return fail_cuda(e, "fp8 quantize launch");
+    }
+    return PKV_OK;
 }
 
 int pkv_decode_attn_graph(const pkv_decode_desc* d, const int32_t* step_dev, int64_t max_length, void* stream) {

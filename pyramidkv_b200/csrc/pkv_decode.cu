@@ -18,15 +18,7 @@ constexpr int kDecodeThreads = 256;
 constexpr int kDecodeWarps = kDecodeThreads / 32;
 constexpr int kDecodeUnroll = 4;
 
-// split count for T rows (decode_num_splits); shared by the host launch and the DEVLEN kernels
-__host__ __device__ inline int64_t splits_for(int64_t Hq, int64_t T, int64_t num_sms) {
-    int64_t ns = (T + 255) / 256;                       // ~256 rows (32 per warp) per CTA
-    const int64_t cap = (num_sms * 4 + Hq - 1) / Hq;    // at most ~4 CTAs per SM in flight
-    if (ns > cap) ns = cap;
-    if (ns < 1) ns = 1;
-    if (ns > 64) ns = 64;
-    return ns;
-}
+__host__ __device__ inline int64_t splits_for(int64_t Hq, int64_t T, int64_t num_sms) { return decode_splits_for(Hq, T, num_sms); }
 
 struct DecodeParams {
     const uint16_t *q, *k_new, *v_new;   // q [num_seqs][Hq][D], k_new / v_new [num_seqs][Hkv][D]
@@ -244,6 +236,20 @@ int decode_num_splits(int Hq, int64_t T, int num_sms) { return int(splits_for(Hq
 cudaError_t launch_decode(const DecodeArgs& a, cudaStream_t st) {
     if (a.dtype == PKV_BF16) return a.D == 128 ? launch_decode_t<__nv_bfloat16, 128>(a, st) : launch_decode_t<__nv_bfloat16, 64>(a, st);
     return a.D == 128 ? launch_decode_t<__half, 128>(a, st) : launch_decode_t<__half, 64>(a, st);
+}
+
+cudaError_t launch_decode_combine(const DecodeArgs& a, cudaStream_t st) {
+    const DecodeParams p = make_params(a);
+    const unsigned grid = unsigned(int64_t(a.num_seqs) * a.Hq);
+    if (a.dtype == PKV_BF16) {
+        if (a.D == 128) decode_combine_kernel<__nv_bfloat16, 128><<<grid, 128, 0, st>>>(p);
+        else decode_combine_kernel<__nv_bfloat16, 64><<<grid, 64, 0, st>>>(p);
+    } else {
+        if (a.D == 128) decode_combine_kernel<__half, 128><<<grid, 128, 0, st>>>(p);
+        else decode_combine_kernel<__half, 64><<<grid, 64, 0, st>>>(p);
+    }
+    count_launch();
+    return cudaGetLastError();
 }
 
 cudaError_t launch_append(const DecodeArgs& a, cudaStream_t st) {

@@ -117,10 +117,39 @@ struct DecodeArgs {
     int num_sms;
     const int32_t* step_dev = nullptr;  // device step counter added to T inside the kernel
     const int32_t* rows = nullptr;      // [num_seqs*Hq] per (sequence, head) row counts added to T inside the kernel
+    // FP8 cache (launch_decode_fp8): k_cache / v_cache hold E4M3 bytes, one fp32 scale per (sequence, head, row)
+    float *k_scale = nullptr, *v_scale = nullptr;
+    int64_t scale_sh = 0, scale_sb = 0;   // floats between the scales of consecutive heads / sequences
 };
+// split count for T rows (decode_num_splits); shared by the host launch and the device-length decode kernels
+__host__ __device__ inline int64_t decode_splits_for(int64_t Hq, int64_t T, int64_t num_sms) {
+    int64_t ns = (T + 255) / 256;                       // ~256 rows (32 per warp) per CTA
+    const int64_t cap = (num_sms * 4 + Hq - 1) / Hq;    // at most ~4 CTAs per SM in flight
+    if (ns > cap) ns = cap;
+    if (ns < 1) ns = 1;
+    if (ns > 64) ns = 64;
+    return ns;
+}
 int decode_num_splits(int Hq, int64_t T, int num_sms);
 cudaError_t launch_decode(const DecodeArgs& a, cudaStream_t st);
+cudaError_t launch_decode_combine(const DecodeArgs& a, cudaStream_t st);   // merges the split partials in a.ws into a.out
 cudaError_t launch_append(const DecodeArgs& a, cudaStream_t st);
+
+// ---- FP8 (E4M3) compacted cache (pkv_fp8.cu) ----
+cudaError_t launch_decode_fp8(const DecodeArgs& a, cudaStream_t st);   // device-length form only (a.devlen)
+struct QuantLayer {
+    const uint16_t* src[2];   // K, V: 16-bit [num_seqs][H][src_cap][D]
+    uint8_t* dst[2];          // K, V: E4M3 [num_seqs][H][dst_cap][D]
+    float* scale[2];          // K, V: fp32 [num_seqs][H][dst_cap]
+    int64_t src_cap, dst_cap;
+    int64_t rows;             // rows per (sequence, head); with rows_dev the bound of the device counts
+    const int32_t* rows_dev;  // optional device int32 [num_seqs*H]
+};
+struct QuantArgs {
+    int dtype, num_seqs, H, D, n_layers;   // n_layers <= kMaxLayerBatch
+    QuantLayer layer[kMaxLayerBatch];
+};
+cudaError_t launch_quantize_fp8(const QuantArgs& a, int num_sms, cudaStream_t st);
 
 // RoPE in place on Q and K (pkv_rope.cu)
 struct RopeArgs {

@@ -16,6 +16,9 @@ CPU, eager mode with the test backend; `-m gpu`: graph vs eager vs HF generate).
 `greedy_generate`), their compacted caches are joined (`cache.join_caches`) and one step decodes all of them - one graph
 replay per token, one attention launch per layer (`pkv_decode_attn_batch`) - so the weights are streamed once per step for
 the whole batch instead of once per sequence.
+
+With `model.config.pkv_kv_cache_dtype = "fp8_e4m3"` the prefill leaves FP8 caches (`cache.PkvFp8CacheLayer`); all three loops
+take them as they are (the knob is the single source: no parameter here), one `pkv_decode_attn_batch_fp8` launch per layer.
 """
 from __future__ import annotations
 

@@ -69,6 +69,15 @@ class CudaBackend:
                           out=None, softmax_scale=0.0):
         return ops.decode_attn_batch(q, k_buf, v_buf, length, k_new, v_new, rows, step, max_length, workspace, out, softmax_scale)
 
+    # -- the opt-in FP8 cache (model.config.pkv_kv_cache_dtype = "fp8_e4m3") --
+    def cache_quantize_fp8(self, layers):
+        ops.cache_quantize_fp8(layers)
+
+    def decode_attn_batch_fp8(self, q, k_q, v_q, k_scale, v_scale, length, k_new, v_new, rows=None, step=None, max_length=0,
+                              workspace=None, out=None, softmax_scale=0.0):
+        return ops.decode_attn_batch_fp8(q, k_q, v_q, k_scale, v_scale, length, k_new, v_new, rows, step, max_length, workspace,
+                                         out, softmax_scale)
+
     def rope_inplace(self, q, k, cos, sin):
         ops.rope_inplace(q, k, cos, sin)
 

@@ -465,6 +465,123 @@ def decode_attn_batch(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor,
     return out
 
 
+# ---- the opt-in FP8 (E4M3) compacted cache (include/pkv.h: pkv_cache_quantize_fp8, pkv_decode_attn_batch_fp8) ----
+FP8_DTYPE = torch.float8_e4m3fn
+
+
+def _check_fp8_buffers(kq: torch.Tensor, vq: torch.Tensor, ks: torch.Tensor, vs: torch.Tensor, what: str):
+    if kq.dtype != FP8_DTYPE or vq.dtype != FP8_DTYPE:
+        raise ValueError(f"{what}: the FP8 buffers must be torch.float8_e4m3fn, got {kq.dtype} / {vq.dtype}")
+    if kq.dim() != 4 or kq.shape != vq.shape or not kq.is_contiguous() or not vq.is_contiguous():
+        raise ValueError(f"{what}: the FP8 buffers must be contiguous [B, Hq, capacity, D] tensors of equal shape")
+    if ks.dtype != torch.float32 or vs.dtype != torch.float32 or ks.shape != kq.shape[:3] or vs.shape != ks.shape \
+            or not ks.is_contiguous() or not vs.is_contiguous():
+        raise ValueError(f"{what}: the scales must be contiguous float32 [B, Hq, capacity] = {tuple(kq.shape[:3])} tensors")
+    if kq.data_ptr() % 16 or vq.data_ptr() % 16:
+        raise ValueError(f"{what}: the FP8 buffers must be 16-byte aligned")
+
+
+def cache_quantize_fp8(layers) -> None:
+    """Convert the compacted 16-bit caches of several layers to FP8 on the current stream: one launch per 32 layers
+    (`pkv_cache_quantize_fp8`). `layers`: (k, v, k_q, v_q, k_scale, v_scale, rows, rows_dev) per layer, with k / v the
+    16-bit [B, Hq, capacity, D] buffers the eviction wrote, k_q / v_q float8_e4m3fn [B, Hq, capacity', D] and k_scale /
+    v_scale float32 [B, Hq, capacity'] to fill; every (sequence, head) converts `rows` rows, or, when `rows_dev` (int32
+    [B*Hq] on the device) is given, its own count from it (at most `rows`). Rows past the count are not written."""
+    layers = list(layers)
+    if not layers:
+        return
+    k0 = layers[0][0]
+    B, Hq, _, D = k0.shape
+    n = len(layers)
+    src, dst, scl = (C.c_void_p * (2 * n))(), (C.c_void_p * (2 * n))(), (C.c_void_p * (2 * n))()
+    scap, dcap, rows_t = (C.c_int64 * n)(), (C.c_int64 * n)(), (C.c_int64 * n)()
+    rdev = (C.c_void_p * n)()
+    for i, (k, v, kq, vq, ks, vs, rows, rows_dev) in enumerate(layers):
+        _require_cuda(k, v, kq, vq, ks, vs, rows_dev)
+        if k.dim() != 4 or k.shape != v.shape or not k.is_contiguous() or not v.is_contiguous() or k.dtype != v.dtype:
+            raise ValueError(f"cache_quantize_fp8: layer {i}: the 16-bit buffers must be contiguous [B, Hq, capacity, D] tensors of equal shape")
+        if k.dtype != k0.dtype or k.device != k0.device or (k.shape[0], k.shape[1], k.shape[3]) != (B, Hq, D):
+            raise ValueError(f"cache_quantize_fp8: layer {i}: batch, heads, head_dim, dtype and device must match layer 0")
+        _check_fp8_buffers(kq, vq, ks, vs, f"cache_quantize_fp8: layer {i}")
+        if (kq.shape[0], kq.shape[1], kq.shape[3]) != (B, Hq, D) or kq.device != k.device:
+            raise ValueError(f"cache_quantize_fp8: layer {i}: the FP8 buffers must be [B, Hq, capacity, D] = [{B}, {Hq}, *, {D}] on {k.device}")
+        if not 0 <= int(rows) <= min(k.shape[2], kq.shape[2]):
+            raise ValueError(f"cache_quantize_fp8: layer {i}: rows={rows} exceeds a capacity ({k.shape[2]}, {kq.shape[2]})")
+        if rows_dev is not None and (rows_dev.dtype != torch.int32 or rows_dev.numel() != B * Hq or not rows_dev.is_contiguous()):
+            raise ValueError(f"cache_quantize_fp8: layer {i}: rows_dev must be a contiguous int32 device tensor of B*Hq = {B * Hq} elements")
+        src[2 * i], src[2 * i + 1] = k.data_ptr(), v.data_ptr()
+        dst[2 * i], dst[2 * i + 1] = kq.data_ptr(), vq.data_ptr()
+        scl[2 * i], scl[2 * i + 1] = ks.data_ptr(), vs.data_ptr()
+        scap[i], dcap[i], rows_t[i] = k.shape[2], kq.shape[2], int(rows)
+        rdev[i] = rows_dev.data_ptr() if rows_dev is not None else None
+    dev = k0.device.index if k0.device.index is not None else torch.cuda.current_device()
+    _lib.check(_lib.lib().pkv_cache_quantize_fp8(_dtype_code(k0), B, Hq, D, dev, n, src, dst, scl, scap, dcap, rows_t,
+                                                 rdev if any(l[7] is not None for l in layers) else None,
+                                                 torch.cuda.current_stream(k0.device).cuda_stream))
+
+
+def decode_attn_batch_fp8(q: torch.Tensor, k_q: torch.Tensor, v_q: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor,
+                          length: int, k_new: Optional[torch.Tensor] = None, v_new: Optional[torch.Tensor] = None,
+                          rows: Optional[torch.Tensor] = None, step: Optional[torch.Tensor] = None, max_length: int = 0,
+                          workspace: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                          softmax_scale: float = 0.0) -> torch.Tensor:
+    """`decode_attn_batch` over an FP8 cache (`pkv_decode_attn_batch_fp8`): k_q / v_q float8_e4m3fn [B, Hq, capacity, D],
+    k_scale / v_scale float32 [B, Hq, capacity]; q [B, Hq, D] and k_new / v_new [B, Hkv, D] in bf16 / fp16. The new row
+    is quantised, stored (bytes and scale) and attended as stored. The same row counts, launch sizing and graph
+    replayability as `decode_attn_batch`; one sequence is B = 1 (step None for a host launch). Returns out [B, Hq, D]."""
+    _require_cuda(q, k_q, v_q, k_scale, v_scale, k_new, v_new, rows, step, workspace, out)
+    _check_fp8_buffers(k_q, v_q, k_scale, v_scale, "decode_attn_batch_fp8")
+    B, Hq, cap, D = k_q.shape
+    if q.shape != (B, Hq, D):
+        raise ValueError(f"q must be [B, Hq, D] = {(B, Hq, D)}, got {tuple(q.shape)}")
+    if not q.is_contiguous():
+        q = q.contiguous()
+    if out is None:
+        out = torch.empty(B, Hq, D, dtype=q.dtype, device=q.device)
+    elif out.shape != (B, Hq, D) or not out.is_contiguous() or out.dtype != q.dtype:
+        raise ValueError("out must be a contiguous [B, Hq, D] tensor of q's dtype")
+    max_length = int(max_length) or cap
+    if not 1 <= length <= max_length <= cap:
+        raise ValueError(f"cache capacity {cap} exceeded or bad row counts (length {length}, max_length {max_length})")
+    if step is not None and (step.dtype != torch.int32 or step.numel() != 1):
+        raise ValueError("step must be an int32 device tensor with one element")
+    if rows is not None:
+        if rows.dtype != torch.int32 or rows.numel() != B * Hq or not rows.is_contiguous():
+            raise ValueError(f"rows must be a contiguous int32 device tensor of B*Hq = {B * Hq} elements")
+        if not torch.cuda.is_current_stream_capturing():
+            most = int(rows.max()) + int(length) + (int(step) if step is not None else 0)
+            if most > max_length:
+                raise ValueError(f"cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
+    d = DecodeDesc()
+    d.struct_bytes = C.sizeof(DecodeDesc)
+    d.dtype, d.num_q_heads, d.head_dim = _dtype_code(q), Hq, D
+    d.device = q.device.index if q.device.index is not None else torch.cuda.current_device()
+    d.length = int(length)
+    d.q, d.k_cache, d.v_cache, d.cache_stride_h, d.out = q.data_ptr(), k_q.data_ptr(), v_q.data_ptr(), k_q.stride(1), out.data_ptr()
+    keep = [q, out]
+    if k_new is not None:
+        if k_new.dim() != 3 or k_new.shape[0] != B or k_new.shape[2] != D or v_new is None or v_new.shape != k_new.shape \
+                or k_new.dtype != q.dtype or v_new.dtype != q.dtype:
+            raise ValueError("k_new / v_new must be [B, Hkv, D] tensors of q's dtype")
+        k_new, v_new = k_new.contiguous(), v_new.contiguous()
+        d.num_kv_heads = k_new.shape[1]
+        d.k_new, d.v_new = k_new.data_ptr(), v_new.data_ptr()
+        keep += [k_new, v_new]
+    else:
+        d.num_kv_heads = Hq
+    d.num_q_heads = B * Hq                 # workspace query: one set of split partials per (sequence, head)
+    nbytes = int(_lib.lib().pkv_decode_workspace_bytes(C.byref(d)))
+    d.num_q_heads = Hq
+    ws = workspace if workspace is not None else _workspace(q.device, nbytes)
+    d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel() * ws.element_size()
+    d.softmax_scale = float(softmax_scale)
+    _lib.check(_lib.lib().pkv_decode_attn_batch_fp8(C.byref(d), B, k_q.stride(0), rows.data_ptr() if rows is not None else None,
+                                                    step.data_ptr() if step is not None else None, max_length,
+                                                    k_scale.data_ptr(), v_scale.data_ptr(), k_scale.stride(1), k_scale.stride(0),
+                                                    torch.cuda.current_stream(q.device).cuda_stream))
+    return out
+
+
 def decode_workspace_bytes(num_q_heads: int, head_dim: int) -> int:
     """Upper bound of the decode workspace for any cache length (`pkv_decode_workspace_bytes`)."""
     d = DecodeDesc()

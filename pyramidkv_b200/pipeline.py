@@ -94,6 +94,9 @@ class PipelineRunner:
 
     def __init__(self, stage: Stage, group=None):
         from transformers import DynamicCache
+        if getattr(stage.config, "pkv_kv_cache_dtype", None) not in (None, "auto"):
+            raise NotImplementedError("the FP8 compacted cache (pkv_kv_cache_dtype) is converted by the model's last layer in one "
+                                      "launch; the layer-sliced pipeline flushes per rank and keeps the 16-bit cache")
         self.stage, self.group = stage, group
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1

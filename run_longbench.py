@@ -55,6 +55,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--prompt_tokens", type=int, default=0, help="override the task's typical prompt length")
     p.add_argument("--decode_loop", type=str, default="hf", choices=["hf", "static", "static-eager"],
                    help="hf: model.generate as in the reference; static: pyramidkv_b200.generate (CUDA-graph replay per token)")
+    p.add_argument("--kv_cache_dtype", type=str, default="auto", choices=["auto", "fp8_e4m3"],
+                   help="auto: the compacted cache in the model dtype; fp8_e4m3: FP8 bytes + one fp32 scale per row (half the KV bytes)")
     return p
 
 
@@ -87,7 +89,8 @@ def main(argv=None, backend_factory=None, device=None):
                             attn_implementation=args.attn_implementation, merge=args.merge, seed=args.seed,
                             backend_factory=backend_factory, out_path=out, decode_loop=args.decode_loop,
                             floor=args.floor, head_beta=args.head_beta, head_path=args.head_path,
-                            capacity_ratio=args.max_capacity_prompts_ratio, eval_batch_size=args.eval_batch_size)
+                            capacity_ratio=args.max_capacity_prompts_ratio, eval_batch_size=args.eval_batch_size,
+                            kv_cache_dtype=args.kv_cache_dtype)
     n = len(recs)
     print(json.dumps({"summary": True, "arch": arch, "method": method, "max_capacity_prompts": capacity, "examples": n,
                       "mean_prefill_ms": sum(r["prefill_ms"] for r in recs) / n,

@@ -8,6 +8,10 @@ reference runners' knobs (window 8, kernel 7, maxpool). Prints one JSON line wit
                   launch per layer) per batch size B: aggregate tok/s, ms per step, and the bound
                   (weight bytes + algorithmic KV bytes) / HBM bandwidth
   decode_batched_attn  the attention launches of one step alone, KV bytes read over their time as a fraction of the bandwidth
+--kv_cache_dtype bf16,fp8_e4m3 measures both caches, alternating them per batch size in the same process: the FP8 caches are
+the bf16 caches of the same prompts converted exactly as the knob pkv_kv_cache_dtype = "fp8_e4m3" converts them after the
+prefill; their KV bytes count one byte per element plus the two 4-byte scales of every row and head. --batch max picks, per
+dtype, the largest batch whose joined caches fit the free device memory, computed from bytes before allocating.
 Writes nothing but stdout.
 """
 import argparse
@@ -41,77 +45,117 @@ def gpu_card(device):
     return info
 
 
-def decode_batched_numbers(model, device, ctx, batch_sizes, weight_bytes, new_tokens=32, distinct=2, attn_steps=50):
+def _kv_row_bytes(D, kv_dtype):
+    """Bytes one (sequence, head) reads per cached row for K and V: bf16 elements, or E4M3 bytes plus two fp32 scales."""
+    return 2 * D * 2 if kv_dtype == "bf16" else 2 * D + 8
+
+
+def _cache_bytes_per_seq(model, caches, reserve, kv_dtype):
+    """Bytes one sequence's joined cache allocates (the buffers are [Hq, longest + reserve, D] per layer)."""
+    Hq, D = model.config.num_attention_heads, model.config.head_dim
+    return sum(Hq * (max(l.length for l in ls) + reserve) * _kv_row_bytes(D, kv_dtype) for ls in zip(*[c.layers for c in caches]))
+
+
+def decode_batched_numbers(model, device, ctx, batch_sizes, weight_bytes, new_tokens=32, distinct=2, attn_steps=50,
+                           kv_dtypes=("bf16",), headroom_bytes=4 << 30):
     """Batched greedy decode (pyramidkv_b200.generate: joined compacted caches, one CUDA-graph replay per step, one attention
     launch per layer whatever the batch). `distinct` prompts are prefilled and joined repeated up to each batch size B: the
     cost of a decode step does not depend on the cache contents, and this avoids B prefills of the long prompt.
     decode_batched: aggregate tok/s and ms per step next to the bound (weight bytes + KV bytes) / HBM bandwidth.
     decode_batched_attn: the attention launches of one step alone (all layers, CUDA events over attn_steps steps); KV bytes
-    read per step over their time as a fraction of the bandwidth."""
+    read per step over their time as a fraction of the bandwidth. For each B the cache dtypes are measured one after the
+    other. batch_sizes may hold "max": the largest B whose joined caches fit the free memory less `headroom_bytes`."""
+    from transformers import DynamicCache
     from pyramidkv_b200 import ops
-    from pyramidkv_b200.cache import join_caches
+    from pyramidkv_b200.cache import PkvFp8CacheLayer, join_caches, quantize_caches_fp8
     from pyramidkv_b200.generate import StaticDecoder, _prefill
     bw_gbs, bw_src = peaks()
-    firsts, caches = [], []
+    firsts, caches = [], {"bf16": []}
     for i in range(distinct):
         ids = torch.randint(1, model.config.vocab_size, (1, ctx), generator=torch.Generator().manual_seed(100 + i)).to(device)
         f, c = _prefill(model, ids)
         firsts.append(f)
-        caches.append(c)
-    points, attn = [], []
-    for B in batch_sizes:
-        pick = [i % distinct for i in range(B)]
-        cache = join_caches([caches[i] for i in pick], reserve=new_tokens + 3)
-        first = torch.cat([firsts[i] for i in pick])
-        D = cache.layers[0].k_buf.shape[3]
-        # algorithmic KV bytes of one step: every (sequence, head) reads its K and V rows (+ the appended one), bf16
-        kv_bytes = sum(2 * (r + 1) * D * 2 for l in cache.layers for row in l.rows_host for r in row)
-        # attention alone: the per-layer batched launches of one step at the first step's row counts (fixed step counter)
-        Hq, Hkv = model.config.num_attention_heads, model.config.num_key_value_heads
-        g = torch.Generator(device=device).manual_seed(B)
-        q = torch.randn(B, Hq, D, generator=g, device=device).bfloat16()
-        kn = torch.randn(B, Hkv, D, generator=g, device=device).bfloat16()
-        step = torch.zeros(1, dtype=torch.int32, device=device)
-        ws = torch.empty(ops.decode_workspace_bytes(B * Hq, D), dtype=torch.uint8, device=device)
-        out = torch.empty(B, Hq, D, dtype=torch.bfloat16, device=device)
+        caches["bf16"].append(c)
+    if "fp8_e4m3" in kv_dtypes:
+        backend = model.model.layers[0].self_attn.kv_cluster.backend
+        caches["fp8_e4m3"] = []
+        for c in caches["bf16"]:                         # the conversion the knob runs after the prefill, on a copy of the list
+            c8 = DynamicCache()
+            c8.layers = list(c.layers)
+            quantize_caches_fp8(c8, backend)
+            caches["fp8_e4m3"].append(c8)
+    reserve = new_tokens + 3
+    points, attn, fits = [], [], {}
+    torch.cuda.synchronize()
+    for Bspec in batch_sizes:
+        for kv_dtype in kv_dtypes:
+            per_seq = _cache_bytes_per_seq(model, caches[kv_dtype], reserve, kv_dtype)
+            if Bspec == "max":
+                free, total = torch.cuda.mem_get_info(device)
+                B = max(1, int((free - headroom_bytes) // per_seq))
+                fits[kv_dtype] = {"batch": B, "cache_bytes_per_seq": per_seq, "free_bytes": free, "total_bytes": total,
+                                  "headroom_bytes": headroom_bytes}
+            else:
+                B = int(Bspec)
+            pick = [i % distinct for i in range(B)]
+            cache = join_caches([caches[kv_dtype][i] for i in pick], reserve=reserve)
+            first = torch.cat([firsts[i] for i in pick])
+            fp8 = isinstance(cache.layers[0], PkvFp8CacheLayer)
+            D = cache.layers[0].k_buf.shape[3]
+            # algorithmic KV bytes of one step: every (sequence, head) reads its K and V rows (+ the appended one)
+            kv_bytes = sum((r + 1) * _kv_row_bytes(D, kv_dtype) for l in cache.layers for row in l.rows_host for r in row)
+            # attention alone: the per-layer batched launches of one step at the first step's row counts (fixed step counter)
+            Hq, Hkv = model.config.num_attention_heads, model.config.num_key_value_heads
+            g = torch.Generator(device=device).manual_seed(B)
+            q = torch.randn(B, Hq, D, generator=g, device=device).bfloat16()
+            kn = torch.randn(B, Hkv, D, generator=g, device=device).bfloat16()
+            step = torch.zeros(1, dtype=torch.int32, device=device)
+            ws = torch.empty(ops.decode_workspace_bytes(B * Hq, D), dtype=torch.uint8, device=device)
+            out = torch.empty(B, Hq, D, dtype=torch.bfloat16, device=device)
 
-        def attn_step():
-            for l in cache.layers:
-                ops.decode_attn_batch(q, l.k_buf, l.v_buf, 1, kn, kn, rows=l.rows, step=step, max_length=l.capacity,
-                                      workspace=ws, out=out)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        for _ in range(3):
-            attn_step()
-        graph = torch.cuda.CUDAGraph()                   # replayed: the host-side argument checks are not kernel time
-        with torch.cuda.graph(graph):
-            attn_step()
-        graph.replay()
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(attn_steps):
+            def attn_step():
+                for l in cache.layers:
+                    if fp8:
+                        ops.decode_attn_batch_fp8(q, l.k_buf, l.v_buf, l.k_scale, l.v_scale, 1, kn, kn, rows=l.rows, step=step,
+                                                  max_length=l.capacity, workspace=ws, out=out)
+                    else:
+                        ops.decode_attn_batch(q, l.k_buf, l.v_buf, 1, kn, kn, rows=l.rows, step=step, max_length=l.capacity,
+                                              workspace=ws, out=out)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            for _ in range(3):
+                attn_step()
+            graph = torch.cuda.CUDAGraph()                   # replayed: the host-side argument checks are not kernel time
+            with torch.cuda.graph(graph):
+                attn_step()
             graph.replay()
-        e1.record()
-        torch.cuda.synchronize()
-        attn_ms = e0.elapsed_time(e1) / attn_steps
-        attn.append({"batch": B, "attn_ms_per_step": attn_ms, "launches_per_step": len(cache.layers), "kv_bytes_per_step": kv_bytes,
-                     "kv_gbs": kv_bytes / (attn_ms * 1e-3) / 1e9, "frac_of_hbm": kv_bytes / (attn_ms * 1e-3) / (bw_gbs * 1e9)})
-        dec = StaticDecoder(model, cache, first, new_tokens + 3, use_graph=True)
-        dec.run(3)
-        torch.cuda.synchronize()
-        e0.record()
-        dec.run(new_tokens)
-        e1.record()
-        torch.cuda.synchronize()
-        ms = e0.elapsed_time(e1) / new_tokens
-        bound_ms = (weight_bytes + kv_bytes) / (bw_gbs * 1e9) * 1e3
-        points.append({"batch": B, "ms_per_step": ms, "aggregate_tok_s": B * 1e3 / ms, "kv_bytes_per_step": kv_bytes,
-                       "weight_bytes": weight_bytes, "weight_floor_ms": weight_bytes / (bw_gbs * 1e9) * 1e3,
-                       "bound_ms": bound_ms, "step_over_bound": ms / bound_ms})
-        dec.finish()
-        del graph, dec, cache, first
-        torch.cuda.empty_cache()
+            torch.cuda.synchronize()
+            e0.record()
+            for _ in range(attn_steps):
+                graph.replay()
+            e1.record()
+            torch.cuda.synchronize()
+            attn_ms = e0.elapsed_time(e1) / attn_steps
+            attn.append({"batch": B, "kv_cache_dtype": kv_dtype, "attn_ms_per_step": attn_ms, "launches_per_step": len(cache.layers),
+                         "kv_bytes_per_step": kv_bytes, "kv_gbs": kv_bytes / (attn_ms * 1e-3) / 1e9,
+                         "frac_of_hbm": kv_bytes / (attn_ms * 1e-3) / (bw_gbs * 1e9)})
+            del graph
+            dec = StaticDecoder(model, cache, first, new_tokens + 3, use_graph=True)
+            dec.run(3)
+            torch.cuda.synchronize()
+            e0.record()
+            dec.run(new_tokens)
+            e1.record()
+            torch.cuda.synchronize()
+            ms = e0.elapsed_time(e1) / new_tokens
+            bound_ms = (weight_bytes + kv_bytes) / (bw_gbs * 1e9) * 1e3
+            points.append({"batch": B, "kv_cache_dtype": kv_dtype, "ms_per_step": ms, "aggregate_tok_s": B * 1e3 / ms,
+                           "kv_bytes_per_step": kv_bytes, "weight_bytes": weight_bytes,
+                           "weight_floor_ms": weight_bytes / (bw_gbs * 1e9) * 1e3, "bound_ms": bound_ms, "step_over_bound": ms / bound_ms})
+            dec.finish()
+            del dec, cache, first
+            torch.cuda.empty_cache()
     note = f"bandwidth {bw_gbs:.0f} GB/s: {bw_src}"
-    return ({"ctx": ctx, "new_tokens": new_tokens, "distinct_prompts": distinct, "bandwidth": note, "points": points},
+    return ({"ctx": ctx, "new_tokens": new_tokens, "distinct_prompts": distinct, "bandwidth": note, "points": points, "fits": fits},
             {"steps": attn_steps, "bandwidth": note, "points": attn})
 
 
@@ -139,7 +183,12 @@ def main():
     ap.add_argument("--ctx", type=int, default=32768)
     ap.add_argument("--budget", type=int, default=128)
     ap.add_argument("--new", type=int, default=32, help="timed decode steps per batch size")
+    ap.add_argument("--kv_cache_dtype", default="bf16", help="comma-separated cache dtypes: bf16, fp8_e4m3")
+    ap.add_argument("--no_single", action="store_true", help="skip the single-sequence loop")
     args = ap.parse_args()
+    kv_dtypes = [x.strip() for x in args.kv_cache_dtype.split(",") if x.strip()]
+    if not kv_dtypes or any(x not in ("bf16", "fp8_e4m3") for x in kv_dtypes):
+        raise SystemExit(f"--kv_cache_dtype takes bf16 and / or fp8_e4m3, got {args.kv_cache_dtype!r}")
     if not torch.cuda.is_available():
         raise SystemExit("tools/decode_batch_bench.py measures on a CUDA device (H100); there is none here")
     device = torch.device("cuda", 0)
@@ -154,14 +203,15 @@ def main():
         model.config.pkv_fused_rope = True
         weight_bytes = sum(p.numel() * p.element_size() for p in model.parameters())
         with torch.no_grad():
-            single = single_sequence(model, device, args.ctx)
+            single = None if args.no_single else single_sequence(model, device, args.ctx)
             torch.cuda.empty_cache()
-            batched, attn = decode_batched_numbers(model, device, args.ctx, [int(x) for x in args.batch.split(",") if x.strip()],
-                                                   weight_bytes, new_tokens=args.new)
+            batch = [x.strip() if x.strip() == "max" else int(x) for x in args.batch.split(",") if x.strip()]
+            batched, attn = decode_batched_numbers(model, device, args.ctx, batch, weight_bytes, new_tokens=args.new,
+                                                   kv_dtypes=kv_dtypes)
     finally:
         restore()
     print(json.dumps({"model": "llama3-8b (random init)", "method": "pyramidkv", "ctx": args.ctx, "budget": args.budget,
-                      "dtype": "bf16", "fused_rope": True, "gpu": gpu_card(device), "weight_bytes": weight_bytes,
+                      "dtype": "bf16", "kv_cache_dtypes": kv_dtypes, "fused_rope": True, "gpu": gpu_card(device), "weight_bytes": weight_bytes,
                       "single": single, "decode_batched": batched, "decode_batched_attn": attn}))
 
 
