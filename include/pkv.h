@@ -80,6 +80,25 @@ typedef enum pkv_pooling { PKV_AVGPOOL = 0, PKV_MAXPOOL = 1 } pkv_pooling;
  * kernel, for every shape that kernel supports. Identical results. Not the default: its flag waits need every CTA to be
  * co-resident, which only the slower cooperative launch guarantees. */
 #define PKV_FLAG_FUSED 64u
+/* pkv_evict_desc.flags bit 7: GQA-shared selection — ONE compacted cache per KV head instead of one per query head.
+ * k_cache / v_cache / cache_stride_h then describe [num_kv_heads, >= top_k+window, head_dim] and idx_out is
+ * [num_kv_heads, top_k]. With G = num_q_heads / num_kv_heads:
+ *  - PyramidKV, SnapKV, H2O: stage 2 writes `pooled` [num_q_heads][S-W] exactly as without the flag; a group reduction then
+ *    writes pooled_kv[j][t] = rn_dtype((sum over g = 0..G-1, ascending, in fp32, of f32(pooled[j*G+g][t])) / f32(G)) (one
+ *    correctly rounded fp32 division, one rounding to the model dtype) into a workspace segment of its own
+ *    (pkv_evict_pooled_kv_offset), and
+ *    stages 3-4 run over num_kv_heads "heads" with G = 1 on it: KV head j keeps K[j] / V[j] at its top_k indices under the
+ *    stage-3 tie rule, in score order, followed by the last `window` rows. The reduction follows the pooling, so with
+ *    maxpool the mean of pooled scores is not the pool of the mean.
+ *  - StreamingLLM, L2Norm: the selection does not depend on the query head; each KV head is selected directly (the cache
+ *    of the flagless call with the G identical copies removed). L2Norm's key norms are computed per KV head in `pooled`.
+ * With G = 1 the flag changes nothing. PKV_FLAG_FUSED / PKV_FLAG_SINGLE_LAUNCH and the layer batch (pkv_evict_prefill_batch,
+ * pkv_evict_batch_supported, pkv_stage_batch) return PKV_ERR_UNSUPPORTED with it, as do pkv_stage_scan_pool,
+ * pkv_adakv_counts and pkv_ragged_place_window. The stage entry points follow the same split: pkv_stage_pool includes
+ * the group reduction, pkv_stage_topk / pkv_stage_gather run per KV head. */
+#define PKV_FLAG_GQA_SHARED 128u
+/* Flags outside this set are rejected with PKV_ERR_INVALID_ARG. */
+#define PKV_EVICT_KNOWN_FLAGS 255u
 
 /* One layer's prefill eviction: the body of *KVCluster.update_kv with merge=None. */
 typedef struct pkv_evict_desc {
@@ -104,7 +123,8 @@ typedef struct pkv_evict_desc {
     int64_t* idx_out;      /* optional [num_q_heads, top_k] int64 selected token indices, may be NULL */
     void* workspace;
     uint64_t workspace_bytes;
-    uint32_t flags;        /* PKV_SCORE_* | PKV_FLAG_WINDOW_MEAN | PKV_FLAG_INPUTS_READY | PKV_FLAG_STAGED | PKV_FLAG_SINGLE_LAUNCH */
+    uint32_t flags;        /* PKV_SCORE_* | PKV_FLAG_WINDOW_MEAN | PKV_FLAG_INPUTS_READY | PKV_FLAG_STAGED | PKV_FLAG_SINGLE_LAUNCH |
+                            * PKV_FLAG_FUSED | PKV_FLAG_GQA_SHARED */
     uint32_t reserved;
 } pkv_evict_desc;
 
@@ -155,6 +175,11 @@ int pkv_layer_budget(int method, int64_t max_capacity_prompt, int64_t window, in
 /* Workspace size / layout for pkv_evict_prefill and its stage entry points. */
 int pkv_evict_workspace_layout(const pkv_evict_desc* d, pkv_ws_layout* out);
 uint64_t pkv_evict_workspace_bytes(const pkv_evict_desc* d);
+/* PKV_FLAG_GQA_SHARED with a scoring method (not StreamingLLM): *off_out = byte offset in the workspace of the per-KV-head top-k
+ * input, dtype [num_kv_heads][pooled_pitch] (the group reduction of `pooled`; = pooled_off for L2Norm and when G = 1). For
+ * stage-level tests and debugging; kept out of pkv_ws_layout so that the struct callers allocate keeps its size.
+ * PKV_ERR_INVALID_ARG without the flag, for StreamingLLM (no scores) or a null pointer. */
+int pkv_evict_pooled_kv_offset(const pkv_evict_desc* d, uint64_t* off_out);
 
 /* Whole eviction of one layer = stages 1-4 below on `stream` (three launches: window scores; softmax + pool; select +
  * gather). PKV_FLAG_FUSED / PKV_FLAG_SINGLE_LAUNCH select the fused forms (identical results) where the shape allows
@@ -269,6 +294,24 @@ int pkv_decode_attn_batch(const pkv_decode_desc* d, int32_t num_seqs, int64_t ca
 int pkv_decode_attn_batch_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
                               const int32_t* step_dev, int64_t max_length, float* k_scale, float* v_scale, int64_t scale_stride_h,
                               int64_t scale_stride_b, void* stream);
+/* The decode step over GQA-shared caches (PKV_FLAG_GQA_SHARED): one cache per KV head, [num_seqs, num_kv_heads, capacity,
+ * head_dim], read ONCE for the G = num_q_heads / num_kv_heads query heads of its group (G in {2, 4, 8}). q / out are
+ * [num_seqs, num_q_heads, head_dim] and k_new / v_new [num_seqs, num_kv_heads, head_dim]; cache_stride_h counts the elements
+ * (FP8: bytes) between KV heads and cache_stride_b those between sequences (>= num_kv_heads*cache_stride_h). Sequence s, KV
+ * head j attends rows = d->length (+ *step_dev) (+ rows[s*num_kv_heads + j]), `rows` DEVICE int32 [num_seqs*num_kv_heads].
+ * Grid (split, KV head, sequence): one CTA reads each row once and computes all G query heads (G = 8 on the FP8 cache: two
+ * CTAs of four heads each). The split count is the one pkv_decode_attn_batch uses for num_q_heads heads and that row count,
+ * and the partials stay per query head, so the workspace is pkv_decode_workspace_bytes with num_q_heads =
+ * num_seqs*num_q_heads. Query head h's output and the appended row are bit-identical to pkv_decode_attn_batch /
+ * pkv_decode_attn_batch_fp8 over the same cache repeat-interleaved G times along the heads. The CTA that owns the last row
+ * stores (FP8: quantises and stores) k_new / v_new of its KV head once and attends it as stored. Graph replayability,
+ * NaN output for a row count outside [1, max_length] and argument errors follow pkv_decode_attn_batch /
+ * pkv_decode_attn_batch_fp8; G outside {2, 4, 8} is PKV_ERR_UNSUPPORTED. FP8 scales: [num_seqs, num_kv_heads, capacity]. */
+int pkv_decode_attn_batch_gqa(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
+                              const int32_t* step_dev, int64_t max_length, void* stream);
+int pkv_decode_attn_batch_gqa_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
+                                  const int32_t* step_dev, int64_t max_length, float* k_scale, float* v_scale,
+                                  int64_t scale_stride_h, int64_t scale_stride_b, void* stream);
 /* Conversion of the compacted 16-bit caches of num_layers layers (one prompt, or one equal-length batch of num_seqs
  * sequences) to the FP8 format above, in one launch per 32 layers; the per-layer tables travel as kernel parameters.
  * Layer l: src[2l] / src[2l+1] = K / V, 16-bit contiguous [num_seqs, num_heads, src_capacity[l], head_dim]; dst[2l] /

@@ -21,8 +21,10 @@ EXPORTS = [
     "pkv_stage_gather", "pkv_decode_workspace_bytes", "pkv_decode_attn", "pkv_decode_attn_graph", "pkv_cache_append", "pkv_host_pick_rows", "pkv_debug_read_stamps", "pkv_rope_inplace", "pkv_update_flatten_view", "pkv_adakv_scratch_bytes", "pkv_adakv_counts",
     "pkv_ragged_place_window", "pkv_decode_attn_ragged", "pkv_evict_single_launch", "pkv_stage_scan_pool",
     "pkv_evict_prefill_batch", "pkv_evict_batch_supported", "pkv_stage_batch", "pkv_decode_attn_batch",
-    "pkv_decode_attn_batch_fp8", "pkv_cache_quantize_fp8",
+    "pkv_decode_attn_batch_fp8", "pkv_cache_quantize_fp8", "pkv_decode_attn_batch_gqa", "pkv_decode_attn_batch_gqa_fp8",
+    "pkv_evict_pooled_kv_offset",
 ]
+FLAG_GQA_SHARED = 128          # pkv_evict_desc.flags: one compacted cache per KV head
 
 
 class EvictDesc(C.Structure):
@@ -102,6 +104,8 @@ def lib() -> C.CDLL:
     L.pkv_evict_workspace_layout.restype = i32
     L.pkv_evict_workspace_bytes.argtypes = [C.POINTER(EvictDesc)]
     L.pkv_evict_workspace_bytes.restype = u64
+    L.pkv_evict_pooled_kv_offset.argtypes = [C.POINTER(EvictDesc), C.POINTER(u64)]
+    L.pkv_evict_pooled_kv_offset.restype = i32
     for name in ("pkv_evict_prefill", "pkv_stage_scores", "pkv_stage_pool", "pkv_stage_topk", "pkv_stage_gather", "pkv_stage_scan_pool"):
         fn = getattr(L, name)
         fn.argtypes = [C.POINTER(EvictDesc), p]
@@ -138,6 +142,10 @@ def lib() -> C.CDLL:
     L.pkv_decode_attn_batch.restype = i32
     L.pkv_decode_attn_batch_fp8.argtypes = [C.POINTER(DecodeDesc), C.c_int32, i64, p, p, i64, p, p, i64, i64, p]
     L.pkv_decode_attn_batch_fp8.restype = i32
+    L.pkv_decode_attn_batch_gqa.argtypes = [C.POINTER(DecodeDesc), C.c_int32, i64, p, p, i64, p]
+    L.pkv_decode_attn_batch_gqa.restype = i32
+    L.pkv_decode_attn_batch_gqa_fp8.argtypes = [C.POINTER(DecodeDesc), C.c_int32, i64, p, p, i64, p, p, i64, i64, p]
+    L.pkv_decode_attn_batch_gqa_fp8.restype = i32
     # tables: src / dst / scales [2*layers] pointers, capacities and rows [layers] int64, rows_dev [layers] pointers or NULL
     L.pkv_cache_quantize_fp8.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p, p, p, p, p, p, p, p]
     L.pkv_cache_quantize_fp8.restype = i32

@@ -22,8 +22,8 @@ from typing import Callable, Optional
 import torch
 from transformers.modeling_utils import ALL_ATTENTION_FUNCTIONS
 
-from .cache import (PkvBatchCacheLayer, PkvCacheLayer, PkvFp8CacheLayer, PkvRaggedCacheLayer, install_layer, kv_cache_dtype,
-                    layer_is_empty, quantize_caches_fp8)
+from .cache import (PkvBatchCacheLayer, PkvCacheLayer, PkvFp8CacheLayer, PkvRaggedCacheLayer, gqa_shared, install_layer,
+                    kv_cache_dtype, layer_is_empty, quantize_caches_fp8)
 from .kv_cluster import INIT_BY_METHOD, flush_pending
 
 DEFAULT_DECODE_RESERVE = 256   # rows of head-room behind the compacted prompt (grows by doubling)
@@ -111,6 +111,10 @@ def make_forward(method: str, modeling, original_forward):
                                                          attention_mask, **kwargs)
             cluster.inputs_ready = True      # the launch in front of the eviction is the dense attention: it only reads q / k / v
             reserve = int(getattr(self.config, "pkv_decode_reserve", DEFAULT_DECODE_RESERVE))
+            group = num_q_heads // key_states.shape[1] if gqa_shared(self.config) else 1
+            if group > 1 and getattr(cluster, "ragged", False):
+                raise NotImplementedError(f"pkv_gqa_shared: {method} sets a budget per QUERY head, which one cache per KV head "
+                                          "cannot hold (AdaKV / HeadKV with per-KV-head budgets are not built)")
             if getattr(cluster, "ragged", False) and cluster.compressed(q_len):
                 # AdaKV / HeadKV (llama_model.py:2317-2320): per-head budgets -> padded buffers + per-head row counts
                 if bsz != 1:
@@ -129,7 +133,8 @@ def make_forward(method: str, modeling, original_forward):
                 pending = getattr(past_key_values, "_pkv_pending", None)
                 if pending is None:
                     pending = past_key_values._pkv_pending = []
-            bufs = [cluster.evict_into(query_states[b], key_states[b], value_states[b], reserve=reserve, pending=pending) for b in range(bsz)]
+            bufs = [cluster.evict_into(query_states[b], key_states[b], value_states[b], reserve=reserve, pending=pending,
+                                       **({"gqa_shared": True} if group > 1 else {})) for b in range(bsz)]
             if pending and self.layer_idx == last_layer_idx(self):
                 flush_pending(pending, cluster.backend)
             rows = bufs[0][2]
@@ -137,7 +142,12 @@ def make_forward(method: str, modeling, original_forward):
                 k_buf, v_buf = bufs[0][0][None], bufs[0][1][None]
             else:
                 k_buf, v_buf = torch.stack([t[0] for t in bufs]), torch.stack([t[1] for t in bufs])
-            install_layer(past_key_values, self.layer_idx, PkvCacheLayer(k_buf, v_buf, rows, seen_tokens=q_len))
+            if group > 1:
+                # knob pkv_gqa_shared: one cache per KV head, held in the per-(sequence, head) row-count form
+                layer = PkvBatchCacheLayer(k_buf, v_buf, [[rows] * k_buf.shape[1]] * bsz, [q_len] * bsz, group=group)
+            else:
+                layer = PkvCacheLayer(k_buf, v_buf, rows, seen_tokens=q_len)
+            install_layer(past_key_values, self.layer_idx, layer)
             _maybe_quantize(self, past_key_values, cluster)
         else:
             # ---------------- decode (llama_model.py:169-170) ----------------
@@ -155,7 +165,23 @@ def make_forward(method: str, modeling, original_forward):
             # rows = `rows_arg` (+ head_rows[h] for ragged caches, + the device step counter in static mode)
             rows_arg = (layer.appended if ragged else layer.length) + 1
             head_rows = {"head_rows": layer.head_rows} if ragged else {}
-            if q_len == 1 and isinstance(layer, PkvFp8CacheLayer):
+            if q_len == 1 and getattr(layer, "group", 1) > 1:
+                # GQA-shared cache (knob pkv_gqa_shared): one launch for any batch size, host-launched or in the static loop's
+                # graph; each KV head's rows are read once for its group; rows = layer.rows[b, j] + 1 (+ the step counter)
+                if static is None:
+                    layer.reserve(1)
+                kw = dict(rows=layer.rows, step=static.step if static is not None else None, max_length=layer.capacity,
+                          workspace=static.workspace if static is not None else None, softmax_scale=self.scaling)
+                q1, k1, v1 = query_states[:, :, 0, :], key_states[:, :, 0, :], value_states[:, :, 0, :]
+                if isinstance(layer, PkvFp8CacheLayer):
+                    out = cluster.backend.decode_attn_batch_gqa_fp8(q1, layer.k_buf, layer.v_buf, layer.k_scale, layer.v_scale, 1,
+                                                                    k1, v1, **kw)
+                else:
+                    out = cluster.backend.decode_attn_batch_gqa(q1, layer.k_buf, layer.v_buf, 1, k1, v1, **kw)
+                if static is None:
+                    layer.advance(1)
+                attn_output = out[:, None]
+            elif q_len == 1 and isinstance(layer, PkvFp8CacheLayer):
                 # FP8 cache (knob pkv_kv_cache_dtype): one launch for any batch size, host-launched or in the static loop's
                 # graph; rows = layer.rows[b, h] + 1 (+ the device step counter in static mode). The kernel quantises the new
                 # K / V row and attends it as stored.

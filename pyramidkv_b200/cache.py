@@ -141,14 +141,23 @@ class PkvBatchCacheLayer(PkvCacheLayer):
     every row; AdaKV / HeadKV heads differ) and `rows` the same counts on the device (int32 [B*Hq], what
     `pkv_decode_attn_batch` adds to its row count). Decode appends one row to every sequence per step; `settle` books the
     rows each sequence really kept (a sequence that stopped at its EOS keeps fewer). `length` is the longest (sequence,
-    head)'s row count (what the buffers must hold); `seq_seen[b]` the tokens sequence b has seen."""
+    head)'s row count (what the buffers must hold); `seq_seen[b]` the tokens sequence b has seen.
 
-    def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, rows_host, seq_seen):
+    `group` G > 1: a GQA-shared cache (knob `pkv_gqa_shared`): one cache per KV head, [B, Hkv, capacity, D], read once for
+    the G query heads of its group (`pkv_decode_attn_batch_gqa`); `rows_host[b][j]` counts KV head j's rows. G = 1 (the
+    default) is the per-query-head cache."""
+
+    def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, rows_host, seq_seen, group: int = 1):
+        self.group = int(group)
         self.rows_host = [[int(r) for r in row] for row in rows_host]
         self.seq_seen = [int(s) for s in seq_seen]
         assert len(self.rows_host) == len(self.seq_seen) == k_buf.shape[0] and all(len(r) == k_buf.shape[1] for r in self.rows_host)
         self.rows = self._device_rows(k_buf.device)
         super().__init__(k_buf, v_buf, max(max(r) for r in self.rows_host), max(self.seq_seen))
+
+    @property
+    def num_q_heads(self) -> int:
+        return self.k_buf.shape[1] * self.group
 
     def _device_rows(self, device) -> torch.Tensor:
         return torch.tensor([r for row in self.rows_host for r in row], dtype=torch.int32, device=device)
@@ -195,6 +204,14 @@ def kv_cache_dtype(config) -> Optional[str]:
     return v
 
 
+def gqa_shared(config) -> bool:
+    """The knob `pkv_gqa_shared` of a model config (default False): one selection and one compacted cache per KV head."""
+    v = getattr(config, "pkv_gqa_shared", False)
+    if v not in (False, True, None, 0, 1):
+        raise ValueError(f"pkv_gqa_shared={v!r}: expected True or False")
+    return bool(v)
+
+
 class PkvFp8CacheLayer(PkvBatchCacheLayer):
     """The compacted cache in FP8 (knob `pkv_kv_cache_dtype = "fp8_e4m3"`): `k_buf` / `v_buf` hold E4M3 bytes
     (torch.float8_e4m3fn [B, Hq, capacity, D]) and `k_scale` / `v_scale` one fp32 scale per (sequence, head, row)
@@ -204,10 +221,11 @@ class PkvFp8CacheLayer(PkvBatchCacheLayer):
     prompt, an equal-length batch, AdaKV / HeadKV heads of different lengths and joined prompts. Decode appends one
     quantised row per sequence and step (`pkv_decode_attn_batch_fp8`)."""
 
-    def __init__(self, k_q: torch.Tensor, v_q: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor, rows_host, seq_seen):
+    def __init__(self, k_q: torch.Tensor, v_q: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor, rows_host, seq_seen,
+                 group: int = 1):
         assert k_q.dtype == torch.float8_e4m3fn and k_scale.shape == k_q.shape[:3] and v_scale.shape == k_scale.shape
         self.k_scale, self.v_scale = k_scale, v_scale
-        super().__init__(k_q, v_q, rows_host, seq_seen)
+        super().__init__(k_q, v_q, rows_host, seq_seen, group)
 
     def reserve(self, extra_rows: int) -> None:
         need = self.length + extra_rows
@@ -251,12 +269,24 @@ class PkvFp8CacheLayer(PkvBatchCacheLayer):
 
 
 def quantize_caches_fp8(past_key_values, backend) -> int:
-    """Convert every compacted layer of `past_key_values` (`PkvCacheLayer` / `PkvRaggedCacheLayer`, filled by the patched
-    prefill) to a `PkvFp8CacheLayer` with ONE backend call (`pkv_cache_quantize_fp8`: one launch per 32 layers) and drop
-    the 16-bit buffers. The FP8 buffers keep each layer's capacity (the decode head-room included). Returns the number of
-    layers converted."""
+    """Convert every compacted layer of `past_key_values` (`PkvCacheLayer` / `PkvRaggedCacheLayer`, or a GQA-shared
+    `PkvBatchCacheLayer`, filled by the patched prefill) to a `PkvFp8CacheLayer` with ONE backend call
+    (`pkv_cache_quantize_fp8`: one launch per 32 layers; a GQA-shared cache converts its Hkv heads) and drop the 16-bit
+    buffers. The FP8 buffers keep each layer's capacity (the decode head-room included). Returns the number of layers
+    converted."""
     idx, items, metas = [], [], []
     for i, l in enumerate(past_key_values.layers):
+        if isinstance(l, PkvBatchCacheLayer) and l.group > 1 and not isinstance(l, PkvFp8CacheLayer):
+            B, H, cap, D = l.k_buf.shape
+            kq = torch.empty(B, H, cap, D, dtype=torch.float8_e4m3fn, device=l.device)
+            vq = torch.empty_like(kq)
+            ks = torch.empty(B, H, cap, dtype=torch.float32, device=l.device)
+            vs = torch.empty_like(ks)
+            uniform = all(r == l.length for row in l.rows_host for r in row)
+            items.append((l.k_buf, l.v_buf, kq, vq, ks, vs, l.length, None if uniform else l.rows))
+            metas.append((kq, vq, ks, vs, l.rows_host, l.seq_seen, l.group))
+            idx.append(i)
+            continue
         if not isinstance(l, PkvCacheLayer) or isinstance(l, PkvBatchCacheLayer):
             continue
         B, Hq, cap, D = l.k_buf.shape
@@ -290,6 +320,7 @@ def _join_fp8(caches, reserve: int):
             raise ValueError(f"join_caches: layer {i}: head counts, head_dim or device differ between the caches")
         rows = [list(l.rows_host[0]) for l in src]
         cap = max(max(r) for r in rows) + int(reserve)
+        group = src[0].group
         k = torch.empty(len(src), hq, cap, d, dtype=torch.float8_e4m3fn, device=src[0].device)
         v = torch.empty_like(k)
         ks = torch.empty(len(src), hq, cap, dtype=torch.float32, device=src[0].device)
@@ -298,7 +329,7 @@ def _join_fp8(caches, reserve: int):
             n = l.length
             k[b, :, :n], v[b, :, :n] = l.k_buf[0, :, :n], l.v_buf[0, :, :n]
             ks[b, :, :n], vs[b, :, :n] = l.k_scale[0, :, :n], l.v_scale[0, :, :n]
-        out.layers.append(PkvFp8CacheLayer(k, v, ks, vs, rows, [l.seq_seen[0] for l in src]))
+        out.layers.append(PkvFp8CacheLayer(k, v, ks, vs, rows, [l.seq_seen[0] for l in src], group))
     return out
 
 
@@ -307,11 +338,15 @@ def join_caches(caches, reserve: int = 0):
     `PkvRaggedCacheLayer`): layer by layer the valid rows are copied once into [B, Hq, longest + reserve, D] buffers
     (`PkvBatchCacheLayer`). A cache may be passed several times. Stock / FullKV caches raise. Single-prompt FP8 caches
     (`PkvFp8CacheLayer`) join the same way, bytes and scales copied once, into a `PkvFp8CacheLayer`; FP8 and 16-bit
-    caches do not mix."""
+    caches do not mix. GQA-shared caches (knob `pkv_gqa_shared`, `group` > 1) join into a layer of the same group; caches of
+    different groups do not mix either."""
     from transformers import DynamicCache
     if not caches:
         raise ValueError("join_caches: no caches")
     n_layers = len(caches[0].layers)
+    if len({getattr(l, "group", 1) for c in caches for l in c.layers}) > 1:
+        raise ValueError("join_caches: GQA-shared and per-query-head caches (or caches of different groups) cannot be joined "
+                         "together (set pkv_gqa_shared the same for every prompt)")
     fp8 = [isinstance(l, PkvFp8CacheLayer) for c in caches for l in c.layers]
     if any(fp8):
         if not all(fp8) or any(len(c.layers) != n_layers for c in caches):
@@ -320,8 +355,10 @@ def join_caches(caches, reserve: int = 0):
         if any(l.k_buf.shape[0] != 1 for c in caches for l in c.layers):
             raise ValueError("join_caches joins single-prompt (batch 1) caches")
         return _join_fp8(caches, reserve)
+    group = getattr(caches[0].layers[0], "group", 1) if n_layers else 1
+    single = (lambda l: isinstance(l, PkvBatchCacheLayer)) if group > 1 else (lambda l: not isinstance(l, PkvBatchCacheLayer))
     for c in caches:
-        if len(c.layers) != n_layers or not all(isinstance(l, PkvCacheLayer) and not isinstance(l, PkvBatchCacheLayer) for l in c.layers):
+        if len(c.layers) != n_layers or not all(isinstance(l, PkvCacheLayer) and single(l) for l in c.layers):
             raise RuntimeError("join_caches needs caches prefilled by the patched forward on every layer "
                                "(method 'fullkv' and stock caches are not compacted)")
         if any(l.k_buf.shape[0] != 1 for l in c.layers):
@@ -334,6 +371,8 @@ def join_caches(caches, reserve: int = 0):
         for l in src:
             if isinstance(l, PkvRaggedCacheLayer):
                 rows.append([r + l.appended for r in l.head_rows_host])
+            elif group > 1:
+                rows.append(list(l.rows_host[0]))
             else:
                 rows.append([l.length] * l.k_buf.shape[1])
         _, hq, _, d = src[0].k_buf.shape
@@ -345,7 +384,7 @@ def join_caches(caches, reserve: int = 0):
         for b, l in enumerate(src):
             k[b, :, : l.length] = l.k_buf[0, :, : l.length]
             v[b, :, : l.length] = l.v_buf[0, :, : l.length]
-        out.layers.append(PkvBatchCacheLayer(k, v, rows, [l.seen_tokens for l in src]))
+        out.layers.append(PkvBatchCacheLayer(k, v, rows, [l.seen_tokens for l in src], group))
     return out
 
 

@@ -70,13 +70,29 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 
 static bool is_window_method(int m) { return m == PKV_PYRAMIDKV || m == PKV_SNAPKV; }
 
-// Shape-only validation + layout (no device access): shared by the workspace queries and the launches.
-static int compute_layout(const pkv_evict_desc* d, pkv_ws_layout* L) {
+// PKV_FLAG_GQA_SHARED: the selection stages seen as Hkv "heads" with G = 1 — top-k over the group-reduced scores, the gather
+// writing KV head j's cache from K[j] / V[j]. (The caller's cache is [Hkv, capacity, D].)
+static EvictArgs kv_view(const EvictArgs& a) {
+    EvictArgs b = a;
+    b.Hq = a.Hkv;
+    b.G = 1;
+    b.ws.nw = a.W;
+    b.ws.pooled_off = a.pooled_kv_off;
+    b.gqa_shared = false;
+    return b;
+}
+
+// Shape-only validation + layout (no device access): shared by the workspace queries and the launches. *pooled_kv_off: the
+// PKV_FLAG_GQA_SHARED segment (0 without the flag or for StreamingLLM).
+static int compute_layout(const pkv_evict_desc* d, pkv_ws_layout* L, uint64_t* pooled_kv_off = nullptr) {
     if (!d) return fail(PKV_ERR_INVALID_ARG, "null descriptor");
     if (d->struct_bytes != sizeof(pkv_evict_desc))
         return fail(PKV_ERR_INVALID_ARG, "pkv_evict_desc.struct_bytes=%u, library expects %zu (ABI mismatch)", d->struct_bytes, sizeof(pkv_evict_desc));
     if (d->dtype != PKV_BF16 && d->dtype != PKV_FP16) return fail(PKV_ERR_UNSUPPORTED_DTYPE, "dtype %d: only bf16 (0) and fp16 (1) are supported", d->dtype);
     if (d->method < PKV_PYRAMIDKV || d->method > PKV_L2NORM) return fail(PKV_ERR_INVALID_ARG, "unknown method %d", d->method);
+    if (d->flags & ~PKV_EVICT_KNOWN_FLAGS) return fail(PKV_ERR_INVALID_ARG, "unknown pkv_evict_desc.flags bits 0x%x", d->flags & ~PKV_EVICT_KNOWN_FLAGS);
+    if ((d->flags & PKV_FLAG_GQA_SHARED) && (d->flags & (PKV_FLAG_FUSED | PKV_FLAG_SINGLE_LAUNCH)))
+        return fail(PKV_ERR_UNSUPPORTED, "PKV_FLAG_GQA_SHARED runs the staged kernels: PKV_FLAG_FUSED / PKV_FLAG_SINGLE_LAUNCH are not built with it");
     if (d->num_q_heads <= 0 || d->num_kv_heads <= 0 || d->num_q_heads % d->num_kv_heads)
         return fail(PKV_ERR_INVALID_ARG, "num_q_heads=%d must be a positive multiple of num_kv_heads=%d", d->num_q_heads, d->num_kv_heads);
     if (d->head_dim != 64 && d->head_dim != 128) return fail(PKV_ERR_UNSUPPORTED, "head_dim=%d: only 64 and 128 are built", d->head_dim);
@@ -115,13 +131,18 @@ static int compute_layout(const pkv_evict_desc* d, pkv_ws_layout* L) {
         L->h2o_acc_off = L->h2o_stats_off;  // column sums are accumulated in registers; no extra segment
         seg(uint64_t(d->num_q_heads) * uint64_t(L->s_pad) * sizeof(float4));   // stats4 of the wgmma kernels: h2o_stats4_offset()
     }
+    uint64_t kv_off = 0;
+    if ((d->flags & PKV_FLAG_GQA_SHARED) && d->method != PKV_STREAMINGLLM)
+        kv_off = (G > 1 && d->method != PKV_L2NORM) ? seg(uint64_t(d->num_kv_heads) * uint64_t(L->pooled_pitch) * 2) : L->pooled_off;
+    if (pooled_kv_off) *pooled_kv_off = kv_off;
     L->total_bytes = off > 0 ? off : 256;
     return PKV_OK;
 }
 
 static int resolve(const pkv_evict_desc* d, EvictArgs* a) {
     pkv_ws_layout L;
-    int rc = compute_layout(d, &L);
+    uint64_t kv_off = 0;
+    int rc = compute_layout(d, &L, &kv_off);
     if (rc) return rc;
     const DevInfo* di = nullptr;
     rc = device_info(d->device, &di);
@@ -150,6 +171,8 @@ static int resolve(const pkv_evict_desc* d, EvictArgs* a) {
     a->ws = L; a->ws_base = static_cast<uint8_t*>(d->workspace);
     a->flags = d->flags; a->device = d->device; a->num_sms = di->sms;
     a->window_mean = (d->flags & PKV_FLAG_WINDOW_MEAN) != 0;
+    a->gqa_shared = (d->flags & PKV_FLAG_GQA_SHARED) != 0 && a->G > 1;
+    a->pooled_kv_off = kv_off;
     if (a->window_mean && (!is_window_method(a->method) || (a->W & (a->W - 1)) != 0))
         return fail(PKV_ERR_UNSUPPORTED, "PKV_FLAG_WINDOW_MEAN needs a window method and a power-of-two window_size (got %d)", a->W);
     // which stage-1 kernel runs is a pure function of the descriptor (stage 2 must read the partials it wrote)
@@ -162,7 +185,7 @@ static int resolve(const pkv_evict_desc* d, EvictArgs* a) {
     }
     if (a->method != PKV_STREAMINGLLM) {
         const char* why = nullptr;
-        if (!topk_supported(*a, &why)) return fail(PKV_ERR_UNSUPPORTED, "%s", why);
+        if (!topk_supported(a->gqa_shared ? kv_view(*a) : *a, &why)) return fail(PKV_ERR_UNSUPPORTED, "%s", why);
     }
     return PKV_OK;
 }
@@ -176,6 +199,7 @@ static bool h2o_use_tc5() {
 }
 
 static int run_scores(const EvictArgs& a, cudaStream_t st) {
+    if (a.gqa_shared && a.method == PKV_L2NORM) return run_scores(kv_view(a), st);   // the key norms of each KV head, once
     cudaError_t e = cudaSuccess;
     if (a.method == PKV_H2O) e = (h2o_use_tc5() && h2o_tc5_supported(a)) ? launch_h2o_tc5_rowstats(a, st) : launch_h2o_rowstats(a, st);
     else if (a.method == PKV_L2NORM) e = launch_l2norm_scores(a, st);
@@ -186,15 +210,16 @@ static int run_pool(const EvictArgs& a, cudaStream_t st) {
     cudaError_t e = cudaSuccess;
     if (a.method == PKV_H2O) e = (h2o_use_tc5() && h2o_tc5_supported(a)) ? launch_h2o_tc5_colsum(a, st) : launch_h2o_colsum(a, st);
     else if (is_window_method(a.method)) e = launch_softmax_pool(a, st);
+    if (e == cudaSuccess && a.gqa_shared && (a.method == PKV_H2O || is_window_method(a.method))) e = launch_group_reduce(a, st);
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "pool launch");
 }
 static int run_topk(const EvictArgs& a, cudaStream_t st) {
     if (a.method == PKV_STREAMINGLLM) return PKV_OK;
-    const cudaError_t e = launch_topk(a, st);
+    const cudaError_t e = launch_topk(a.gqa_shared ? kv_view(a) : a, st);
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "topk launch");
 }
 static int run_gather(const EvictArgs& a, cudaStream_t st) {
-    const cudaError_t e = launch_gather(a, st);
+    const cudaError_t e = launch_gather(a.gqa_shared ? kv_view(a) : a, st);
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "gather launch");
 }
 
@@ -265,6 +290,18 @@ uint64_t pkv_evict_workspace_bytes(const pkv_evict_desc* d) {
     return compute_layout(d, &L) == PKV_OK ? L.total_bytes : 0;
 }
 
+int pkv_evict_pooled_kv_offset(const pkv_evict_desc* d, uint64_t* off_out) {
+    if (!off_out) return fail(PKV_ERR_INVALID_ARG, "null output pointer");
+    pkv_ws_layout L;
+    uint64_t off = 0;
+    const int rc = compute_layout(d, &L, &off);
+    if (rc) return rc;
+    if (!(d->flags & PKV_FLAG_GQA_SHARED) || d->method == PKV_STREAMINGLLM)
+        return fail(PKV_ERR_INVALID_ARG, "pkv_evict_pooled_kv_offset: per-KV-head scores exist only with PKV_FLAG_GQA_SHARED and a scoring method");
+    *off_out = off;
+    return PKV_OK;
+}
+
 #define PKV_STAGE_PROLOGUE()                      \
     EvictArgs a;                                  \
     int rc = resolve(d, &a);                      \
@@ -277,7 +314,7 @@ uint64_t pkv_evict_workspace_bytes(const pkv_evict_desc* d) {
 // cooperative launch guarantees; they stay available (PKV_FLAG_FUSED / PKV_FLAG_SINGLE_LAUNCH, or PKV_ONEPASS=1 / 2 for A/B runs).
 static int fused_mode(const EvictArgs& a) {
     static const int env = []() { const char* e = getenv("PKV_ONEPASS"); return e ? atoi(e) : 0; }();
-    if ((a.flags & PKV_FLAG_STAGED) || a.score_impl != 1 || !evict_fused_supported(a)) return 0;
+    if ((a.flags & PKV_FLAG_STAGED) || a.gqa_shared || a.score_impl != 1 || !evict_fused_supported(a)) return 0;
     if (a.flags & PKV_FLAG_SINGLE_LAUNCH) return 2;
     if (a.flags & PKV_FLAG_FUSED) return 1;
     return env < 0 ? 0 : env > 2 ? 2 : env;
@@ -291,7 +328,7 @@ int pkv_evict_single_launch(const pkv_evict_desc* d) {
 
 int pkv_stage_scan_pool(const pkv_evict_desc* d, void* stream) {
     PKV_STAGE_PROLOGUE();
-    if ((a.flags & PKV_FLAG_STAGED) || a.score_impl != 1 || !evict_fused_supported(a))
+    if ((a.flags & PKV_FLAG_STAGED) || a.gqa_shared || a.score_impl != 1 || !evict_fused_supported(a))
         return fail(PKV_ERR_UNSUPPORTED, "pkv_stage_scan_pool: this shape runs as staged launches (pkv_stage_scores + pkv_stage_pool)");
     const cudaError_t e = launch_evict_fused(a, true, st);
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "fused scan+pool launch");
@@ -323,6 +360,18 @@ int pkv_evict_prefill(const pkv_evict_desc* d, void* stream) {
         return run_gather(a, st);
     }
     if ((rc = run_scores(a, st))) return rc;
+    if (a.gqa_shared) {
+        // scores and pool per query head, the group reduction, then select + gather per KV head (never pooling inside the select
+        // cluster: the reduction sits between the pool and the select)
+        if ((rc = run_pool(a, st))) return rc;
+        const EvictArgs b = kv_view(a);
+        if (a.method != PKV_STREAMINGLLM && fused > 0 && select_fused_supported(b, false)) {
+            const cudaError_t e = launch_select_fused(b, false, st);
+            return e == cudaSuccess ? PKV_OK : fail_cuda(e, "select launch");
+        }
+        if ((rc = run_topk(a, st))) return rc;
+        return run_gather(a, st);
+    }
     if (a.method != PKV_STREAMINGLLM && fused > 0) {
         // Pooling inside the select cluster saves one launch; it wins while the three kernels are launch-bound (short prompts)
         // and loses once the exp-heavy pool phase is big enough to want the whole-chip pool grid. PKV_FUSED=1 / 2 pin either form.
@@ -359,6 +408,7 @@ static int resolve_batch(const pkv_evict_desc* descs, int n, std::vector<EvictAr
         if (rc) return rc;
     }
     const EvictArgs& a = (*out)[0];
+    if (a.flags & PKV_FLAG_GQA_SHARED) return fail(PKV_ERR_UNSUPPORTED, "layer batch: not built for PKV_FLAG_GQA_SHARED (evict layer by layer)");
     if (!is_window_method(a.method) || a.window_mean || a.score_impl != 1)
         return fail(PKV_ERR_UNSUPPORTED, "layer batch: window methods (pyramidkv / snapkv) on the wgmma score kernel only");
     if (a.ws.s_pad / kTileTokens < 8) return fail(PKV_ERR_UNSUPPORTED, "layer batch: prompts of at least 897 tokens (8 K tiles per kv head)");
@@ -595,6 +645,62 @@ int pkv_decode_attn_batch_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "fp8 decode launch");
 }
 
+// GQA-shared caches: the checks of pkv_decode_attn_batch(_fp8) with KV-head strides; `elem` = bytes per cached element.
+static int resolve_decode_gqa(const char* fn, const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
+                              const int32_t* step_dev, int64_t max_length, int elem, DecodeArgs* a) {
+    if ((reinterpret_cast<uintptr_t>(rows) & 3u) || (reinterpret_cast<uintptr_t>(step_dev) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned int32 pointer", fn);
+    if (max_length < 1) return fail(PKV_ERR_INVALID_ARG, "%s: max_length must be >= 1", fn);
+    if (num_seqs < 1 || num_seqs > 65535) return fail(PKV_ERR_INVALID_ARG, "%s: num_seqs=%d outside [1, 65535]", fn, num_seqs);
+    int rc = resolve_decode(d, a, true, max_length, num_seqs);
+    if (rc) return rc;
+    if (a->G != 2 && a->G != 4 && a->G != 8)
+        return fail(PKV_ERR_UNSUPPORTED, "%s: group size num_q_heads/num_kv_heads = %d: the grouped kernels are built for 2, 4 and 8", fn, a->G);
+    const int64_t align = 16 / elem;   // cache strides in elements that keep every row 16-byte aligned
+    if (a->cache_sh % align) return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_h=%lld is not a multiple of 16 bytes", fn, (long long)a->cache_sh);
+    a->cache_sb = int64_t(a->Hkv) * a->cache_sh;
+    if (num_seqs > 1) {
+        if (cache_stride_b < a->cache_sb || cache_stride_b % align)
+            return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_b=%lld is below num_kv_heads*cache_stride_h=%lld or not a multiple of 16 bytes", fn,
+                        (long long)cache_stride_b, (long long)a->cache_sb);
+        a->cache_sb = cache_stride_b;
+    }
+    a->devlen = true;
+    a->rows = rows;
+    a->step_dev = step_dev;
+    return PKV_OK;
+}
+
+int pkv_decode_attn_batch_gqa(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
+                              const int32_t* step_dev, int64_t max_length, void* stream) {
+    DecodeArgs a;
+    const int rc = resolve_decode_gqa("pkv_decode_attn_batch_gqa", d, num_seqs, cache_stride_b, rows, step_dev, max_length, 2, &a);
+    if (rc) return rc;
+    DeviceGuard guard(d->device);
+    const cudaError_t e = launch_decode_gqa(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "grouped decode launch");
+}
+
+int pkv_decode_attn_batch_gqa_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
+                                  const int32_t* step_dev, int64_t max_length, float* k_scale, float* v_scale,
+                                  int64_t scale_stride_h, int64_t scale_stride_b, void* stream) {
+    const char* fn = "pkv_decode_attn_batch_gqa_fp8";
+    if (!k_scale || !v_scale) return fail(PKV_ERR_INVALID_ARG, "%s: null scale pointer", fn);
+    if ((reinterpret_cast<uintptr_t>(k_scale) & 3u) || (reinterpret_cast<uintptr_t>(v_scale) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned scale pointer", fn);
+    DecodeArgs a;
+    const int rc = resolve_decode_gqa(fn, d, num_seqs, cache_stride_b, rows, step_dev, max_length, 1, &a);
+    if (rc) return rc;
+    if (scale_stride_h < max_length || (num_seqs > 1 && scale_stride_b < int64_t(a.Hkv) * scale_stride_h))
+        return fail(PKV_ERR_INVALID_ARG, "%s: scale strides (%lld, %lld) hold fewer than max_length=%lld rows per KV head", fn,
+                    (long long)scale_stride_h, (long long)scale_stride_b, (long long)max_length);
+    a.k_scale = k_scale;
+    a.v_scale = v_scale;
+    a.scale_sh = scale_stride_h;
+    a.scale_sb = num_seqs > 1 ? scale_stride_b : int64_t(a.Hkv) * scale_stride_h;
+    DeviceGuard guard(d->device);
+    const cudaError_t e = launch_decode_gqa_fp8(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "grouped fp8 decode launch");
+}
+
 int pkv_cache_quantize_fp8(int32_t dtype, int32_t num_seqs, int32_t num_heads, int32_t head_dim, int32_t device, int32_t num_layers,
                            const void* const* src, void* const* dst, float* const* scales, const int64_t* src_capacity,
                            const int64_t* dst_capacity, const int64_t* rows, const int32_t* const* rows_dev, void* stream) {
@@ -683,6 +789,7 @@ int pkv_adakv_counts(const pkv_evict_desc* d, int64_t base_capacity, int32_t nor
                      int32_t* counts, void* stream) {
     PKV_STAGE_PROLOGUE();
     if (!is_window_method(a.method)) return fail(PKV_ERR_INVALID_ARG, "pkv_adakv_counts: the scores come from a window method (use PKV_SNAPKV)");
+    if (a.flags & PKV_FLAG_GQA_SHARED) return fail(PKV_ERR_UNSUPPORTED, "pkv_adakv_counts: per-query-head budgets are not built for PKV_FLAG_GQA_SHARED");
     if (!a.window_mean) return fail(PKV_ERR_INVALID_ARG, "pkv_adakv_counts: the scores must come from stage 2 with PKV_FLAG_WINDOW_MEAN (calcul_attn_sore averages the window rows)");
     if (base_capacity < 1 || base_capacity > a.n) return fail(PKV_ERR_INVALID_ARG, "base_capacity=%lld out of range [1, seq_len-window=%lld]", (long long)base_capacity, (long long)a.n);
     if (!scratch || !counts || scratch_bytes < adakv_scratch_bytes(a.Hq)) return fail(PKV_ERR_WORKSPACE, "pkv_adakv_counts: scratch of %zu bytes and a counts buffer are required", adakv_scratch_bytes(a.Hq));
@@ -694,6 +801,7 @@ int pkv_adakv_counts(const pkv_evict_desc* d, int64_t base_capacity, int32_t nor
 int pkv_ragged_place_window(const pkv_evict_desc* d, const int32_t* caps, void* stream) {
     PKV_STAGE_PROLOGUE();
     if (!caps) return fail(PKV_ERR_INVALID_ARG, "pkv_ragged_place_window: null caps");
+    if (a.flags & PKV_FLAG_GQA_SHARED) return fail(PKV_ERR_UNSUPPORTED, "pkv_ragged_place_window: per-query-head budgets are not built for PKV_FLAG_GQA_SHARED");
     const cudaError_t e = launch_ragged_window(a, caps, st);
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "ragged window launch");
 }

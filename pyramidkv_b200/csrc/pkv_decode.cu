@@ -25,6 +25,7 @@ struct DecodeParams {
     uint16_t *k_cache, *v_cache, *out;   // caches at + s*cache_sb + h*cache_sh; out [num_seqs][Hq][D]
     int64_t cache_sh, cache_sb, T, chunk, max_rows;
     int G, nsplit, num_sms;
+    int Hq;     // query heads per sequence (the grouped kernel's split rule; the per-head kernel reads gridDim.y)
     float scale;
     float* ws;  // [num_seqs*Hq][nsplit][2 + D] partial (m, l, acc) when nsplit > 1
     const int32_t* step_dev;  // DEVLEN kernels: rows = T + *step_dev (graph-replayable decode; the grid is sized for the maximum)
@@ -172,6 +173,145 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
     }
 }
 
+// decode_kernel<T, D, true> over a GQA-shared cache ([num_seqs][Hkv][capacity][D], rows[s*Hkv + j]): the CTA of (split, KV
+// head j, sequence) loads every row of its split once and runs, for each of the GH query heads h0..h0+GH-1 of the group, the
+// arithmetic decode_kernel runs for that head on the repeat-interleaved cache - the same rows per warp and lane group, the same
+// dot-product and online-softmax order, the same merges - so each head's output is bit-identical to it. The split count is
+// the per-query-head kernel's for Hq heads, and the partials are written per query head for decode_combine_kernel.
+// GH < G: the group is covered by G / GH CTAs (blockIdx.y = j * (G / GH) + part); part 0 appends the new row.
+template <typename T, int D, int GH>
+__global__ void __launch_bounds__(kDecodeThreads) decode_gqa_kernel(const DecodeParams p) {
+    constexpr int LPR = D / 8;
+    constexpr int RPW = 32 / LPR;
+    __shared__ float s_m[GH][kDecodeWarps], s_l[GH][kDecodeWarps];
+    __shared__ float s_acc[GH][kDecodeWarps][D];
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int parts = p.G / GH, split = blockIdx.x, j = blockIdx.y / parts, part = blockIdx.y % parts;
+    const int Hkv = p.Hq / p.G;
+    const int64_t sg = int64_t(blockIdx.z) * Hkv + j;                          // (sequence, kv head) index
+    const int64_t sh0 = int64_t(blockIdx.z) * p.Hq + int64_t(j) * p.G + part * GH;   // (sequence, first query head) index
+    const int sub = lane / LPR, piece = lane % LPR;
+    uint16_t* kc = p.k_cache + int64_t(blockIdx.z) * p.cache_sb + int64_t(j) * p.cache_sh;
+    uint16_t* vc = p.v_cache + int64_t(blockIdx.z) * p.cache_sb + int64_t(j) * p.cache_sh;
+    const uint16_t* k_new = p.k_new + sg * D;
+    const uint16_t* v_new = p.v_new + sg * D;
+    int64_t rows = p.T;
+    if (p.step_dev) rows += int64_t(__ldg(p.step_dev));
+    if (p.rows) rows += int64_t(__ldg(p.rows + sg));
+    if (rows < 1 || rows > p.max_rows) rows = 0;
+    const int64_t ns = min(int64_t(p.nsplit), splits_for(p.Hq, rows, p.num_sms));
+    const int64_t chunk = (rows + ns - 1) / ns;
+    const int64_t r_begin = int64_t(split) * chunk;
+    const int64_t r_end = min(rows, r_begin + chunk);
+    const bool has_new = p.k_new != nullptr;
+    const int64_t new_row = rows - 1;
+
+    // fused append, once per KV head
+    if (has_new && part == 0 && new_row >= r_begin && new_row < r_end && warp == 0 && lane < LPR) {
+        *reinterpret_cast<uint4*>(kc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(k_new + lane * 8);
+        *reinterpret_cast<uint4*>(vc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(v_new + lane * 8);
+    }
+
+    float qf[GH][8], m[GH], l[GH], acc[GH][8];
+#pragma unroll
+    for (int i = 0; i < GH; ++i) {
+        unpack8<T>(*reinterpret_cast<const uint4*>(p.q + (sh0 + i) * D + piece * 8), qf[i]);
+        m[i] = -INFINITY;
+        l[i] = 0.f;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[i][e] = 0.f;
+    }
+
+    for (int64_t rb = r_begin + warp * RPW; rb < r_end; rb += int64_t(kDecodeWarps) * RPW * kDecodeUnroll) {
+        uint4 kv[kDecodeUnroll], vv[kDecodeUnroll];
+        bool ok[kDecodeUnroll];
+#pragma unroll
+        for (int u = 0; u < kDecodeUnroll; ++u) {
+            const int64_t r = rb + sub + int64_t(u) * kDecodeWarps * RPW;
+            kv[u] = make_uint4(0, 0, 0, 0);
+            vv[u] = make_uint4(0, 0, 0, 0);
+            ok[u] = r < r_end;
+            if (ok[u]) {
+                const bool is_new = has_new && r == new_row;
+                const uint16_t* kr = is_new ? k_new : kc + r * D;
+                const uint16_t* vr = is_new ? v_new : vc + r * D;
+                kv[u] = *reinterpret_cast<const uint4*>(kr + piece * 8);
+                vv[u] = *reinterpret_cast<const uint4*>(vr + piece * 8);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < kDecodeUnroll; ++u) {
+            float kf[8], vf[8];
+            unpack8<T>(kv[u], kf);
+            unpack8<T>(vv[u], vf);
+#pragma unroll
+            for (int i = 0; i < GH; ++i) {
+                float dot = 0.f;
+#pragma unroll
+                for (int e = 0; e < 8; ++e) dot = fmaf(qf[i][e], kf[e], dot);
+#pragma unroll
+                for (int o = 1; o < LPR; o <<= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+                if (ok[u]) {
+                    // Explicit roundings: the forms the compiler picks for decode_kernel (with the G heads unrolled it may
+                    // contract a*b + c*d around the other product, or fuse dot * scale into s - mn), so the bits match it.
+                    const float s = __fmul_rn(dot, p.scale);
+                    const float mn = fmaxf(m[i], s);
+                    const float corr = expf(m[i] - mn), pe = expf(s - mn);
+                    l[i] = __fmaf_rn(l[i], corr, pe);
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) acc[i][e] = __fmaf_rn(acc[i][e], corr, __fmul_rn(pe, vf[e]));
+                    m[i] = mn;
+                }
+            }
+        }
+    }
+
+#pragma unroll
+    for (int i = 0; i < GH; ++i) {
+#pragma unroll
+        for (int o = LPR; o < 32; o <<= 1) {
+            const float m2 = __shfl_xor_sync(0xffffffffu, m[i], o);
+            const float l2 = __shfl_xor_sync(0xffffffffu, l[i], o);
+            const float mn = fmaxf(m[i], m2);
+            const float c1 = (mn == -INFINITY) ? 0.f : expf(m[i] - mn), c2 = (mn == -INFINITY) ? 0.f : expf(m2 - mn);
+            l[i] = __fmaf_rn(l[i], c1, __fmul_rn(l2, c2));
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const float a2 = __shfl_xor_sync(0xffffffffu, acc[i][e], o);
+                acc[i][e] = __fmaf_rn(acc[i][e], c1, __fmul_rn(a2, c2));
+            }
+            m[i] = mn;
+        }
+        if (sub == 0) {
+            if (piece == 0) { s_m[i][warp] = m[i]; s_l[i][warp] = l[i]; }
+#pragma unroll
+            for (int e = 0; e < 8; ++e) s_acc[i][warp][piece * 8 + e] = acc[i][e];
+        }
+    }
+    __syncthreads();
+    for (int x = tid; x < GH * D; x += kDecodeThreads) {
+        const int i = x / D, d = x % D;
+        float mn = -INFINITY;
+#pragma unroll
+        for (int w = 0; w < kDecodeWarps; ++w) mn = fmaxf(mn, s_m[i][w]);
+        float lt = 0.f, at = 0.f;
+#pragma unroll
+        for (int w = 0; w < kDecodeWarps; ++w) {
+            const float c = (s_m[i][w] == -INFINITY) ? 0.f : expf(s_m[i][w] - mn);
+            lt += s_l[i][w] * c;
+            at += s_acc[i][w][d] * c;
+        }
+        if (p.nsplit == 1) {
+            p.out[(sh0 + i) * D + d] = DT<T>::from_f32(at / lt);
+        } else {
+            float* w = p.ws + ((sh0 + i) * p.nsplit + split) * (2 + D);
+            if (d == 0) { w[0] = mn; w[1] = lt; }
+            w[2 + d] = at;
+        }
+    }
+}
+
 template <typename T, int D>
 __global__ void decode_combine_kernel(const DecodeParams p) {   // one CTA per (sequence, head)
     const int64_t h = blockIdx.x;
@@ -207,6 +347,7 @@ DecodeParams make_params(const DecodeArgs& a) {
     p.k_cache = a.k_cache; p.v_cache = a.v_cache; p.out = a.out;
     p.cache_sh = a.cache_sh; p.cache_sb = a.cache_sb; p.T = a.T; p.max_rows = a.max_rows;
     p.G = a.G; p.nsplit = a.nsplit; p.num_sms = a.num_sms;
+    p.Hq = a.Hq;
     p.chunk = (a.T + a.nsplit - 1) / a.nsplit;
     p.scale = a.scale;
     p.ws = a.ws;
@@ -229,7 +370,25 @@ cudaError_t launch_decode_t(const DecodeArgs& a, cudaStream_t st) {
     return cudaGetLastError();
 }
 
+template <typename T, int D>
+cudaError_t launch_decode_gqa_t(const DecodeArgs& a, cudaStream_t st) {
+    const DecodeParams p = make_params(a);
+    const dim3 grid(unsigned(a.nsplit), unsigned(a.Hkv), unsigned(a.num_seqs));
+    if (a.G == 2) decode_gqa_kernel<T, D, 2><<<grid, kDecodeThreads, 0, st>>>(p);
+    else if (a.G == 4) decode_gqa_kernel<T, D, 4><<<grid, kDecodeThreads, 0, st>>>(p);
+    else decode_gqa_kernel<T, D, 8><<<grid, kDecodeThreads, 0, st>>>(p);
+    count_launch();
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess || a.nsplit == 1) return e;
+    return launch_decode_combine(a, st);
+}
+
 }  // namespace
+
+cudaError_t launch_decode_gqa(const DecodeArgs& a, cudaStream_t st) {
+    if (a.dtype == PKV_BF16) return a.D == 128 ? launch_decode_gqa_t<__nv_bfloat16, 128>(a, st) : launch_decode_gqa_t<__nv_bfloat16, 64>(a, st);
+    return a.D == 128 ? launch_decode_gqa_t<__half, 128>(a, st) : launch_decode_gqa_t<__half, 64>(a, st);
+}
 
 int decode_num_splits(int Hq, int64_t T, int num_sms) { return int(splits_for(Hq, T, num_sms)); }
 

@@ -137,6 +137,7 @@ struct Fp8DecodeParams {
     float *k_scale, *v_scale;            // at + s*scale_sb + h*scale_sh
     int64_t cache_sh, cache_sb, scale_sh, scale_sb, T, max_rows;
     int G, nsplit, num_sms;
+    int Hq;   // query heads per sequence (the grouped kernel's split rule)
     float scale;
     float* ws;
     const int32_t* step_dev;
@@ -294,6 +295,168 @@ __global__ void __launch_bounds__(kThreads) decode_fp8_kernel(const Fp8DecodePar
     }
 }
 
+// decode_fp8_kernel over a GQA-shared FP8 cache ([num_seqs][Hkv][capacity][D] bytes, [num_seqs][Hkv][capacity] scales, rows
+// [s*Hkv + j]): the CTA of (split, KV head j, sequence) loads every row of its split once and runs, for each of the GH query
+// heads of the group it covers, the arithmetic decode_fp8_kernel runs for that head on the repeat-interleaved cache, so each
+// head's output is bit-identical to it. GH < G (G = 8: GH = 4, the registers of eight heads do not fit): G / GH CTAs per group,
+// blockIdx.y = j * (G / GH) + part. Every part quantises the new row into shared memory; part 0 stores it.
+template <typename T, int D, int GH>
+__global__ void __launch_bounds__(kThreads) decode_gqa_fp8_kernel(const Fp8DecodeParams p) {
+    constexpr int LPR = D / 16;
+    constexpr int RPW = 32 / LPR;
+    __shared__ float s_m[GH][kWarps], s_l[GH][kWarps];
+    __shared__ float s_acc[GH][kWarps][D];
+    __shared__ uint4 s_new[2][LPR];
+    __shared__ float s_new_scale[2];
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int parts = p.G / GH, split = blockIdx.x, j = blockIdx.y / parts, part = blockIdx.y % parts;
+    const int Hkv = p.Hq / p.G;
+    const int64_t sg = int64_t(blockIdx.z) * Hkv + j;
+    const int64_t sh0 = int64_t(blockIdx.z) * p.Hq + int64_t(j) * p.G + part * GH;
+    const int sub = lane / LPR, piece = lane % LPR;
+    uint8_t* kc = p.k_cache + int64_t(blockIdx.z) * p.cache_sb + int64_t(j) * p.cache_sh;
+    uint8_t* vc = p.v_cache + int64_t(blockIdx.z) * p.cache_sb + int64_t(j) * p.cache_sh;
+    float* ksc = p.k_scale + int64_t(blockIdx.z) * p.scale_sb + int64_t(j) * p.scale_sh;
+    float* vsc = p.v_scale + int64_t(blockIdx.z) * p.scale_sb + int64_t(j) * p.scale_sh;
+    int64_t rows = p.T;
+    if (p.step_dev) rows += int64_t(__ldg(p.step_dev));
+    if (p.rows) rows += int64_t(__ldg(p.rows + sg));
+    if (rows < 1 || rows > p.max_rows) rows = 0;
+    const int64_t ns = min(int64_t(p.nsplit), decode_splits_for(p.Hq, rows, p.num_sms));
+    const int64_t chunk = (rows + ns - 1) / ns;
+    const int64_t r_begin = int64_t(split) * chunk;
+    const int64_t r_end = min(rows, r_begin + chunk);
+    const int64_t new_row = rows - 1;
+    const bool own_new = p.k_new != nullptr && new_row >= r_begin && new_row < r_end;
+
+    if (own_new && warp == 0) {
+        const int which = sub & 1;
+        float x[16];
+        load16<T>((which ? p.v_new : p.k_new) + sg * D + piece * 16, x);
+        const float amax = row_amax<LPR>(x);
+        float s;
+        const uint4 qv = quantize16(x, amax, s);
+        if (sub < 2) {
+            if (part == 0) *reinterpret_cast<uint4*>((which ? vc : kc) + new_row * D + piece * 16) = qv;
+            s_new[which][piece] = qv;
+            if (piece == 0) {
+                if (part == 0) (which ? vsc : ksc)[new_row] = s;
+                s_new_scale[which] = s;
+            }
+        }
+    }
+    __syncthreads();
+
+    float qf[GH][16], m[GH], l[GH], acc[GH][16];
+#pragma unroll
+    for (int i = 0; i < GH; ++i) {
+        load16<T>(p.q + (sh0 + i) * D + piece * 16, qf[i]);
+        m[i] = -INFINITY;
+        l[i] = 0.f;
+#pragma unroll
+        for (int e = 0; e < 16; ++e) acc[i][e] = 0.f;
+    }
+
+    for (int64_t rb = r_begin + warp * RPW; rb < r_end; rb += int64_t(kWarps) * RPW * kUnroll) {
+        uint4 kv[kUnroll], vv[kUnroll];
+        float ks[kUnroll], vs[kUnroll];
+        bool ok[kUnroll];
+#pragma unroll
+        for (int u = 0; u < kUnroll; ++u) {
+            const int64_t r = rb + sub + int64_t(u) * kWarps * RPW;
+            kv[u] = make_uint4(0, 0, 0, 0);
+            vv[u] = make_uint4(0, 0, 0, 0);
+            ks[u] = vs[u] = 0.f;
+            ok[u] = r < r_end;
+            if (ok[u]) {
+                if (own_new && r == new_row) {
+                    kv[u] = s_new[0][piece];
+                    vv[u] = s_new[1][piece];
+                    ks[u] = s_new_scale[0];
+                    vs[u] = s_new_scale[1];
+                } else {
+                    kv[u] = *reinterpret_cast<const uint4*>(kc + r * D + piece * 16);
+                    vv[u] = *reinterpret_cast<const uint4*>(vc + r * D + piece * 16);
+                    ks[u] = ksc[r];
+                    vs[u] = vsc[r];
+                }
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < kUnroll; ++u) {
+            float kf[16];
+            fp8x16_to_f32(kv[u], kf);
+            float vf[16];
+            fp8x16_to_f32(vv[u], vf);
+#pragma unroll
+            for (int i = 0; i < GH; ++i) {
+                float dot = 0.f;
+#pragma unroll
+                for (int e = 0; e < 16; ++e) dot = fmaf(qf[i][e], kf[e], dot);
+#pragma unroll
+                for (int o = 1; o < LPR; o <<= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+                if (ok[u]) {
+                    const float s = dot * ks[u] * p.scale;
+                    const float mn = fmaxf(m[i], s);
+                    const float corr = expf(m[i] - mn), pe = expf(s - mn);
+                    l[i] = l[i] * corr + pe;
+                    const float pv = pe * vs[u];
+#pragma unroll
+                    for (int e = 0; e < 16; ++e) acc[i][e] = acc[i][e] * corr + pv * vf[e];
+                    m[i] = mn;
+                }
+            }
+        }
+    }
+
+#pragma unroll
+    for (int i = 0; i < GH; ++i) {
+#pragma unroll
+        for (int o = LPR; o < 32; o <<= 1) {
+            const float m2 = __shfl_xor_sync(0xffffffffu, m[i], o);
+            const float l2 = __shfl_xor_sync(0xffffffffu, l[i], o);
+            const float mn = fmaxf(m[i], m2);
+            const float c1 = (mn == -INFINITY) ? 0.f : expf(m[i] - mn), c2 = (mn == -INFINITY) ? 0.f : expf(m2 - mn);
+            // explicit roundings: the contraction the compiler picks in decode_fp8_kernel (with the heads unrolled it may
+            // contract l * c1 + l2 * c2 around the other product), so the bits match it
+            l[i] = __fmaf_rn(l[i], c1, __fmul_rn(l2, c2));
+#pragma unroll
+            for (int e = 0; e < 16; ++e) {
+                const float a2 = __shfl_xor_sync(0xffffffffu, acc[i][e], o);
+                acc[i][e] = __fmaf_rn(acc[i][e], c1, __fmul_rn(a2, c2));
+            }
+            m[i] = mn;
+        }
+        if (sub == 0) {
+            if (piece == 0) { s_m[i][warp] = m[i]; s_l[i][warp] = l[i]; }
+#pragma unroll
+            for (int e = 0; e < 16; ++e) s_acc[i][warp][piece * 16 + e] = acc[i][e];
+        }
+    }
+    __syncthreads();
+    for (int x = tid; x < GH * D; x += kThreads) {
+        const int i = x / D, d = x % D;
+        float mn = -INFINITY;
+#pragma unroll
+        for (int w = 0; w < kWarps; ++w) mn = fmaxf(mn, s_m[i][w]);
+        float lt = 0.f, at = 0.f;
+#pragma unroll
+        for (int w = 0; w < kWarps; ++w) {
+            const float c = (s_m[i][w] == -INFINITY) ? 0.f : expf(s_m[i][w] - mn);
+            lt += s_l[i][w] * c;
+            at += s_acc[i][w][d] * c;
+        }
+        if (p.nsplit == 1) {
+            p.out[(sh0 + i) * D + d] = DT<T>::from_f32(at / lt);
+        } else {
+            float* w = p.ws + ((sh0 + i) * p.nsplit + split) * (2 + D);
+            if (d == 0) { w[0] = mn; w[1] = lt; }
+            w[2 + d] = at;
+        }
+    }
+}
+
 template <typename T, int D>
 cudaError_t launch_decode_fp8_t(const DecodeArgs& a, cudaStream_t st) {
     Fp8DecodeParams p;
@@ -303,12 +466,20 @@ cudaError_t launch_decode_fp8_t(const DecodeArgs& a, cudaStream_t st) {
     p.cache_sh = a.cache_sh; p.cache_sb = a.cache_sb; p.scale_sh = a.scale_sh; p.scale_sb = a.scale_sb;
     p.T = a.T; p.max_rows = a.max_rows;
     p.G = a.G; p.nsplit = a.nsplit; p.num_sms = a.num_sms;
+    p.Hq = a.Hq;
     p.scale = a.scale;
     p.ws = a.ws;
     p.step_dev = a.step_dev;
     p.rows = a.rows;
-    const dim3 grid(unsigned(a.nsplit), unsigned(a.Hq), unsigned(a.num_seqs));
-    decode_fp8_kernel<T, D><<<grid, kThreads, 0, st>>>(p);
+    if (a.gqa) {
+        const unsigned parts = a.G > 4 ? unsigned(a.G / 4) : 1u;
+        const dim3 grid(unsigned(a.nsplit), unsigned(a.Hkv) * parts, unsigned(a.num_seqs));
+        if (a.G == 2) decode_gqa_fp8_kernel<T, D, 2><<<grid, kThreads, 0, st>>>(p);
+        else decode_gqa_fp8_kernel<T, D, 4><<<grid, kThreads, 0, st>>>(p);
+    } else {
+        const dim3 grid(unsigned(a.nsplit), unsigned(a.Hq), unsigned(a.num_seqs));
+        decode_fp8_kernel<T, D><<<grid, kThreads, 0, st>>>(p);
+    }
     count_launch();
     if (a.nsplit > 1) {
         const cudaError_t e = cudaGetLastError();
@@ -336,6 +507,12 @@ cudaError_t launch_quantize_t(const QuantArgs& a, int num_sms, cudaStream_t st) 
 cudaError_t launch_decode_fp8(const DecodeArgs& a, cudaStream_t st) {
     if (a.dtype == PKV_BF16) return a.D == 128 ? launch_decode_fp8_t<__nv_bfloat16, 128>(a, st) : launch_decode_fp8_t<__nv_bfloat16, 64>(a, st);
     return a.D == 128 ? launch_decode_fp8_t<__half, 128>(a, st) : launch_decode_fp8_t<__half, 64>(a, st);
+}
+
+cudaError_t launch_decode_gqa_fp8(const DecodeArgs& a, cudaStream_t st) {
+    DecodeArgs g = a;
+    g.gqa = true;
+    return launch_decode_fp8(g, st);
 }
 
 cudaError_t launch_quantize_fp8(const QuantArgs& a, int num_sms, cudaStream_t st) {

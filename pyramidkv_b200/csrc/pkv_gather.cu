@@ -61,7 +61,46 @@ __global__ void iota_idx_kernel(int64_t* idx64, int64_t k, int64_t total) {
     if (i < total) idx64[i] = i % k;
 }
 
+// PKV_FLAG_GQA_SHARED: out[j][t] = rn_dtype((sum_g f32(in[j*G+g][t]), g ascending) / f32(G)) over whole pooled rows (the pitch
+// is a multiple of 8 elements); 8 elements per thread, grid (row blocks, kv head). The division is correctly rounded, so the
+// result does not depend on how the compiler would treat a multiply by 1/G.
+template <typename T>
+__global__ void __launch_bounds__(256) group_reduce_kernel(const uint16_t* __restrict__ in, uint16_t* __restrict__ out, int64_t pitch, int G) {
+    const int64_t i = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) * 8;
+    if (i >= pitch) return;
+    const int j = blockIdx.y;
+    float s[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) s[e] = 0.f;
+    for (int g = 0; g < G; ++g) {
+        const uint4 v = ldg_nc_v4(in + (int64_t(j) * G + g) * pitch + i);
+        const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            s[2 * e] = __fadd_rn(s[2 * e], DT<T>::to_f32(uint16_t(u[e] & 0xffffu)));
+            s[2 * e + 1] = __fadd_rn(s[2 * e + 1], DT<T>::to_f32(uint16_t(u[e] >> 16)));
+        }
+    }
+    const float fg = float(G);
+    uint32_t w[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+        w[e] = uint32_t(DT<T>::from_f32(__fdiv_rn(s[2 * e], fg))) | (uint32_t(DT<T>::from_f32(__fdiv_rn(s[2 * e + 1], fg))) << 16);
+    *reinterpret_cast<uint4*>(out + int64_t(j) * pitch + i) = make_uint4(w[0], w[1], w[2], w[3]);
+}
+
 }  // namespace
+
+cudaError_t launch_group_reduce(const EvictArgs& a, cudaStream_t st) {
+    const uint16_t* in = reinterpret_cast<const uint16_t*>(a.ws_base + a.ws.pooled_off);
+    uint16_t* out = reinterpret_cast<uint16_t*>(a.ws_base + a.pooled_kv_off);
+    const int64_t vecs = a.ws.pooled_pitch / 8;
+    const dim3 grid(unsigned((vecs + 255) / 256), unsigned(a.Hkv));
+    if (a.dtype == PKV_BF16) group_reduce_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(in, out, a.ws.pooled_pitch, a.G);
+    else group_reduce_kernel<__half><<<grid, 256, 0, st>>>(in, out, a.ws.pooled_pitch, a.G);
+    count_launch();
+    return cudaGetLastError();
+}
 
 cudaError_t launch_gather(const EvictArgs& a, cudaStream_t st) {
     GatherParams p;

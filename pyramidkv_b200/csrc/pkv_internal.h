@@ -24,6 +24,8 @@ struct EvictArgs {
     int device;
     int num_sms;
     bool window_mean = false;   // PKV_FLAG_WINDOW_MEAN: stage 2 averages the window rows (AdaKV / HeadKV scores)
+    bool gqa_shared = false;    // PKV_FLAG_GQA_SHARED with G > 1: one cache per KV head (stages 3-4 run on kv_view(*this))
+    uint64_t pooled_kv_off = 0; // PKV_FLAG_GQA_SHARED: workspace offset of the per-KV-head top-k input (pkv_evict_pooled_kv_offset)
     int score_impl;   // 0 = mma.sync (one softmax partial per tile), 1 = TMA + wgmma (one partial per CTA and kv head)
     int score_grid;   // persistent grid of the wgmma kernel
 };
@@ -71,6 +73,8 @@ cudaError_t launch_select_layers(const EvictArgs* as, int n, cudaStream_t st);
 bool select_batch_supported(const EvictArgs& a);
 // stage 4
 cudaError_t launch_gather(const EvictArgs& a, cudaStream_t st);
+// PKV_FLAG_GQA_SHARED: pooled [Hq][pitch] -> pooled_kv [Hkv][pitch], the fp32 mean over each group rounded once (pkv_gather.cu)
+cudaError_t launch_group_reduce(const EvictArgs& a, cudaStream_t st);
 
 // ---- the whole eviction of a window method in ONE persistent launch (pkv_evict_fused.cu) ----
 constexpr int kFusedStages = 5;        // cross-CTA exchanges: statistics, pooling halo, histogram pass 0 / 1, winners
@@ -120,6 +124,7 @@ struct DecodeArgs {
     // FP8 cache (launch_decode_fp8): k_cache / v_cache hold E4M3 bytes, one fp32 scale per (sequence, head, row)
     float *k_scale = nullptr, *v_scale = nullptr;
     int64_t scale_sh = 0, scale_sb = 0;   // floats between the scales of consecutive heads / sequences
+    bool gqa = false;   // launch_decode_fp8: the cache is GQA-shared (launch_decode_gqa_fp8)
 };
 // split count for T rows (decode_num_splits); shared by the host launch and the device-length decode kernels
 __host__ __device__ inline int64_t decode_splits_for(int64_t Hq, int64_t T, int64_t num_sms) {
@@ -134,9 +139,13 @@ int decode_num_splits(int Hq, int64_t T, int num_sms);
 cudaError_t launch_decode(const DecodeArgs& a, cudaStream_t st);
 cudaError_t launch_decode_combine(const DecodeArgs& a, cudaStream_t st);   // merges the split partials in a.ws into a.out
 cudaError_t launch_append(const DecodeArgs& a, cudaStream_t st);
+// GQA-shared caches ([num_seqs][Hkv][capacity][D], rows[s*Hkv + j]): one CTA per (split, KV head, sequence) computes the G query
+// heads of the group; device-length form only. The split rule and the partials stay those of Hq query heads.
+cudaError_t launch_decode_gqa(const DecodeArgs& a, cudaStream_t st);
 
 // ---- FP8 (E4M3) compacted cache (pkv_fp8.cu) ----
 cudaError_t launch_decode_fp8(const DecodeArgs& a, cudaStream_t st);   // device-length form only (a.devlen)
+cudaError_t launch_decode_gqa_fp8(const DecodeArgs& a, cudaStream_t st);   // GQA-shared FP8 caches (launch_decode_gqa)
 struct QuantLayer {
     const uint16_t* src[2];   // K, V: 16-bit [num_seqs][H][src_cap][D]
     uint8_t* dst[2];          // K, V: E4M3 [num_seqs][H][dst_cap][D]

@@ -19,6 +19,8 @@ the whole batch instead of once per sequence.
 
 With `model.config.pkv_kv_cache_dtype = "fp8_e4m3"` the prefill leaves FP8 caches (`cache.PkvFp8CacheLayer`); all three loops
 take them as they are (the knob is the single source: no parameter here), one `pkv_decode_attn_batch_fp8` launch per layer.
+Likewise with `model.config.pkv_gqa_shared = True` (one cache per KV head, `group` > 1): one `pkv_decode_attn_batch_gqa(_fp8)`
+launch per layer.
 """
 from __future__ import annotations
 
@@ -60,7 +62,7 @@ class StaticDecoder:
         for l in layers:
             l.reserve(self.max_steps)                      # off the per-token path: no reallocation while the graph lives
         backend = model.model.layers[0].self_attn.kv_cluster.backend
-        hq, d = layers[0].k_buf.shape[1], layers[0].k_buf.shape[3]
+        hq, d = layers[0].k_buf.shape[1] * getattr(layers[0], "group", 1), layers[0].k_buf.shape[3]   # query heads
         self.state = _StaticState(step=torch.zeros(1, dtype=torch.int32, device=dev),
                                   workspace=backend.decode_workspace(bsz * hq, d, dev))
         self.ids = first_token.reshape(bsz, 1).to(device=dev, dtype=torch.long).clone()

@@ -27,8 +27,10 @@ class CudaBackend:
 
     accepts_inputs_ready = True
 
-    def evict(self, method, q, k, v, window_size, top_k, k_cache, v_cache, kernel_size, pooling, idx_out=None, inputs_ready=False):
-        ops.evict_prefill(method, q, k, v, window_size, top_k, k_cache, v_cache, kernel_size, pooling, idx_out, inputs_ready=inputs_ready)
+    def evict(self, method, q, k, v, window_size, top_k, k_cache, v_cache, kernel_size, pooling, idx_out=None, inputs_ready=False,
+              gqa_shared=False):
+        ops.evict_prefill(method, q, k, v, window_size, top_k, k_cache, v_cache, kernel_size, pooling, idx_out, inputs_ready=inputs_ready,
+                          gqa_shared=gqa_shared)
 
     accepts_layer_batch = True
 
@@ -77,6 +79,16 @@ class CudaBackend:
                               workspace=None, out=None, softmax_scale=0.0):
         return ops.decode_attn_batch_fp8(q, k_q, v_q, k_scale, v_scale, length, k_new, v_new, rows, step, max_length, workspace,
                                          out, softmax_scale)
+
+    # -- GQA-shared caches (model.config.pkv_gqa_shared = True): one cache per KV head --
+    def decode_attn_batch_gqa(self, q, k_buf, v_buf, length, k_new, v_new, rows=None, step=None, max_length=0, workspace=None,
+                              out=None, softmax_scale=0.0):
+        return ops.decode_attn_batch_gqa(q, k_buf, v_buf, length, k_new, v_new, rows, step, max_length, workspace, out, softmax_scale)
+
+    def decode_attn_batch_gqa_fp8(self, q, k_q, v_q, k_scale, v_scale, length, k_new, v_new, rows=None, step=None, max_length=0,
+                                  workspace=None, out=None, softmax_scale=0.0):
+        return ops.decode_attn_batch_gqa_fp8(q, k_q, v_q, k_scale, v_scale, length, k_new, v_new, rows, step, max_length, workspace,
+                                             out, softmax_scale)
 
     def rope_inplace(self, q, k, cos, sin):
         ops.rope_inplace(q, k, cos, sin)
@@ -178,12 +190,18 @@ class _KVCluster:
     def budget(self, q_len: int) -> Tuple[int, int]:
         return self.backend.layer_budget(self.method, self.max_capacity_prompt, self.window_size, 2, 0, q_len)
 
-    def evict_into(self, query_states, key_states, value_states, reserve: int = 0, pending: Optional[list] = None):
+    def evict_into(self, query_states, key_states, value_states, reserve: int = 0, pending: Optional[list] = None,
+                   gqa_shared: bool = False):
         """Evict one prompt (bsz == 1 slice, [H,S,D] tensors on the GPU) into freshly allocated cache buffers.
         Returns (k_buf, v_buf, rows): buffers [Hq, rows + reserve, D]; rows = S when nothing is evicted.
         `pending`: a list to PARK this eviction on instead of launching it (window methods only): the buffers are returned
-        unfilled and `flush_pending(pending, backend)` later evicts all parked layers in one pass (CudaBackend.evict_batch)."""
+        unfilled and `flush_pending(pending, backend)` later evicts all parked layers in one pass (CudaBackend.evict_batch).
+        `gqa_shared` (knob pkv_gqa_shared, Hq > Hkv): one selection per KV head (PKV_FLAG_GQA_SHARED), buffers
+        [Hkv, rows + reserve, D]; never parked (the layer batch is not built for it)."""
         Hq, D = query_states.shape[-3], query_states.shape[-1]
+        gqa_shared = gqa_shared and key_states.shape[-3] != Hq
+        if gqa_shared:
+            Hq, pending = key_states.shape[-3], None          # the heads of the cache
         S = key_states.shape[-2]          # query_states may hold only the last window_size rows
         mode, top_k = self.budget(S)
         method, W = self.method, self.window_size
@@ -215,6 +233,8 @@ class _KVCluster:
             pending.append(dict(method=method, q=q_win, k=key_states, v=value_states, W=W, top_k=top_k, k_cache=k_buf, v_cache=v_buf,
                                 kernel_size=self.kernel_size, pooling=self.pooling, idx_out=idx))
             return k_buf, v_buf, rows
+        if gqa_shared:
+            extra["gqa_shared"] = True
         self.backend.evict(method, query_states, key_states, value_states, W, top_k, k_buf, v_buf,
                            self.kernel_size, self.pooling, idx, **extra)
         return k_buf, v_buf, rows

@@ -84,12 +84,14 @@ def plan_evict(method: str, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, w
                k_cache: torch.Tensor, v_cache: torch.Tensor, kernel_size: int = 5, pooling: str = "avgpool",
                idx_out: Optional[torch.Tensor] = None, score_kernel: str = "auto",
                workspace: Optional[torch.Tensor] = None, window_mean: bool = False, staged: bool = False,
-               inputs_ready: bool = False, single_launch: bool = False, fused: bool = False) -> EvictPlan:
+               inputs_ready: bool = False, single_launch: bool = False, fused: bool = False,
+               gqa_shared: bool = False) -> EvictPlan:
     """`staged`: PKV_FLAG_STAGED (stages 1-4 as separate launches even where the fused kernel applies). `single_launch`:
     PKV_FLAG_SINGLE_LAUNCH (stages 1-4 in ONE launch instead of the default fused stages 1-2 + select kernel). `fused`:
     PKV_FLAG_FUSED (the fused stages 1-2 kernel for every supported shape, not only where it is measured faster).
     `inputs_ready`: PKV_FLAG_INPUTS_READY (q/k/v were not written by the kernel just before this call: K streaming may
-    start early)."""
+    start early). `gqa_shared`: PKV_FLAG_GQA_SHARED (one selection and one cache per KV head: k_cache / v_cache are
+    [Hkv, capacity, D] and idx_out [Hkv, top_k]; include/pkv.h gives the group reduction)."""
     if method not in METHODS:
         raise ValueError(f"unknown method {method!r}")
     if pooling not in POOLING:
@@ -116,8 +118,9 @@ def plan_evict(method: str, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, w
         # (StreamingLLM never reads q at all.)
         q_tail = Sq != S and method != "h2o" and (Sq == window_size or method == "streamingllm")
         assert Sq == S or q_tail                                   # pyramidkv_utils.py:200
-    if not (kc.is_contiguous() and vc.is_contiguous()) or kc.shape != vc.shape or kc.shape[0] != Hq or kc.shape[2] != D:
-        raise ValueError("k_cache/v_cache must be contiguous [Hq, capacity, D] tensors of equal shape")
+    Hc = Hkv if gqa_shared else Hq            # heads of the cache
+    if not (kc.is_contiguous() and vc.is_contiguous()) or kc.shape != vc.shape or kc.shape[0] != Hc or kc.shape[2] != D:
+        raise ValueError(f"k_cache/v_cache must be contiguous [{'Hkv' if gqa_shared else 'Hq'}, capacity, D] tensors of equal shape")
     d = EvictDesc()
     d.struct_bytes = C.sizeof(EvictDesc)
     d.method, d.dtype, d.pooling, d.kernel_size = METHODS[method], _dtype_code(k), POOLING[pooling], int(kernel_size)
@@ -134,10 +137,11 @@ def plan_evict(method: str, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, w
     d.v, d.v_stride_h, d.v_stride_s = v.data_ptr(), v.stride(0), v.stride(1)
     d.k_cache, d.v_cache, d.cache_stride_h = kc.data_ptr(), vc.data_ptr(), kc.stride(0)
     if idx_out is not None:
-        if idx_out.dtype != torch.int64 or not idx_out.is_contiguous() or idx_out.numel() != Hq * top_k:
-            raise ValueError("idx_out must be a contiguous int64 [Hq, top_k] tensor")
+        if idx_out.dtype != torch.int64 or not idx_out.is_contiguous() or idx_out.numel() != Hc * top_k:
+            raise ValueError("idx_out must be a contiguous int64 [heads of the cache, top_k] tensor")
         d.idx_out = idx_out.data_ptr()
     d.flags = SCORE_KERNELS[score_kernel] | (4 if window_mean else 0) | (8 if inputs_ready else 0) | (16 if staged else 0) | (32 if single_launch else 0) | (64 if fused else 0)
+    d.flags |= _lib.FLAG_GQA_SHARED if gqa_shared else 0
     L = WsLayout()
     _lib.check(_lib.lib().pkv_evict_workspace_layout(C.byref(d), C.byref(L)))
     ws = workspace if workspace is not None else _workspace(k.device, int(L.total_bytes))
@@ -153,13 +157,15 @@ def workspace_bytes_for(plan: EvictPlan, top_k: int) -> int:
 
 
 def evict_prefill(method: str, q, k, v, window_size: int, top_k: int, k_cache, v_cache, kernel_size: int = 5,
-                  pooling: str = "avgpool", idx_out=None, score_kernel: str = "auto", inputs_ready: bool = False) -> None:
+                  pooling: str = "avgpool", idx_out=None, score_kernel: str = "auto", inputs_ready: bool = False,
+                  gqa_shared: bool = False) -> None:
     """One layer's prefill eviction on the current CUDA stream (asynchronous).
 
     q [Hq,S,D]; k, v [Hkv,S,D] un-repeated (or Hkv == Hq after repeat_kv); writes rows 0..top_k+W-1 of
-    k_cache/v_cache [Hq, capacity, D]. Replaces *KVCluster.update_kv (pyramidkv_utils.py:197-620)."""
+    k_cache/v_cache [Hq, capacity, D] ([Hkv, capacity, D] with `gqa_shared`). Replaces *KVCluster.update_kv
+    (pyramidkv_utils.py:197-620)."""
     plan = plan_evict(method, q, k, v, window_size, top_k, k_cache, v_cache, kernel_size, pooling, idx_out, score_kernel,
-                      inputs_ready=inputs_ready)
+                      inputs_ready=inputs_ready, gqa_shared=gqa_shared)
     _lib.check(_lib.lib().pkv_evict_prefill(C.byref(plan.desc), plan.stream_ptr()))
 
 
@@ -262,6 +268,17 @@ def ws_pooled(plan: EvictPlan) -> torch.Tensor:
     dt = torch.bfloat16 if d.dtype == 0 else torch.float16
     n = d.num_q_heads * L.pooled_pitch
     return plan.workspace[L.pooled_off:L.pooled_off + 2 * n].view(dt).view(d.num_q_heads, L.pooled_pitch)[:, :d.seq_len - d.window]
+
+
+def ws_pooled_kv(plan: EvictPlan) -> torch.Tensor:
+    """[Hkv, S-W] view of the per-KV-head top-k input of a `gqa_shared` plan (the group reduction of `ws_pooled`)."""
+    d, L = plan.desc, plan.layout
+    off = C.c_uint64(0)
+    _lib.check(_lib.lib().pkv_evict_pooled_kv_offset(C.byref(d), C.byref(off)))
+    off = int(off.value)
+    dt = torch.bfloat16 if d.dtype == 0 else torch.float16
+    n = d.num_kv_heads * L.pooled_pitch
+    return plan.workspace[off:off + 2 * n].view(dt).view(d.num_kv_heads, L.pooled_pitch)[:, :d.seq_len - d.window]
 
 
 def single_launch(plan: EvictPlan) -> int:
@@ -580,6 +597,89 @@ def decode_attn_batch_fp8(q: torch.Tensor, k_q: torch.Tensor, v_q: torch.Tensor,
                                                     k_scale.data_ptr(), v_scale.data_ptr(), k_scale.stride(1), k_scale.stride(0),
                                                     torch.cuda.current_stream(q.device).cuda_stream))
     return out
+
+
+# ---- GQA-shared caches (PKV_FLAG_GQA_SHARED): one cache per KV head, decoded once per group ----
+def _decode_gqa(what, q, k_buf, v_buf, length, k_new, v_new, rows, step, max_length, workspace, out, softmax_scale, scales=None):
+    _require_cuda(q, k_buf, v_buf, k_new, v_new, rows, step, workspace, out, *(scales or ()))
+    if scales is not None:
+        _check_fp8_buffers(k_buf, v_buf, scales[0], scales[1], what)
+    elif k_buf.dim() != 4 or k_buf.shape != v_buf.shape or k_buf.stride() != v_buf.stride() or k_buf.stride(3) != 1 \
+            or k_buf.stride(2) != k_buf.shape[3]:
+        raise ValueError(f"{what}: k_buf / v_buf must be [B, Hkv, capacity, D] tensors of equal shape and strides, rows contiguous")
+    B, Hkv, cap, D = k_buf.shape
+    if q.dim() != 3 or q.shape[0] != B or q.shape[2] != D or q.shape[1] % Hkv:
+        raise ValueError(f"{what}: q must be [B, Hq, D] with Hq a multiple of Hkv = {Hkv}, got {tuple(q.shape)}")
+    Hq = q.shape[1]
+    q = q.contiguous()
+    if out is None:
+        out = torch.empty(B, Hq, D, dtype=q.dtype, device=q.device)
+    elif out.shape != (B, Hq, D) or not out.is_contiguous() or out.dtype != q.dtype:
+        raise ValueError(f"{what}: out must be a contiguous [B, Hq, D] tensor of q's dtype")
+    max_length = int(max_length) or cap
+    if not 1 <= length <= max_length <= cap:
+        raise ValueError(f"{what}: cache capacity {cap} exceeded or bad row counts (length {length}, max_length {max_length})")
+    if step is not None and (step.dtype != torch.int32 or step.numel() != 1):
+        raise ValueError("step must be an int32 device tensor with one element")
+    if rows is not None:
+        if rows.dtype != torch.int32 or rows.numel() != B * Hkv or not rows.is_contiguous():
+            raise ValueError(f"{what}: rows must be a contiguous int32 device tensor of B*Hkv = {B * Hkv} elements")
+        if not torch.cuda.is_current_stream_capturing():
+            most = int(rows.max()) + int(length) + (int(step) if step is not None else 0)
+            if most > max_length:
+                raise ValueError(f"{what}: cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
+    d = DecodeDesc()
+    d.struct_bytes = C.sizeof(DecodeDesc)
+    d.dtype, d.num_q_heads, d.num_kv_heads, d.head_dim = _dtype_code(q), B * Hq, Hkv, D
+    d.device = q.device.index if q.device.index is not None else torch.cuda.current_device()
+    nbytes = int(_lib.lib().pkv_decode_workspace_bytes(C.byref(d)))      # one set of split partials per (sequence, query head)
+    d.num_q_heads = Hq
+    d.length = int(length)
+    d.q, d.k_cache, d.v_cache, d.cache_stride_h, d.out = q.data_ptr(), k_buf.data_ptr(), v_buf.data_ptr(), k_buf.stride(1), out.data_ptr()
+    keep = [q, out]
+    if k_new is not None:
+        if k_new.dim() != 3 or k_new.shape != (B, Hkv, D) or v_new is None or v_new.shape != k_new.shape \
+                or k_new.dtype != q.dtype or v_new.dtype != q.dtype:
+            raise ValueError(f"{what}: k_new / v_new must be [B, Hkv, D] = {(B, Hkv, D)} tensors of q's dtype")
+        k_new, v_new = k_new.contiguous(), v_new.contiguous()
+        d.k_new, d.v_new = k_new.data_ptr(), v_new.data_ptr()
+        keep += [k_new, v_new]
+    ws = workspace if workspace is not None else _workspace(q.device, nbytes)
+    d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel() * ws.element_size()
+    d.softmax_scale = float(softmax_scale)
+    common = (C.byref(d), B, k_buf.stride(0), rows.data_ptr() if rows is not None else None,
+              step.data_ptr() if step is not None else None, max_length)
+    stream = torch.cuda.current_stream(q.device).cuda_stream
+    if scales is None:
+        _lib.check(_lib.lib().pkv_decode_attn_batch_gqa(*common, stream))
+    else:
+        ks, vs = scales
+        _lib.check(_lib.lib().pkv_decode_attn_batch_gqa_fp8(*common, ks.data_ptr(), vs.data_ptr(), ks.stride(1), ks.stride(0), stream))
+    return out
+
+
+def decode_attn_batch_gqa(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor, length: int,
+                          k_new: Optional[torch.Tensor] = None, v_new: Optional[torch.Tensor] = None,
+                          rows: Optional[torch.Tensor] = None, step: Optional[torch.Tensor] = None, max_length: int = 0,
+                          workspace: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                          softmax_scale: float = 0.0) -> torch.Tensor:
+    """`decode_attn_batch` over GQA-shared caches (`pkv_decode_attn_batch_gqa`): buffers [B, Hkv, capacity, D], one per KV
+    head, read once for the Hq / Hkv query heads of its group; q / out [B, Hq, D]; k_new / v_new [B, Hkv, D]; `rows` int32
+    [B*Hkv]. Query head h's output and the appended row are bit-identical to `decode_attn_batch` over the cache
+    repeat-interleaved along the heads. Workspace: `decode_workspace_bytes(B*Hq, D)`."""
+    return _decode_gqa("decode_attn_batch_gqa", q, k_buf, v_buf, length, k_new, v_new, rows, step, max_length, workspace, out,
+                       softmax_scale)
+
+
+def decode_attn_batch_gqa_fp8(q: torch.Tensor, k_q: torch.Tensor, v_q: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor,
+                              length: int, k_new: Optional[torch.Tensor] = None, v_new: Optional[torch.Tensor] = None,
+                              rows: Optional[torch.Tensor] = None, step: Optional[torch.Tensor] = None, max_length: int = 0,
+                              workspace: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                              softmax_scale: float = 0.0) -> torch.Tensor:
+    """`decode_attn_batch_fp8` over GQA-shared FP8 caches (`pkv_decode_attn_batch_gqa_fp8`): k_q / v_q float8_e4m3fn
+    [B, Hkv, capacity, D], k_scale / v_scale float32 [B, Hkv, capacity]; otherwise as `decode_attn_batch_gqa`."""
+    return _decode_gqa("decode_attn_batch_gqa_fp8", q, k_q, v_q, length, k_new, v_new, rows, step, max_length, workspace, out,
+                       softmax_scale, scales=(k_scale, v_scale))
 
 
 def decode_workspace_bytes(num_q_heads: int, head_dim: int) -> int:

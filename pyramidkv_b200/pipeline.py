@@ -97,6 +97,9 @@ class PipelineRunner:
         if getattr(stage.config, "pkv_kv_cache_dtype", None) not in (None, "auto"):
             raise NotImplementedError("the FP8 compacted cache (pkv_kv_cache_dtype) is converted by the model's last layer in one "
                                       "launch; the layer-sliced pipeline flushes per rank and keeps the 16-bit cache")
+        if getattr(stage.config, "pkv_gqa_shared", False):
+            raise NotImplementedError("the GQA-shared cache (pkv_gqa_shared) is installed in the batched row-count form that the "
+                                      "layer-sliced pipeline does not decode; it keeps the per-query-head cache")
         self.stage, self.group = stage, group
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1

@@ -292,17 +292,23 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
               dtype: torch.dtype = torch.float16, attn_implementation: str = "sdpa", merge=None, seed: int = 42,
               backend_factory: Optional[Callable] = None, out_path: Optional[str] = None, tag: Optional[dict] = None,
               decode_loop: str = "hf", floor: float = 0.2, head_beta: float = 1.01, head_path: str = "",
-              capacity_ratio: float = -1, eval_batch_size: int = 1, kv_cache_dtype: str = "auto") -> List[dict]:
+              capacity_ratio: float = -1, eval_batch_size: int = 1, kv_cache_dtype: str = "auto",
+              gqa_shared: bool = False) -> List[dict]:
     """prompts: iterable of (name, prompt_tokens, max_new_tokens). One JSON record per prompt (also appended to out_path).
     eval_batch_size N > 1: consecutive prompts with the same max_new_tokens are decoded N at a time (static loops only;
     each prompt is still prefilled alone, so its prefill_ms, cache rows and tokens are its own).
     kv_cache_dtype "fp8_e4m3": the compacted caches are converted to FP8 after the prefill (model.config.pkv_kv_cache_dtype);
-    the records then carry "kv_cache_dtype". "auto" (the default) changes nothing."""
+    the records then carry "kv_cache_dtype". "auto" (the default) changes nothing.
+    gqa_shared: one selection and one compacted cache per KV head (model.config.pkv_gqa_shared); the records then carry
+    "gqa_shared". FullKV, AdaKV and HeadKV refuse it."""
     if kv_cache_dtype not in ("auto", "fp8_e4m3"):
         raise ValueError(f"kv_cache_dtype must be auto or fp8_e4m3, got {kv_cache_dtype!r}")
     if kv_cache_dtype != "auto" and canonical_method(method) == "fullkv":
         raise NotImplementedError("--kv_cache_dtype fp8_e4m3 converts the compacted cache of an eviction method; FullKV keeps "
                                   "HF's own cache (the reference's --quant_method caches are not built)")
+    if gqa_shared and canonical_method(method) in ("fullkv", "adakv", "headkv"):
+        raise NotImplementedError(f"--gqa_shared selects one compacted cache per KV head; {canonical_method(method)} "
+                                  + ("keeps HF's own cache" if canonical_method(method) == "fullkv" else "sets budgets per query head"))
     if eval_batch_size < 1:
         raise ValueError(f"eval_batch_size must be >= 1, got {eval_batch_size}")
     if eval_batch_size > 1 and (decode_loop == "hf" or canonical_method(method) == "fullkv"):
@@ -325,6 +331,8 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
             raise ValueError("either max_capacity_prompts or max_capacity_prompts_ratio must be given")
         if kv_cache_dtype != "auto":
             model.config.pkv_kv_cache_dtype = kv_cache_dtype
+        if gqa_shared:
+            model.config.pkv_gqa_shared = True
         records = []
         prompts = list(prompts)
         if eval_batch_size > 1 and max_capacity_prompt == -1 and capacity_ratio != -1 and len({p[1] for p in prompts}) > 1:
@@ -350,6 +358,7 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
                        "max_capacity_prompt": model.config.max_capacity_prompt if method != "fullkv" else max_capacity_prompt, "window": window,
                        "decode_loop": decode_loop if method != "fullkv" else "hf",
                        **({"kv_cache_dtype": kv_cache_dtype} if kv_cache_dtype != "auto" else {}),
+                       **({"gqa_shared": True} if gqa_shared else {}),
                        "dtype": str(dtype).replace("torch.", ""), "data": "synthetic token ids, random-init weights", **(tag or {}),
                        "prompt_tokens": r.prompt_tokens, "new_tokens": r.new_tokens, "prefill_ms": r.prefill_ms,
                        "decode_tok_per_s": r.decode_tok_per_s, **batch, "cache_rows_first_last": r.cache_rows_first_last, "pred_ids": r.pred_ids}

@@ -57,6 +57,9 @@ def build_parser() -> argparse.ArgumentParser:
                    help="hf: model.generate as in the reference; static: pyramidkv_b200.generate (CUDA-graph replay per token)")
     p.add_argument("--kv_cache_dtype", type=str, default="auto", choices=["auto", "fp8_e4m3"],
                    help="auto: the compacted cache in the model dtype; fp8_e4m3: FP8 bytes + one fp32 scale per row (half the KV bytes)")
+    p.add_argument("--gqa_shared", action="store_true",
+                   help="one selection and one compacted cache per KV head (the score averaged over each GQA group): "
+                        "Hq/Hkv times fewer cache bytes; not for fullkv / adakv / headkv")
     return p
 
 
@@ -90,7 +93,7 @@ def main(argv=None, backend_factory=None, device=None):
                             backend_factory=backend_factory, out_path=out, decode_loop=args.decode_loop,
                             floor=args.floor, head_beta=args.head_beta, head_path=args.head_path,
                             capacity_ratio=args.max_capacity_prompts_ratio, eval_batch_size=args.eval_batch_size,
-                            kv_cache_dtype=args.kv_cache_dtype)
+                            kv_cache_dtype=args.kv_cache_dtype, gqa_shared=args.gqa_shared)
     n = len(recs)
     print(json.dumps({"summary": True, "arch": arch, "method": method, "max_capacity_prompts": capacity, "examples": n,
                       "mean_prefill_ms": sum(r["prefill_ms"] for r in recs) / n,

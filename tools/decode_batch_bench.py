@@ -12,6 +12,9 @@ reference runners' knobs (window 8, kernel 7, maxpool). Prints one JSON line wit
 the bf16 caches of the same prompts converted exactly as the knob pkv_kv_cache_dtype = "fp8_e4m3" converts them after the
 prefill; their KV bytes count one byte per element plus the two 4-byte scales of every row and head. --batch max picks, per
 dtype, the largest batch whose joined caches fit the free device memory, computed from bytes before allocating.
+--gqa_shared off,on measures the per-query-head caches and the GQA-shared ones (knob pkv_gqa_shared: one cache per KV head,
+decoded by pkv_decode_attn_batch_gqa(_fp8)) of the same prompts, alternating them per batch size like the dtypes; the KV bytes
+of a shared cache count its Hkv heads.
 Writes nothing but stdout.
 """
 import argparse
@@ -51,13 +54,15 @@ def _kv_row_bytes(D, kv_dtype):
 
 
 def _cache_bytes_per_seq(model, caches, reserve, kv_dtype):
-    """Bytes one sequence's joined cache allocates (the buffers are [Hq, longest + reserve, D] per layer)."""
-    Hq, D = model.config.num_attention_heads, model.config.head_dim
-    return sum(Hq * (max(l.length for l in ls) + reserve) * _kv_row_bytes(D, kv_dtype) for ls in zip(*[c.layers for c in caches]))
+    """Bytes one sequence's joined cache allocates (the buffers are [H, longest + reserve, D] per layer, H the cache's heads:
+    Hq, or Hkv for a GQA-shared cache)."""
+    D = model.config.head_dim
+    return sum(ls[0].k_buf.shape[1] * (max(l.length for l in ls) + reserve) * _kv_row_bytes(D, kv_dtype)
+               for ls in zip(*[c.layers for c in caches]))
 
 
 def decode_batched_numbers(model, device, ctx, batch_sizes, weight_bytes, new_tokens=32, distinct=2, attn_steps=50,
-                           kv_dtypes=("bf16",), headroom_bytes=4 << 30):
+                           kv_dtypes=("bf16",), headroom_bytes=4 << 30, gqa_modes=(False,)):
     """Batched greedy decode (pyramidkv_b200.generate: joined compacted caches, one CUDA-graph replay per step, one attention
     launch per layer whatever the batch). `distinct` prompts are prefilled and joined repeated up to each batch size B: the
     cost of a decode step does not depend on the cache contents, and this avoids B prefills of the long prompt.
@@ -70,35 +75,41 @@ def decode_batched_numbers(model, device, ctx, batch_sizes, weight_bytes, new_to
     from pyramidkv_b200.cache import PkvFp8CacheLayer, join_caches, quantize_caches_fp8
     from pyramidkv_b200.generate import StaticDecoder, _prefill
     bw_gbs, bw_src = peaks()
-    firsts, caches = [], {"bf16": []}
-    for i in range(distinct):
-        ids = torch.randint(1, model.config.vocab_size, (1, ctx), generator=torch.Generator().manual_seed(100 + i)).to(device)
-        f, c = _prefill(model, ids)
-        firsts.append(f)
-        caches["bf16"].append(c)
-    if "fp8_e4m3" in kv_dtypes:
-        backend = model.model.layers[0].self_attn.kv_cluster.backend
-        caches["fp8_e4m3"] = []
-        for c in caches["bf16"]:                         # the conversion the knob runs after the prefill, on a copy of the list
-            c8 = DynamicCache()
-            c8.layers = list(c.layers)
-            quantize_caches_fp8(c8, backend)
-            caches["fp8_e4m3"].append(c8)
+    firsts, caches = [], {}
+    for gqa in gqa_modes:
+        model.config.pkv_gqa_shared = gqa
+        caches[gqa, "bf16"] = []
+        for i in range(distinct):
+            ids = torch.randint(1, model.config.vocab_size, (1, ctx), generator=torch.Generator().manual_seed(100 + i)).to(device)
+            f, c = _prefill(model, ids)
+            if gqa == gqa_modes[0]:
+                firsts.append(f)
+            caches[gqa, "bf16"].append(c)
+        if "fp8_e4m3" in kv_dtypes:
+            backend = model.model.layers[0].self_attn.kv_cluster.backend
+            caches[gqa, "fp8_e4m3"] = []
+            for c in caches[gqa, "bf16"]:                # the conversion the knob runs after the prefill, on a copy of the list
+                c8 = DynamicCache()
+                c8.layers = list(c.layers)
+                quantize_caches_fp8(c8, backend)
+                caches[gqa, "fp8_e4m3"].append(c8)
+    model.config.pkv_gqa_shared = False
     reserve = new_tokens + 3
     points, attn, fits = [], [], {}
     torch.cuda.synchronize()
     for Bspec in batch_sizes:
-        for kv_dtype in kv_dtypes:
-            per_seq = _cache_bytes_per_seq(model, caches[kv_dtype], reserve, kv_dtype)
+        for gqa, kv_dtype in [(g, k) for g in gqa_modes for k in kv_dtypes]:
+            tag = {"kv_cache_dtype": kv_dtype, **({"gqa_shared": gqa} if len(gqa_modes) > 1 or gqa else {})}
+            per_seq = _cache_bytes_per_seq(model, caches[gqa, kv_dtype], reserve, kv_dtype)
             if Bspec == "max":
                 free, total = torch.cuda.mem_get_info(device)
                 B = max(1, int((free - headroom_bytes) // per_seq))
-                fits[kv_dtype] = {"batch": B, "cache_bytes_per_seq": per_seq, "free_bytes": free, "total_bytes": total,
-                                  "headroom_bytes": headroom_bytes}
+                fits[kv_dtype + ("+gqa_shared" if gqa else "")] = {"batch": B, "cache_bytes_per_seq": per_seq, "free_bytes": free,
+                                                                   "total_bytes": total, "headroom_bytes": headroom_bytes}
             else:
                 B = int(Bspec)
             pick = [i % distinct for i in range(B)]
-            cache = join_caches([caches[kv_dtype][i] for i in pick], reserve=reserve)
+            cache = join_caches([caches[gqa, kv_dtype][i] for i in pick], reserve=reserve)
             first = torch.cat([firsts[i] for i in pick])
             fp8 = isinstance(cache.layers[0], PkvFp8CacheLayer)
             D = cache.layers[0].k_buf.shape[3]
@@ -115,7 +126,13 @@ def decode_batched_numbers(model, device, ctx, batch_sizes, weight_bytes, new_to
 
             def attn_step():
                 for l in cache.layers:
-                    if fp8:
+                    if l.group > 1 and fp8:
+                        ops.decode_attn_batch_gqa_fp8(q, l.k_buf, l.v_buf, l.k_scale, l.v_scale, 1, kn, kn, rows=l.rows, step=step,
+                                                      max_length=l.capacity, workspace=ws, out=out)
+                    elif l.group > 1:
+                        ops.decode_attn_batch_gqa(q, l.k_buf, l.v_buf, 1, kn, kn, rows=l.rows, step=step, max_length=l.capacity,
+                                                  workspace=ws, out=out)
+                    elif fp8:
                         ops.decode_attn_batch_fp8(q, l.k_buf, l.v_buf, l.k_scale, l.v_scale, 1, kn, kn, rows=l.rows, step=step,
                                                   max_length=l.capacity, workspace=ws, out=out)
                     else:
@@ -135,7 +152,7 @@ def decode_batched_numbers(model, device, ctx, batch_sizes, weight_bytes, new_to
             e1.record()
             torch.cuda.synchronize()
             attn_ms = e0.elapsed_time(e1) / attn_steps
-            attn.append({"batch": B, "kv_cache_dtype": kv_dtype, "attn_ms_per_step": attn_ms, "launches_per_step": len(cache.layers),
+            attn.append({"batch": B, **tag, "attn_ms_per_step": attn_ms, "launches_per_step": len(cache.layers),
                          "kv_bytes_per_step": kv_bytes, "kv_gbs": kv_bytes / (attn_ms * 1e-3) / 1e9,
                          "frac_of_hbm": kv_bytes / (attn_ms * 1e-3) / (bw_gbs * 1e9)})
             del graph
@@ -148,7 +165,7 @@ def decode_batched_numbers(model, device, ctx, batch_sizes, weight_bytes, new_to
             torch.cuda.synchronize()
             ms = e0.elapsed_time(e1) / new_tokens
             bound_ms = (weight_bytes + kv_bytes) / (bw_gbs * 1e9) * 1e3
-            points.append({"batch": B, "kv_cache_dtype": kv_dtype, "ms_per_step": ms, "aggregate_tok_s": B * 1e3 / ms,
+            points.append({"batch": B, **tag, "ms_per_step": ms, "aggregate_tok_s": B * 1e3 / ms,
                            "kv_bytes_per_step": kv_bytes, "weight_bytes": weight_bytes,
                            "weight_floor_ms": weight_bytes / (bw_gbs * 1e9) * 1e3, "bound_ms": bound_ms, "step_over_bound": ms / bound_ms})
             dec.finish()
@@ -184,11 +201,16 @@ def main():
     ap.add_argument("--budget", type=int, default=128)
     ap.add_argument("--new", type=int, default=32, help="timed decode steps per batch size")
     ap.add_argument("--kv_cache_dtype", default="bf16", help="comma-separated cache dtypes: bf16, fp8_e4m3")
+    ap.add_argument("--gqa_shared", default="off", help="comma-separated: off, on (knob pkv_gqa_shared)")
     ap.add_argument("--no_single", action="store_true", help="skip the single-sequence loop")
     args = ap.parse_args()
     kv_dtypes = [x.strip() for x in args.kv_cache_dtype.split(",") if x.strip()]
     if not kv_dtypes or any(x not in ("bf16", "fp8_e4m3") for x in kv_dtypes):
         raise SystemExit(f"--kv_cache_dtype takes bf16 and / or fp8_e4m3, got {args.kv_cache_dtype!r}")
+    gqa_modes = [x.strip() for x in args.gqa_shared.split(",") if x.strip()]
+    if not gqa_modes or any(x not in ("off", "on") for x in gqa_modes):
+        raise SystemExit(f"--gqa_shared takes off and / or on, got {args.gqa_shared!r}")
+    gqa_modes = tuple(x == "on" for x in gqa_modes)
     if not torch.cuda.is_available():
         raise SystemExit("tools/decode_batch_bench.py measures on a CUDA device (H100); there is none here")
     device = torch.device("cuda", 0)
@@ -207,11 +229,11 @@ def main():
             torch.cuda.empty_cache()
             batch = [x.strip() if x.strip() == "max" else int(x) for x in args.batch.split(",") if x.strip()]
             batched, attn = decode_batched_numbers(model, device, args.ctx, batch, weight_bytes, new_tokens=args.new,
-                                                   kv_dtypes=kv_dtypes)
+                                                   kv_dtypes=kv_dtypes, gqa_modes=gqa_modes)
     finally:
         restore()
     print(json.dumps({"model": "llama3-8b (random init)", "method": "pyramidkv", "ctx": args.ctx, "budget": args.budget,
-                      "dtype": "bf16", "kv_cache_dtypes": kv_dtypes, "fused_rope": True, "gpu": gpu_card(device), "weight_bytes": weight_bytes,
+                      "dtype": "bf16", "kv_cache_dtypes": kv_dtypes, "gqa_shared": list(gqa_modes), "fused_rope": True, "gpu": gpu_card(device), "weight_bytes": weight_bytes,
                       "single": single, "decode_batched": batched, "decode_batched_attn": attn}))
 
 
