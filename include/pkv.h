@@ -322,6 +322,23 @@ int pkv_decode_attn_batch_gqa_fp8(const pkv_decode_desc* d, int32_t num_seqs, in
 int pkv_cache_quantize_fp8(int32_t dtype, int32_t num_seqs, int32_t num_heads, int32_t head_dim, int32_t device, int32_t num_layers,
                            const void* const* src, void* const* dst, float* const* scales, const int64_t* src_capacity,
                            const int64_t* dst_capacity, const int64_t* rows, const int32_t* const* rows_dev, void* stream);
+/* Admission of one prompt into slot `slot` of a batched compacted cache (continuous batching), in one launch per 32 layers;
+ * the per-layer tables travel as kernel parameters. Layer l: src[2l] / src[2l+1] = the prompt's K / V, [num_heads,
+ * src_capacity[l], head_dim] elements of elem_bytes bytes (2: bf16 / fp16; 1: E4M3); dst[2l] / dst[2l+1] = the batched
+ * buffers [num_seqs, num_heads, dst_capacity[l], head_dim]. With elem_bytes 1, src_scales / dst_scales hold the fp32 row
+ * scales, [num_heads, src_capacity[l]] and [num_seqs, num_heads, dst_capacity[l]]; with elem_bytes 2 dst_scales is NULL.
+ * Head h copies n_h = rows[l] rows, or, when rows_dev != NULL and rows_dev[l] != NULL, n_h = min(rows[l],
+ * rows_dev[l][h]) (DEVICE int32, AdaKV / HeadKV heads). The same launch writes the decode row counts
+ *     dst_rows[l][slot*num_heads + h] = n_h - *step_dev
+ * so that the next decode step (which attends length 1 + *step_dev + rows rows) appends row n_h and attends n_h + 1 rows:
+ * the host never reads the step counter. rows[l] = 0 parks the slot (src may be NULL): each later step attends and
+ * overwrites row 0. Rows past n_h and every other slot are neither read nor written; the launch replays in a CUDA graph.
+ * PKV_ERR_INVALID_ARG: slot outside [0, num_seqs), rows above a capacity, null or misaligned pointers (16 bytes for K / V,
+ * 4 for scales and row counts), scale tables that do not match elem_bytes. */
+int pkv_cache_install(int32_t elem_bytes, int32_t num_seqs, int32_t num_heads, int32_t head_dim, int32_t device, int32_t num_layers,
+                      int32_t slot, const void* const* src, void* const* dst, const float* const* src_scales, float* const* dst_scales,
+                      const int64_t* src_capacity, const int64_t* dst_capacity, const int64_t* rows, const int32_t* const* rows_dev,
+                      int32_t* const* dst_rows, const int32_t* step_dev, void* stream);
 /* Append only (no attention): writes k_new/v_new as row length-1. */
 int pkv_cache_append(const pkv_decode_desc* d, void* stream);
 

@@ -22,7 +22,7 @@ EXPORTS = [
     "pkv_ragged_place_window", "pkv_decode_attn_ragged", "pkv_evict_single_launch", "pkv_stage_scan_pool",
     "pkv_evict_prefill_batch", "pkv_evict_batch_supported", "pkv_stage_batch", "pkv_decode_attn_batch",
     "pkv_decode_attn_batch_fp8", "pkv_cache_quantize_fp8", "pkv_decode_attn_batch_gqa", "pkv_decode_attn_batch_gqa_fp8",
-    "pkv_evict_pooled_kv_offset",
+    "pkv_evict_pooled_kv_offset", "pkv_cache_install",
 ]
 FLAG_GQA_SHARED = 128          # pkv_evict_desc.flags: one compacted cache per KV head
 
@@ -149,6 +149,10 @@ def lib() -> C.CDLL:
     # tables: src / dst / scales [2*layers] pointers, capacities and rows [layers] int64, rows_dev [layers] pointers or NULL
     L.pkv_cache_quantize_fp8.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p, p, p, p, p, p, p, p]
     L.pkv_cache_quantize_fp8.restype = i32
+    # elem_bytes, num_seqs, num_heads, head_dim, device, num_layers, slot, then the tables (src, dst, src_scales, dst_scales
+    # [2*layers] pointers; capacities and rows [layers] int64; rows_dev, dst_rows [layers] pointers), step_dev, stream
+    L.pkv_cache_install.argtypes = [C.c_int32] * 7 + [p] * 11
+    L.pkv_cache_install.restype = i32
     if L.pkv_version() != 3:
         raise RuntimeError(f"libpkv ABI version {L.pkv_version()} != 3; rebuild with `python -m pyramidkv_b200.build --force`")
     _lib = L

@@ -181,6 +181,79 @@ class PkvBatchCacheLayer(PkvCacheLayer):
         r = self.rows_host[b][h]
         return self.k_buf[b, h, :r], self.v_buf[b, h, :r]
 
+    # -- continuous batching (generate.ContinuousDecoder): one slot rewritten in place while a decode graph holds the buffers --
+    _BUFFERS = ("k_buf", "v_buf")
+
+    def admit(self, slot: int, src_layer, step: torch.Tensor, backend=None) -> None:
+        """Copy the single-prompt layer `src_layer` (the form this batch holds: `PkvCacheLayer` / `PkvRaggedCacheLayer`, or,
+        for a GQA-shared or FP8 batch, a batch-1 layer of the same group and dtype) into slot `slot`, and set the slot's
+        device row counts to src rows - *step, so that the next decode step appends after them (`pkv_cache_install`). Every
+        write is in place; `rows_host[slot]` and `seq_seen[slot]` follow."""
+        _install([self], slot, [src_layer], step, backend)
+
+    def park(self, slot: int, step: torch.Tensor, backend=None) -> None:
+        """Leave slot `slot` empty: its device row counts become -*step, so a decode step attends and overwrites one row."""
+        _install([self], slot, None, step, backend)
+
+    def grow(self, capacity: int) -> None:
+        """New buffers of `capacity` rows per (sequence, head) holding every row of the old ones (the rows the decode kernel
+        appended included). `rows` stays the same tensor; a decode graph over the old buffers must be captured again."""
+        old = self.capacity
+        if capacity <= old:
+            return
+        for name in self._BUFFERS:
+            t = getattr(self, name)
+            nt = torch.empty((t.shape[0], t.shape[1], capacity) + tuple(t.shape[3:]), dtype=t.dtype, device=t.device)
+            nt[:, :, :old] = t
+            setattr(self, name, nt)
+        self._refresh_views()
+
+    def _install_item(self, slot: int, src):
+        """(the `cache_install` tuple of this layer, the slot's host row counts, its tokens seen)."""
+        B, H, _, D = self.k_buf.shape
+        if not 0 <= int(slot) < B:
+            raise ValueError(f"slot {slot} outside [0, {B})")
+        fp8 = isinstance(self, PkvFp8CacheLayer)
+        dst = (self.k_buf, self.v_buf, (self.k_scale, self.v_scale) if fp8 else None, self.rows)
+        if src is None:
+            return (None, None, None, 0, None, *dst), [0] * H, 0
+        if fp8:
+            ok = isinstance(src, PkvFp8CacheLayer) and src.group == self.group
+        elif self.group > 1:
+            ok = isinstance(src, PkvBatchCacheLayer) and not isinstance(src, PkvFp8CacheLayer) and src.group == self.group
+        else:
+            ok = isinstance(src, PkvCacheLayer) and not isinstance(src, PkvBatchCacheLayer)
+        if not ok:
+            raise ValueError(f"admit: a {type(src).__name__} (group {getattr(src, 'group', 1)}) cannot enter a "
+                             f"{type(self).__name__} of group {self.group}: FP8 and 16-bit caches, and caches of different "
+                             "groups, do not mix")
+        if src.k_buf.shape[0] != 1 or src.k_buf.shape[1] != H or src.k_buf.shape[3] != D or src.dtype != self.dtype \
+                or src.device != self.device:
+            raise ValueError(f"admit: the source must be one prompt of {H} heads, head_dim {D}, {self.dtype} on {self.device}; "
+                             f"got {tuple(src.k_buf.shape)} {src.dtype} on {src.device}")
+        if isinstance(src, PkvRaggedCacheLayer):
+            rows_host = [r + src.appended for r in src.head_rows_host]
+            rows_dev = src.head_rows + src.appended if src.appended else src.head_rows
+            seen = src.seen_tokens
+        elif isinstance(src, PkvBatchCacheLayer):
+            rows_host = list(src.rows_host[0])
+            rows_dev = None if len(set(rows_host)) == 1 else src.rows
+            seen = src.seq_seen[0]
+        else:
+            rows_host, rows_dev, seen = [src.length] * H, None, src.seen_tokens
+        n = max(rows_host)
+        if n > self.capacity:
+            raise ValueError(f"admit: {n} rows exceed the capacity {self.capacity} (grow the batch first)")
+        scales = (src.k_scale, src.v_scale) if fp8 else None
+        return (src.k_buf, src.v_buf, scales, n, rows_dev, *dst), rows_host, seen
+
+    def _book(self, slot: int, rows_host, seen: int) -> None:
+        self.rows_host[slot] = list(rows_host)
+        self.seq_seen[slot] = int(seen)
+        self.length = max(max(r) for r in self.rows_host)
+        self.seen_tokens = max(self.seq_seen)
+        self._refresh_views()
+
     def update(self, key_states, value_states, *args, **kwargs):
         raise NotImplementedError("multi-token append to a joined batch is not defined: its sequences hold different row counts "
                                   "(decode it one token per step: generate.StaticDecoder / greedy_generate_batch)")
@@ -220,6 +293,8 @@ class PkvFp8CacheLayer(PkvBatchCacheLayer):
     row and head. Always in the per-(sequence, head) row-count form of `PkvBatchCacheLayer`, so one class holds a single
     prompt, an equal-length batch, AdaKV / HeadKV heads of different lengths and joined prompts. Decode appends one
     quantised row per sequence and step (`pkv_decode_attn_batch_fp8`)."""
+
+    _BUFFERS = ("k_buf", "v_buf", "k_scale", "v_scale")
 
     def __init__(self, k_q: torch.Tensor, v_q: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor, rows_host, seq_seen,
                  group: int = 1):
@@ -386,6 +461,36 @@ def join_caches(caches, reserve: int = 0):
             v[b, :, : l.length] = l.v_buf[0, :, : l.length]
         out.layers.append(PkvBatchCacheLayer(k, v, rows, [l.seen_tokens for l in src], group))
     return out
+
+
+def _install(layers, slot: int, sources, step: torch.Tensor, backend=None) -> None:
+    """Admit `sources[i]` (None: park) into slot `slot` of `layers[i]`, all layers in ONE backend call (`pkv_cache_install`:
+    one launch per 32 layers), then update the host mirrors."""
+    if backend is None:
+        from .kv_cluster import _default_backend as backend
+    items, books = [], []
+    for i, l in enumerate(layers):
+        if not isinstance(l, PkvBatchCacheLayer):
+            raise ValueError(f"layer {i}: slots are admitted into batched caches (join_caches), not into a {type(l).__name__}")
+        item, rows_host, seen = l._install_item(slot, None if sources is None else sources[i])
+        items.append(item)
+        books.append((rows_host, seen))
+    backend.cache_install(items, int(slot), step)
+    for l, (rows_host, seen) in zip(layers, books):
+        l._book(int(slot), rows_host, seen)
+
+
+def admit_cache(batch, slot: int, src, step: torch.Tensor, backend=None) -> None:
+    """`PkvBatchCacheLayer.admit` for every layer of the batched cache `batch` from the single-prompt cache `src` (both
+    DynamicCaches), in one launch."""
+    if len(src.layers) != len(batch.layers):
+        raise ValueError(f"admit: the source has {len(src.layers)} layers, the batch {len(batch.layers)}")
+    _install(batch.layers, slot, list(src.layers), step, backend)
+
+
+def park_cache(batch, slot: int, step: torch.Tensor, backend=None) -> None:
+    """`PkvBatchCacheLayer.park` for every layer of the batched cache `batch`, in one launch."""
+    _install(batch.layers, slot, None, step, backend)
 
 
 def layer_is_empty(past_key_values, layer_idx: int) -> bool:

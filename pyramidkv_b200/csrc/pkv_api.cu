@@ -749,6 +749,67 @@ int pkv_cache_quantize_fp8(int32_t dtype, int32_t num_seqs, int32_t num_heads, i
     return PKV_OK;
 }
 
+int pkv_cache_install(int32_t elem_bytes, int32_t num_seqs, int32_t num_heads, int32_t head_dim, int32_t device, int32_t num_layers,
+                      int32_t slot, const void* const* src, void* const* dst, const float* const* src_scales, float* const* dst_scales,
+                      const int64_t* src_capacity, const int64_t* dst_capacity, const int64_t* rows, const int32_t* const* rows_dev,
+                      int32_t* const* dst_rows, const int32_t* step_dev, void* stream) {
+    const char* fn = "pkv_cache_install";
+    if (elem_bytes != 1 && elem_bytes != 2) return fail(PKV_ERR_INVALID_ARG, "%s: elem_bytes=%d: 2 (bf16 / fp16) or 1 (E4M3)", fn, elem_bytes);
+    if (head_dim != 64 && head_dim != 128) return fail(PKV_ERR_UNSUPPORTED, "%s: head_dim=%d: only 64 and 128 are built", fn, head_dim);
+    if (num_seqs < 1 || num_heads < 1 || num_heads > 4096 || num_layers < 1)
+        return fail(PKV_ERR_INVALID_ARG, "%s: need num_seqs >= 1, 1 <= num_heads <= 4096, num_layers >= 1", fn);
+    if (slot < 0 || slot >= num_seqs) return fail(PKV_ERR_INVALID_ARG, "%s: slot %d outside [0, %d)", fn, slot, num_seqs);
+    if (!step_dev || (reinterpret_cast<uintptr_t>(step_dev) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned step counter", fn);
+    if (!dst || !dst_rows || !src_capacity || !dst_capacity || !rows) return fail(PKV_ERR_INVALID_ARG, "%s: null table", fn);
+    const bool fp8 = elem_bytes == 1;
+    if (fp8 != (dst_scales != nullptr)) return fail(PKV_ERR_INVALID_ARG, "%s: scale tables go with elem_bytes 1 (E4M3) only, and it needs them", fn);
+    for (int l = 0; l < num_layers; ++l) {
+        if (rows[l] < 0 || rows[l] > dst_capacity[l] || (rows[l] > 0 && rows[l] > src_capacity[l]))
+            return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: rows=%lld outside [0, capacity] (source %lld, destination %lld)", fn, l,
+                        (long long)rows[l], (long long)src_capacity[l], (long long)dst_capacity[l]);
+        if (!dst_rows[l] || (reinterpret_cast<uintptr_t>(dst_rows[l]) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: null or misaligned row counts", fn, l);
+        if (rows_dev && (reinterpret_cast<uintptr_t>(rows_dev[l]) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: misaligned source row counts", fn, l);
+        for (int kv = 0; kv < 2; ++kv) {
+            const void* t = dst[2 * l + kv];
+            if (!t || !aligned16(t)) return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: null or misaligned destination", fn, l);
+            if (fp8 && (!dst_scales[2 * l + kv] || (reinterpret_cast<uintptr_t>(dst_scales[2 * l + kv]) & 3u)))
+                return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: null or misaligned destination scales", fn, l);
+            if (rows[l] == 0) continue;
+            const void* s = src ? src[2 * l + kv] : nullptr;
+            if (!s || !aligned16(s)) return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: null or misaligned source", fn, l);
+            if (fp8 && (!src_scales || !src_scales[2 * l + kv] || (reinterpret_cast<uintptr_t>(src_scales[2 * l + kv]) & 3u)))
+                return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: null or misaligned source scales", fn, l);
+        }
+    }
+    const DevInfo* di = nullptr;
+    int rc = device_info(device, &di);
+    if (rc) return rc;
+    DeviceGuard guard(device);
+    for (int l0 = 0; l0 < num_layers; l0 += kMaxLayerBatch) {
+        InstallArgs a;
+        a.H = num_heads; a.slot = slot; a.step_dev = step_dev;
+        a.n_layers = std::min(kMaxLayerBatch, num_layers - l0);
+        for (int i = 0; i < a.n_layers; ++i) {
+            const int l = l0 + i;
+            InstallLayer& q = a.layer[i];
+            for (int kv = 0; kv < 2; ++kv) {
+                q.src[kv] = rows[l] > 0 ? static_cast<const uint8_t*>(src[2 * l + kv]) : nullptr;
+                q.dst[kv] = static_cast<uint8_t*>(dst[2 * l + kv]);
+                q.src_scale[kv] = fp8 && rows[l] > 0 ? src_scales[2 * l + kv] : nullptr;
+                q.dst_scale[kv] = fp8 ? dst_scales[2 * l + kv] : nullptr;
+            }
+            q.src_cap = src_capacity[l];
+            q.dst_cap = dst_capacity[l];
+            q.rows = rows[l];
+            q.rows_dev = rows_dev && rows[l] > 0 ? rows_dev[l] : nullptr;
+            q.dst_rows = dst_rows[l];
+        }
+        const cudaError_t e = launch_install(a, head_dim * elem_bytes, di->sms, static_cast<cudaStream_t>(stream));
+        if (e != cudaSuccess) return fail_cuda(e, "cache install launch");
+    }
+    return PKV_OK;
+}
+
 int pkv_decode_attn_graph(const pkv_decode_desc* d, const int32_t* step_dev, int64_t max_length, void* stream) {
     if (!step_dev) return fail(PKV_ERR_INVALID_ARG, "pkv_decode_attn_graph: null step counter");
     return decode_devlen("pkv_decode_attn_graph", d, 1, 0, nullptr, step_dev, max_length, stream);

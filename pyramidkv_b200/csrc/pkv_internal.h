@@ -160,6 +160,24 @@ struct QuantArgs {
 };
 cudaError_t launch_quantize_fp8(const QuantArgs& a, int num_sms, cudaStream_t st);
 
+// ---- admission into one slot of a batched cache (pkv_install.cu) ----
+struct InstallLayer {
+    const uint8_t* src[2];      // K, V: [H][src_cap][row_bytes] (one prompt); unused when rows == 0
+    uint8_t* dst[2];            // K, V: [num_seqs][H][dst_cap][row_bytes]
+    const float* src_scale[2];  // FP8 only: [H][src_cap]
+    float* dst_scale[2];        // FP8 only: [num_seqs][H][dst_cap]
+    int64_t src_cap, dst_cap;
+    int64_t rows;               // rows per head; with rows_dev the bound of the device counts
+    const int32_t* rows_dev;    // optional device int32 [H]
+    int32_t* dst_rows;          // device int32 [num_seqs*H]: row counts of the decode kernels
+};
+struct InstallArgs {
+    int H, slot, n_layers;      // n_layers <= kMaxLayerBatch
+    const int32_t* step_dev;
+    InstallLayer layer[kMaxLayerBatch];
+};
+cudaError_t launch_install(const InstallArgs& a, int row_bytes, int num_sms, cudaStream_t st);
+
 // RoPE in place on Q and K (pkv_rope.cu)
 struct RopeArgs {
     int dtype, Hq, Hkv, D;

@@ -21,15 +21,20 @@ With `model.config.pkv_kv_cache_dtype = "fp8_e4m3"` the prefill leaves FP8 cache
 take them as they are (the knob is the single source: no parameter here), one `pkv_decode_attn_batch_fp8` launch per layer.
 Likewise with `model.config.pkv_gqa_shared = True` (one cache per KV head, `group` > 1): one `pkv_decode_attn_batch_gqa(_fp8)`
 launch per layer.
+
+`greedy_generate_continuous` keeps a fixed number of slots busy: when a sequence stops (EOS or its own `max_new_tokens`),
+the next waiting prompt is prefilled and copied into its slot in place (`pkv_cache_install`, one launch for every layer),
+while the captured step graph keeps replaying unchanged.
 """
 from __future__ import annotations
 
+import time
 from dataclasses import dataclass
 from typing import Optional
 
 import torch
 
-from .cache import PkvBatchCacheLayer, PkvCacheLayer, PkvRaggedCacheLayer, join_caches
+from .cache import PkvBatchCacheLayer, PkvCacheLayer, PkvRaggedCacheLayer, admit_cache, join_caches, park_cache
 
 
 @dataclass
@@ -81,8 +86,8 @@ class StaticDecoder:
         self.use_graph = (dev.type == "cuda") if use_graph is None else bool(use_graph)
         cache._pkv_static = self.state
 
-    # one greedy step; every tensor it touches is static, every launch argument constant
-    def _step(self) -> None:
+    def _greedy_token(self) -> torch.Tensor:
+        """The forward of one token per sequence through every layer (appending to the cache); the argmax [B, 1]."""
         m = self.model.model
         h = m.embed_tokens(self.ids)
         pos_emb = m.rotary_emb(h, position_ids=self.pos)
@@ -91,7 +96,11 @@ class StaticDecoder:
                       past_key_values=self.cache, use_cache=True)
         h = m.norm(h)
         logits = self.model.lm_head(h[:, -1, :])
-        nxt = logits.argmax(dim=-1, keepdim=True)                       # [B, 1]
+        return logits.argmax(dim=-1, keepdim=True)                      # [B, 1]
+
+    # one greedy step; every tensor it touches is static, every launch argument constant
+    def _step(self) -> None:
+        nxt = self._greedy_token()
         if self.done is not None:
             nxt = torch.where(self.done, self.pad_token_id, nxt)
             self.done.logical_or_((nxt == self.eos[None, :]).any(dim=1, keepdim=True))
@@ -101,9 +110,13 @@ class StaticDecoder:
         self.cursor.add_(1)
         self.state.step.add_(1)
 
+    def _counters(self) -> list:
+        """The device tensors a step advances (restored after the warm-up step of a capture)."""
+        return [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done) if t is not None]
+
     def _capture(self) -> None:
         # warm up on a side stream (lazy initialisation, cuBLAS workspaces), restore the counters, then capture
-        state = [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done) if t is not None]
+        state = self._counters()
         snap = [t.clone() for t in state]
         s = torch.cuda.Stream(device=self.ids.device)
         s.wait_stream(torch.cuda.current_stream(self.ids.device))
@@ -242,3 +255,209 @@ def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None
         dec.finish(kept)
     seqs = [torch.cat([p[0].cpu(), first[b].cpu(), gen[b, : kept[b]]]).to(p.device) for b, p in enumerate(ids)]
     return (seqs, cache) if return_cache else seqs
+
+
+class ContinuousDecoder(StaticDecoder):
+    """The step of `StaticDecoder` over a fixed set of slots whose sequences come and go (continuous batching).
+
+    cache: a batched cache (`join_caches`) of B slots; first_token [B] the next input per slot; left[b] the decode steps slot b
+    may still take. Per step, on the device: a slot becomes `done` when its `left` reaches 0 or it emits an EOS; a done slot
+    emits `pad_token_id`, and its row counts stop growing (each later step attends and overwrites the same row). The token
+    buffer holds one chunk, [B, chunk]; `run_chunk` replays `steps` steps, reads them with one device-to-host copy and
+    resets the cursor in place. Between chunks `admit` copies a prefilled prompt into a slot and `park` empties one; both
+    write the buffers and row counts in place, so the captured graph keeps replaying. `grow_for` reallocates the buffers
+    when an admission needs more rows; the graph is then captured again."""
+
+    def __init__(self, model, cache, first_token: torch.Tensor, left, chunk: int, use_graph: Optional[bool] = None,
+                 eos_token_id=None, pad_token_id: int = 0):
+        self.model, self.cache, self.max_steps = model, cache, max(1, int(chunk))
+        layers = [l for l in cache.layers if isinstance(l, PkvBatchCacheLayer)]
+        if len(layers) != model.config.num_hidden_layers or len(layers) != len(cache.layers):
+            raise RuntimeError("ContinuousDecoder needs a batched cache (cache.join_caches) on every layer")
+        self.layers = layers
+        dev = layers[0].device
+        bsz = layers[0].k_buf.shape[0]
+        self.backend = model.model.layers[0].self_attn.kv_cluster.backend
+        hq, d = layers[0].num_q_heads, layers[0].k_buf.shape[3]
+        self.state = _StaticState(step=torch.zeros(1, dtype=torch.int32, device=dev),
+                                  workspace=self.backend.decode_workspace(bsz * hq, d, dev))
+        # every layer's row counts are rows of one tensor, so one op per step stops them growing for the done slots
+        self.rows_all = torch.stack([l.rows for l in layers])
+        for i, l in enumerate(layers):
+            l.rows = self.rows_all[i]
+        self.ids = first_token.reshape(bsz, 1).to(device=dev, dtype=torch.long).clone()
+        self.pos = torch.tensor(layers[0].seq_seen, dtype=torch.long, device=dev).reshape(bsz, 1)
+        self.cursor = torch.zeros(1, dtype=torch.long, device=dev)
+        self.tokens = torch.zeros(bsz, self.max_steps, dtype=torch.long, device=dev)
+        self.left = torch.tensor([int(n) for n in left], dtype=torch.long, device=dev).reshape(bsz, 1)
+        self.eos = None
+        if eos_token_id is not None:
+            eos = eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id]
+            self.eos = torch.tensor([int(e) for e in eos], dtype=torch.long, device=dev)
+        self.done = self.left <= 0
+        self.pad_token_id = int(pad_token_id)
+        self.taken = 0
+        self.graph = None
+        self.captures = 0
+        self.parked = set()
+        self.use_graph = (dev.type == "cuda") if use_graph is None else bool(use_graph)
+        cache._pkv_static = self.state
+
+    def _step(self) -> None:
+        nxt = torch.where(self.done, self.pad_token_id, self._greedy_token())
+        self.left.sub_(1)
+        stop = self.left <= 0
+        if self.eos is not None:
+            stop.logical_or_((nxt == self.eos[None, :]).any(dim=1, keepdim=True))
+        self.done.logical_or_(stop)
+        self.rows_all.view(len(self.layers), self.done.shape[0], -1).sub_(self.done.view(1, -1, 1).to(torch.int32))
+        self.tokens.index_copy_(1, self.cursor, nxt)
+        self.ids.copy_(nxt)
+        self.pos.add_(1)
+        self.cursor.add_(1)
+        self.state.step.add_(1)
+
+    def _counters(self) -> list:
+        return super()._counters() + [self.left, self.rows_all]
+
+    def _capture(self) -> None:
+        super()._capture()
+        self.captures += 1
+
+    def run_chunk(self, steps: int) -> torch.Tensor:
+        """Take `steps` (<= chunk) steps; their tokens [B, steps] on the host."""
+        self.run(steps)
+        toks = self.tokens[:, :steps].cpu()
+        self.cursor.zero_()
+        self.taken = 0
+        return toks
+
+    def grow_for(self, src_cache, new_tokens: int) -> bool:
+        """Make every layer hold the rows of the single-prompt cache `src_cache` plus `new_tokens` (amortised doubling, like
+        `reserve`). True when a buffer was reallocated (the graph is then captured again on the next chunk)."""
+        grew = False
+        for l, s in zip(self.layers, src_cache.layers):
+            need = s.length + int(new_tokens)
+            if need > l.capacity:
+                l.grow(max(need, l.capacity + max(64, l.capacity // 2)))
+                grew = True
+        if grew:
+            self.graph = None
+        return grew
+
+    def admit(self, slot: int, src_cache, first_token: torch.Tensor, left: int) -> None:
+        """Slot `slot` continues the prefilled prompt `src_cache` (first token `first_token`, `left` decode steps)."""
+        admit_cache(self.cache, slot, src_cache, self.state.step, self.backend)
+        self.ids[slot] = first_token.reshape(-1)[:1].to(self.ids.device)
+        self.pos[slot] = self.layers[0].seq_seen[slot]
+        self.left[slot] = int(left)
+        self.done[slot] = int(left) <= 0
+        self.parked.discard(slot)
+
+    def park(self, slot: int) -> None:
+        if slot in self.parked:
+            return
+        park_cache(self.cache, slot, self.state.step, self.backend)
+        self.ids[slot] = self.pad_token_id
+        self.done[slot] = True
+        self.parked.add(slot)
+
+    def finish(self, kept=None) -> None:
+        """Leave static mode. The slots' host row counts are those of their admissions (the decoded rows are not booked)."""
+        if getattr(self.cache, "_pkv_static", None) is self.state:
+            del self.cache._pkv_static
+        self.graph = None
+        self.taken = 0
+
+
+def _sync(device: torch.device) -> None:
+    if device.type == "cuda":
+        torch.cuda.synchronize(device)
+
+
+@torch.no_grad()
+def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, eos_token_id=None, pad_token_id: int = 0,
+                               use_graph: Optional[bool] = None, check_every: int = 16, return_stats: bool = False):
+    """Greedy generation for any number of prompts (1-D or [1, S] id tensors) through `num_slots` sequences decoded together
+    (continuous batching). `max_new_tokens`: an int, or one per prompt. The first `num_slots` prompts are prefilled one at a
+    time and joined exactly as in `greedy_generate_batch`; decoding then runs in chunks of `check_every` steps. After each
+    chunk the host reads its tokens once, retires every sequence that emitted an EOS (kept) or reached its own
+    `max_new_tokens`, and prefills the next waiting prompts in order, each into a free slot (`ContinuousDecoder.admit`); a
+    slot with nothing left to admit is parked. Returns one 1-D tensor per prompt, in prompt order, prompt + generated (the
+    format of `greedy_generate_batch`), and with `return_stats` a dict: decode_steps, live_slot_steps (the sum over steps
+    of the slots holding an unfinished sequence), admissions (prompts admitted after the start), regrowths, graph_captures,
+    prefill_s / decode_s (host wall time of the prefills and of the rest of the loop) and per prompt `prefill_ms` and
+    `cache_rows_first_last` (rows of its first and last layer after the prefill)."""
+    ids = [p.reshape(1, -1) for p in prompts]
+    if not ids:
+        raise ValueError("greedy_generate_continuous: no prompts")
+    caps = [int(n) for n in max_new_tokens] if isinstance(max_new_tokens, (list, tuple)) else [int(max_new_tokens)] * len(ids)
+    if len(caps) != len(ids):
+        raise ValueError(f"greedy_generate_continuous: {len(caps)} max_new_tokens for {len(ids)} prompts")
+    if int(num_slots) < 1:
+        raise ValueError(f"greedy_generate_continuous: num_slots must be >= 1, got {num_slots}")
+    eos = _eos_set(eos_token_id)
+    chunk = max(1, int(check_every))
+    dev = ids[0].device
+    gen = [[] for _ in ids]                        # generated tokens per prompt, the prefill's first token included
+    stats = dict(decode_steps=0, live_slot_steps=0, admissions=0, regrowths=0, graph_captures=0, prefill_s=0.0, decode_s=0.0,
+                 prefill_ms=[0.0] * len(ids), cache_rows_first_last=[[] for _ in ids])
+    t_start = time.perf_counter()
+
+    def finished(i):
+        return len(gen[i]) >= max(1, caps[i]) or gen[i][-1] in eos
+
+    def prefill(i):
+        _sync(dev)
+        t0 = time.perf_counter()
+        first, cache = _prefill(model, ids[i])
+        gen[i].append(int(first))                  # waits for the prefill
+        ms = (time.perf_counter() - t0) * 1e3
+        stats["prefill_ms"][i] = ms
+        stats["prefill_s"] += ms / 1e3
+        stats["cache_rows_first_last"][i] = [int(cache.layers[0].length), int(cache.layers[-1].length)]
+        return first, cache
+
+    B = min(int(num_slots), len(ids))
+    firsts, caches = zip(*[prefill(i) for i in range(B)])
+    cache = join_caches(list(caches), reserve=max(caps))
+    del caches
+    slot_req = list(range(B))
+    dec = ContinuousDecoder(model, cache, torch.cat(firsts), [0 if finished(b) else caps[b] - 1 for b in range(B)], chunk,
+                            use_graph=use_graph, eos_token_id=sorted(eos) if eos else None, pad_token_id=pad_token_id)
+    waiting = B
+    while True:
+        for s in range(B):
+            if slot_req[s] is not None and not finished(slot_req[s]):
+                continue
+            slot_req[s] = None
+            while waiting < len(ids) and slot_req[s] is None:
+                i = waiting
+                waiting += 1
+                first, single = prefill(i)
+                if finished(i):
+                    continue
+                stats["regrowths"] += int(dec.grow_for(single, caps[i]))
+                dec.admit(s, single, first, caps[i] - 1)
+                stats["admissions"] += 1
+                slot_req[s] = i
+            if slot_req[s] is None:
+                dec.park(s)
+        live = [s for s in range(B) if slot_req[s] is not None]
+        if not live:
+            break
+        n = min(chunk, max(caps[slot_req[s]] - len(gen[slot_req[s]]) for s in live))
+        toks = dec.run_chunk(n)                    # one device-to-host read per chunk
+        stats["decode_steps"] += n
+        for s in live:
+            r = slot_req[s]
+            for t in toks[s].tolist():
+                gen[r].append(t)
+                stats["live_slot_steps"] += 1
+                if finished(r):
+                    break
+    dec.finish()
+    stats["graph_captures"] = dec.captures
+    stats["decode_s"] = time.perf_counter() - t_start - stats["prefill_s"]
+    seqs = [torch.cat([p[0].cpu(), torch.tensor(g, dtype=torch.long)]).to(p.device) for p, g in zip(ids, gen)]
+    return (seqs, stats) if return_stats else seqs

@@ -90,6 +90,10 @@ class CudaBackend:
         return ops.decode_attn_batch_gqa_fp8(q, k_q, v_q, k_scale, v_scale, length, k_new, v_new, rows, step, max_length, workspace,
                                              out, softmax_scale)
 
+    # -- continuous batching: one prompt's compacted cache into one slot of a batched cache --
+    def cache_install(self, layers, slot, step):
+        ops.cache_install(layers, slot, step)
+
     def rope_inplace(self, q, k, cos, sin):
         ops.rope_inplace(q, k, cos, sin)
 

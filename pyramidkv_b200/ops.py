@@ -682,6 +682,77 @@ def decode_attn_batch_gqa_fp8(q: torch.Tensor, k_q: torch.Tensor, v_q: torch.Ten
                        softmax_scale, scales=(k_scale, v_scale))
 
 
+# ---- continuous batching: admission into one slot of a batched cache (include/pkv.h: pkv_cache_install) ----
+def cache_install(layers, slot: int, step: torch.Tensor) -> None:
+    """Copy one prompt's compacted cache into slot `slot` of batched caches, every layer in one launch per 32 layers
+    (`pkv_cache_install`), and set the slot's decode row counts to `rows - *step` on the device. `layers`: per layer
+    (src_k, src_v, src_scales, rows, rows_dev, dst_k, dst_v, dst_scales, dst_rows) with src_k / src_v the prompt's
+    contiguous [1, H, capacity, D] buffers (None when rows == 0: parking), dst_k / dst_v the batched [B, H, capacity', D]
+    buffers of the same dtype (bf16 / fp16, or float8_e4m3fn with (k_scale, v_scale) float32 scales of shape [.., capacity]
+    as src_scales / dst_scales), `rows` the rows per head, `rows_dev` an optional int32 [H] device count per head (at most
+    `rows`) and dst_rows the int32 [B*H] row counts the decode kernels read. `step`: the int32 [1] device step counter."""
+    layers = list(layers)
+    if not layers:
+        return
+    k0 = layers[0][5]
+    B, H, _, D = k0.shape
+    fp8 = k0.dtype == FP8_DTYPE
+    if not fp8 and k0.dtype not in (torch.bfloat16, torch.float16):
+        raise ValueError(f"cache_install: unsupported cache dtype {k0.dtype}")
+    if step.dtype != torch.int32 or step.numel() != 1:
+        raise ValueError("cache_install: step must be an int32 device tensor with one element")
+    _require_cuda(step)
+    n = len(layers)
+    src, dst = (C.c_void_p * (2 * n))(), (C.c_void_p * (2 * n))()
+    sscl, dscl = (C.c_void_p * (2 * n))(), (C.c_void_p * (2 * n))()
+    scap, dcap, rows_t = (C.c_int64 * n)(), (C.c_int64 * n)(), (C.c_int64 * n)()
+    rdev, drows = (C.c_void_p * n)(), (C.c_void_p * n)()
+    for i, (sk, sv, ss, rows, rows_dev, dk, dv, ds, dr) in enumerate(layers):
+        what = f"cache_install: layer {i}"
+        _require_cuda(sk, sv, rows_dev, dk, dv, dr, *(ss or ()), *(ds or ()))
+        if dk.dim() != 4 or dk.shape != dv.shape or not dk.is_contiguous() or not dv.is_contiguous():
+            raise ValueError(f"{what}: the batched buffers must be contiguous [B, H, capacity, D] tensors of equal shape")
+        if dk.dtype != k0.dtype or dv.dtype != k0.dtype or (dk.shape[0], dk.shape[1], dk.shape[3]) != (B, H, D) or dk.device != k0.device:
+            raise ValueError(f"{what}: batch, heads, head_dim, dtype and device must match layer 0")
+        if fp8:
+            if ds is None:
+                raise ValueError(f"{what}: an FP8 cache needs its scales")
+            _check_fp8_buffers(dk, dv, ds[0], ds[1], what)
+        elif ds is not None or ss is not None:
+            raise ValueError(f"{what}: scales go with FP8 caches only")
+        if dr.dtype != torch.int32 or dr.numel() != B * H or not dr.is_contiguous():
+            raise ValueError(f"{what}: dst_rows must be a contiguous int32 device tensor of B*H = {B * H} elements")
+        rows = int(rows)
+        if rows > 0:
+            if sk is None or sv is None or sk.shape != sv.shape or sk.dim() != 4 or sk.shape[0] != 1 \
+                    or not sk.is_contiguous() or not sv.is_contiguous():
+                raise ValueError(f"{what}: the source must be contiguous [1, H, capacity, D] buffers of equal shape")
+            if sk.dtype != dk.dtype or sv.dtype != dk.dtype:
+                raise ValueError(f"{what}: source dtype {sk.dtype} differs from the batched cache's {dk.dtype}")
+            if sk.shape[1] != H or sk.shape[3] != D:
+                raise ValueError(f"{what}: source heads / head_dim {tuple(sk.shape[1::2])} differ from the batched cache's ({H}, {D})")
+            if fp8:
+                if ss is None:
+                    raise ValueError(f"{what}: an FP8 source needs its scales")
+                _check_fp8_buffers(sk, sv, ss[0], ss[1], what)
+            if rows_dev is not None and (rows_dev.dtype != torch.int32 or rows_dev.numel() != H or not rows_dev.is_contiguous()):
+                raise ValueError(f"{what}: rows_dev must be a contiguous int32 device tensor of H = {H} elements")
+            src[2 * i], src[2 * i + 1] = sk.data_ptr(), sv.data_ptr()
+            scap[i] = sk.shape[2]
+            if fp8:
+                sscl[2 * i], sscl[2 * i + 1] = ss[0].data_ptr(), ss[1].data_ptr()
+            rdev[i] = rows_dev.data_ptr() if rows_dev is not None else None
+        dst[2 * i], dst[2 * i + 1] = dk.data_ptr(), dv.data_ptr()
+        if fp8:
+            dscl[2 * i], dscl[2 * i + 1] = ds[0].data_ptr(), ds[1].data_ptr()
+        dcap[i], rows_t[i], drows[i] = dk.shape[2], rows, dr.data_ptr()
+    dev = k0.device.index if k0.device.index is not None else torch.cuda.current_device()
+    _lib.check(_lib.lib().pkv_cache_install(1 if fp8 else 2, B, H, D, dev, n, int(slot), src, dst, sscl if fp8 else None,
+                                            dscl if fp8 else None, scap, dcap, rows_t,
+                                            rdev if any(r is not None for r in rdev) else None, drows, step.data_ptr(),
+                                            torch.cuda.current_stream(k0.device).cuda_stream))
+
+
 def decode_workspace_bytes(num_q_heads: int, head_dim: int) -> int:
     """Upper bound of the decode workspace for any cache length (`pkv_decode_workspace_bytes`)."""
     d = DecodeDesc()

@@ -253,6 +253,29 @@ def _run_batch_static(model, prompts: List[torch.Tensor], max_new_tokens: int, u
     return res, per_seq * len(prompts)
 
 
+def _run_continuous(model, prompts: List[torch.Tensor], max_new_tokens: List[int], slots: int):
+    """All prompts through one greedy_generate_continuous with `slots` slots (graph replay), after an untimed warm-up prefill
+    per prompt length. Returns (one PromptResult per prompt, the run's `continuous` record block)."""
+    from .generate import _prefill, greedy_generate_continuous
+    dev = prompts[0].device
+    with torch.no_grad():
+        for n in sorted({int(p.shape[1]) for p in prompts}):
+            _prefill(model, next(p for p in prompts if p.shape[1] == n))
+        _sync(dev)
+        seqs, st = greedy_generate_continuous(model, prompts, max_new_tokens, slots, return_stats=True)
+    steps = st["decode_steps"]
+    block = {"slots": min(slots, len(prompts)), "decode_steps": steps,
+             "occupancy": st["live_slot_steps"] / max(1, min(slots, len(prompts)) * steps),
+             "aggregate_tok_per_s": st["live_slot_steps"] / max(st["decode_s"], 1e-9),
+             "admissions": st["admissions"], "regrowths": st["regrowths"], "graph_captures": st["graph_captures"]}
+    res = []
+    for i, (p, n, s) in enumerate(zip(prompts, max_new_tokens, seqs)):
+        pred = s[p.shape[1]:].tolist()
+        rows = [r + len(pred) - 1 for r in st["cache_rows_first_last"][i]]      # the decoded tokens' rows, as the other loops book them
+        res.append(PromptResult(int(p.shape[1]), n, st["prefill_ms"][i], 0.0, rows, pred))
+    return res, block
+
+
 def run_prompt(model, ids: torch.Tensor, max_new_tokens: int, decode_loop: str = "hf") -> PromptResult:
     """Greedy generate exactly as the reference runner does. One untimed warm-up call at this prompt length (allocator,
     cuBLAS heuristics, lazy module init), then two timed calls: one new token (prefill + eviction of all layers) and the
@@ -300,7 +323,10 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
     kv_cache_dtype "fp8_e4m3": the compacted caches are converted to FP8 after the prefill (model.config.pkv_kv_cache_dtype);
     the records then carry "kv_cache_dtype". "auto" (the default) changes nothing.
     gqa_shared: one selection and one compacted cache per KV head (model.config.pkv_gqa_shared); the records then carry
-    "gqa_shared". FullKV, AdaKV and HeadKV refuse it."""
+    "gqa_shared". FullKV, AdaKV and HeadKV refuse it.
+    decode_loop "continuous": every prompt goes through one greedy_generate_continuous with eval_batch_size slots, whatever
+    its max_new_tokens; each record keeps its own prefill_ms, cache rows and tokens and carries the run's "continuous" block
+    (slots, decode_steps, occupancy, aggregate_tok_per_s) instead of a per-prompt decode rate."""
     if kv_cache_dtype not in ("auto", "fp8_e4m3"):
         raise ValueError(f"kv_cache_dtype must be auto or fp8_e4m3, got {kv_cache_dtype!r}")
     if kv_cache_dtype != "auto" and canonical_method(method) == "fullkv":
@@ -311,11 +337,12 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
                                   + ("keeps HF's own cache" if canonical_method(method) == "fullkv" else "sets budgets per query head"))
     if eval_batch_size < 1:
         raise ValueError(f"eval_batch_size must be >= 1, got {eval_batch_size}")
-    if eval_batch_size > 1 and (decode_loop == "hf" or canonical_method(method) == "fullkv"):
+    continuous = decode_loop == "continuous"
+    if (eval_batch_size > 1 or continuous) and (decode_loop == "hf" or canonical_method(method) == "fullkv"):
         raise NotImplementedError("eval_batch_size > 1 decodes the joined compacted caches of the prompts with the static loop: "
                                   "use --decode_loop static or static-eager with an eviction method (padded HF batches are not supported)")
-    if decode_loop not in ("hf", "static", "static-eager"):
-        raise ValueError(f"decode_loop must be hf, static or static-eager, got {decode_loop!r}")
+    if decode_loop not in ("hf", "static", "static-eager", "continuous"):
+        raise ValueError(f"decode_loop must be hf, static, static-eager or continuous, got {decode_loop!r}")
     if device is None:
         if not torch.cuda.is_available():
             raise RuntimeError("the runners need a CUDA device (H100, sm_90a); there is no CPU fallback")
@@ -335,8 +362,35 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
             model.config.pkv_gqa_shared = True
         records = []
         prompts = list(prompts)
-        if eval_batch_size > 1 and max_capacity_prompt == -1 and capacity_ratio != -1 and len({p[1] for p in prompts}) > 1:
+        if (eval_batch_size > 1 or continuous) and max_capacity_prompt == -1 and capacity_ratio != -1 and len({p[1] for p in prompts}) > 1:
             raise NotImplementedError("--max_capacity_prompts_ratio sets a budget per prompt length; batch prompts of one length")
+
+        def emit(group, rs, extra):
+            for j, r in zip(group, rs):
+                rec = {"task": prompts[j][0], "arch": arch, "method": method,
+                       "max_capacity_prompt": model.config.max_capacity_prompt if method != "fullkv" else max_capacity_prompt, "window": window,
+                       "decode_loop": decode_loop if method != "fullkv" else "hf",
+                       **({"kv_cache_dtype": kv_cache_dtype} if kv_cache_dtype != "auto" else {}),
+                       **({"gqa_shared": True} if gqa_shared else {}),
+                       "dtype": str(dtype).replace("torch.", ""), "data": "synthetic token ids, random-init weights", **(tag or {}),
+                       "prompt_tokens": r.prompt_tokens, "new_tokens": r.new_tokens, "prefill_ms": r.prefill_ms,
+                       **({} if continuous else {"decode_tok_per_s": r.decode_tok_per_s}), **extra,
+                       "cache_rows_first_last": r.cache_rows_first_last, "pred_ids": r.pred_ids}
+                records.append(rec)
+                print(json.dumps({k: v for k, v in rec.items() if k != "pred_ids"}), flush=True)
+                if out_path:
+                    os.makedirs(os.path.dirname(os.path.abspath(out_path)), exist_ok=True)
+                    with open(out_path, "a") as f:
+                        f.write(json.dumps(rec) + "\n")
+
+        if continuous:
+            if prompts and max_capacity_prompt == -1 and capacity_ratio != -1:
+                window = set_knobs(model, method, round(prompts[0][1] * capacity_ratio), merge, backend_factory, floor, head_beta, head_path)
+            ids = [synthetic_prompt(model.config.vocab_size, p[1], seed + j, device) for j, p in enumerate(prompts)]
+            if ids:
+                rs, block = _run_continuous(model, ids, [p[2] for p in prompts], eval_batch_size)
+                emit(range(len(prompts)), rs, {"continuous": block})
+            return records
         i = 0
         while i < len(prompts):
             group = [i]                                   # consecutive prompts decoded together: same max_new_tokens
@@ -353,21 +407,7 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
                 batch = {"eval_batch_size": eval_batch_size, "batch_size": len(group), "batch_decode_tok_per_s_aggregate": agg}
             else:
                 rs = [run_prompt(model, ids[0], prompts[i][2], decode_loop if method != "fullkv" else "hf")]
-            for j, r in zip(group, rs):
-                rec = {"task": prompts[j][0], "arch": arch, "method": method,
-                       "max_capacity_prompt": model.config.max_capacity_prompt if method != "fullkv" else max_capacity_prompt, "window": window,
-                       "decode_loop": decode_loop if method != "fullkv" else "hf",
-                       **({"kv_cache_dtype": kv_cache_dtype} if kv_cache_dtype != "auto" else {}),
-                       **({"gqa_shared": True} if gqa_shared else {}),
-                       "dtype": str(dtype).replace("torch.", ""), "data": "synthetic token ids, random-init weights", **(tag or {}),
-                       "prompt_tokens": r.prompt_tokens, "new_tokens": r.new_tokens, "prefill_ms": r.prefill_ms,
-                       "decode_tok_per_s": r.decode_tok_per_s, **batch, "cache_rows_first_last": r.cache_rows_first_last, "pred_ids": r.pred_ids}
-                records.append(rec)
-                print(json.dumps({k: v for k, v in rec.items() if k != "pred_ids"}), flush=True)
-                if out_path:
-                    os.makedirs(os.path.dirname(os.path.abspath(out_path)), exist_ok=True)
-                    with open(out_path, "a") as f:
-                        f.write(json.dumps(rec) + "\n")
+            emit(group, rs, batch)
             i = group[-1] + 1
         return records
     finally:

@@ -53,8 +53,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--chat_formatting_function", type=str, default="")
     p.add_argument("--dtype", type=str, default="float16", choices=["float16", "bfloat16"], help="the reference loads fp16 (:388)")
     p.add_argument("--prompt_tokens", type=int, default=0, help="override the task's typical prompt length")
-    p.add_argument("--decode_loop", type=str, default="hf", choices=["hf", "static", "static-eager"],
-                   help="hf: model.generate as in the reference; static: pyramidkv_b200.generate (CUDA-graph replay per token)")
+    p.add_argument("--decode_loop", type=str, default="hf", choices=["hf", "static", "static-eager", "continuous"],
+                   help="hf: model.generate as in the reference; static: pyramidkv_b200.generate (CUDA-graph replay per token); "
+                        "continuous: every prompt through --eval_batch_size slots, a finished sequence's slot taking the next prompt")
     p.add_argument("--kv_cache_dtype", type=str, default="auto", choices=["auto", "fp8_e4m3"],
                    help="auto: the compacted cache in the model dtype; fp8_e4m3: FP8 bytes + one fp32 scale per row (half the KV bytes)")
     p.add_argument("--gqa_shared", action="store_true",
@@ -97,7 +98,8 @@ def main(argv=None, backend_factory=None, device=None):
     n = len(recs)
     print(json.dumps({"summary": True, "arch": arch, "method": method, "max_capacity_prompts": capacity, "examples": n,
                       "mean_prefill_ms": sum(r["prefill_ms"] for r in recs) / n,
-                      "mean_decode_tok_per_s": sum(r["decode_tok_per_s"] for r in recs) / n}))
+                      **({"continuous": recs[0]["continuous"]} if "continuous" in recs[0] else
+                         {"mean_decode_tok_per_s": sum(r["decode_tok_per_s"] for r in recs) / n})}))
     return recs
 
 
