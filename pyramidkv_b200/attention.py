@@ -22,8 +22,8 @@ from typing import Callable, Optional
 import torch
 from transformers.modeling_utils import ALL_ATTENTION_FUNCTIONS
 
-from .cache import (PkvBatchCacheLayer, PkvCacheLayer, PkvFp8CacheLayer, PkvRaggedCacheLayer, gqa_shared, install_layer,
-                    kv_cache_dtype, layer_is_empty, quantize_caches_fp8)
+from .cache import (PkvBatchCacheLayer, PkvCacheLayer, PkvRaggedCacheLayer, gqa_shared, install_layer, kv_cache_dtype,
+                    layer_is_empty, quantize_caches_fp8)
 from .kv_cluster import INIT_BY_METHOD, flush_pending
 
 DEFAULT_DECODE_RESERVE = 256   # rows of head-room behind the compacted prompt (grows by doubling)
@@ -160,72 +160,17 @@ def make_forward(method: str, modeling, original_forward):
             self.kv_seq_len = getattr(self, "kv_seq_len", layer.seen_tokens) + q_len
             attn_weights = None
             static = getattr(past_key_values, "_pkv_static", None)
-            ragged = isinstance(layer, PkvRaggedCacheLayer)
-            joined = isinstance(layer, PkvBatchCacheLayer)
-            # rows = `rows_arg` (+ head_rows[h] for ragged caches, + the device step counter in static mode)
-            rows_arg = (layer.appended if ragged else layer.length) + 1
-            head_rows = {"head_rows": layer.head_rows} if ragged else {}
-            if q_len == 1 and getattr(layer, "group", 1) > 1:
-                # GQA-shared cache (knob pkv_gqa_shared): one launch for any batch size, host-launched or in the static loop's
-                # graph; each KV head's rows are read once for its group; rows = layer.rows[b, j] + 1 (+ the step counter)
+            if q_len == 1:
+                # one launch per layer: the new row is appended in place and attended (the cache form picks the kernel).
+                # In the static loop (generate.StaticDecoder) the buffers were reserved up front, the row count includes the
+                # device step counter and StaticDecoder.finish() settles the Python bookkeeping.
                 if static is None:
                     layer.reserve(1)
-                kw = dict(rows=layer.rows, step=static.step if static is not None else None, max_length=layer.capacity,
-                          workspace=static.workspace if static is not None else None, softmax_scale=self.scaling)
-                q1, k1, v1 = query_states[:, :, 0, :], key_states[:, :, 0, :], value_states[:, :, 0, :]
-                if isinstance(layer, PkvFp8CacheLayer):
-                    out = cluster.backend.decode_attn_batch_gqa_fp8(q1, layer.k_buf, layer.v_buf, layer.k_scale, layer.v_scale, 1,
-                                                                    k1, v1, **kw)
-                else:
-                    out = cluster.backend.decode_attn_batch_gqa(q1, layer.k_buf, layer.v_buf, 1, k1, v1, **kw)
+                out = layer.decode(cluster.backend, query_states[:, :, 0, :], key_states[:, :, 0, :], value_states[:, :, 0, :],
+                                   static, self.scaling)
                 if static is None:
                     layer.advance(1)
                 attn_output = out[:, None]
-            elif q_len == 1 and isinstance(layer, PkvFp8CacheLayer):
-                # FP8 cache (knob pkv_kv_cache_dtype): one launch for any batch size, host-launched or in the static loop's
-                # graph; rows = layer.rows[b, h] + 1 (+ the device step counter in static mode). The kernel quantises the new
-                # K / V row and attends it as stored.
-                if static is None:
-                    layer.reserve(1)
-                out = cluster.backend.decode_attn_batch_fp8(
-                    query_states[:, :, 0, :], layer.k_buf, layer.v_buf, layer.k_scale, layer.v_scale, 1,
-                    key_states[:, :, 0, :], value_states[:, :, 0, :], rows=layer.rows,
-                    step=static.step if static is not None else None, max_length=layer.capacity,
-                    workspace=static.workspace if static is not None else None, softmax_scale=self.scaling)
-                if static is None:
-                    layer.advance(1)
-                attn_output = out[:, None]
-            elif q_len == 1 and (bsz > 1 or joined):
-                # several sequences: ONE launch for the batch. Rows = layer.length + 1 (equal-length batched prefill) or
-                # layer.rows[b, h] + 1 (joined prompts), + the device step counter in static mode
-                if static is None:
-                    layer.reserve(1)
-                out = cluster.backend.decode_attn_batch(
-                    query_states[:, :, 0, :], layer.k_buf, layer.v_buf, 1 if joined else layer.length + 1,
-                    key_states[:, :, 0, :], value_states[:, :, 0, :], rows=layer.rows if joined else None,
-                    step=static.step if static is not None else None, max_length=layer.capacity,
-                    workspace=static.workspace if static is not None else None, softmax_scale=self.scaling)
-                if static is None:
-                    layer.advance(1)
-                attn_output = out[:, None]
-            elif q_len == 1 and static is not None:
-                # graph-replayable step (generate.StaticDecoder): the row count is layer.length + 1 + *static.step on the
-                # device, the buffers were reserved up front and the Python bookkeeping is settled by StaticDecoder.finish()
-                out = torch.empty(bsz, 1, num_q_heads, self.head_dim, dtype=query_states.dtype, device=query_states.device)
-                for b in range(bsz):
-                    cluster.backend.decode_attn(query_states[b, :, 0, :], layer.k_buf[b], layer.v_buf[b], rows_arg,
-                                                key_states[b, :, 0, :], value_states[b, :, 0, :], out[b, 0], softmax_scale=self.scaling,
-                                                step=static.step, max_length=layer.capacity, workspace=static.workspace, **head_rows)
-                attn_output = out
-            elif q_len == 1:
-                layer.reserve(1)
-                out = torch.empty(bsz, 1, num_q_heads, self.head_dim, dtype=query_states.dtype, device=query_states.device)
-                for b in range(bsz):
-                    cluster.backend.decode_attn(query_states[b, :, 0, :], layer.k_buf[b], layer.v_buf[b], rows_arg,
-                                                key_states[b, :, 0, :], value_states[b, :, 0, :], out[b, 0], softmax_scale=self.scaling,
-                                                **({"max_length": layer.capacity, **head_rows} if ragged else {}))
-                layer.advance(1)
-                attn_output = out
             else:
                 # several new tokens after the prefill (not produced by generate()): generic append + library attention
                 keys, values = layer.update(key_states, value_states)

@@ -15,10 +15,19 @@ import torch
 from transformers.cache_utils import DynamicLayer
 
 
+def _devlen_args(layer, static) -> dict:
+    """The arguments of a device-length decode launch: sized for the capacity; in the static loop (generate.StaticDecoder)
+    the rows also count the device step counter and the launch uses the loop's workspace."""
+    return dict(step=static.step if static is not None else None, max_length=layer.capacity,
+                workspace=static.workspace if static is not None else None)
+
+
 class PkvCacheLayer(DynamicLayer):
     """One layer's compacted cache. keys/values are views of the valid rows of the underlying buffers."""
 
     is_sliding = False
+    group = 1                        # query heads per cache head (> 1: a GQA-shared cache, `PkvBatchCacheLayer`)
+    _BUFFERS = ("k_buf", "v_buf")    # the [B, H, capacity, ...] tensors a resize or a join copies
 
     def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, length: int, seen_tokens: int):
         super().__init__()
@@ -35,23 +44,70 @@ class PkvCacheLayer(DynamicLayer):
     def capacity(self) -> int:
         return self.k_buf.shape[2]
 
+    @property
+    def num_q_heads(self) -> int:
+        return self.k_buf.shape[1] * self.group
+
+    # -- row counts, the same view over every form --
+    @property
+    def rows_host(self) -> list:
+        """[B][H]: the rows sequence b keeps for cache head h."""
+        return [[self.length] * self.k_buf.shape[1] for _ in range(self.k_buf.shape[0])]
+
+    @property
+    def rows_dev(self) -> Optional[torch.Tensor]:
+        """The same counts on the device (int32, B*H) for a kernel to read; None when every count is `length`."""
+        return None
+
+    @property
+    def seq_seen(self) -> list:
+        """[B]: the tokens sequence b has seen."""
+        return [self.seen_tokens] * self.k_buf.shape[0]
+
     def _refresh_views(self) -> None:
         self.keys = self.k_buf[:, :, : self.length]
         self.values = self.v_buf[:, :, : self.length]
 
-    def reserve(self, extra_rows: int) -> None:
-        """Make room for `extra_rows` more rows (amortised doubling; the copy happens off the per-token path)."""
-        need = self.length + extra_rows
-        if need <= self.capacity:
-            return
-        new_cap = max(need, self.capacity + max(64, self.capacity // 2))
-        b, h, _, d = self.k_buf.shape
-        nk = torch.empty(b, h, new_cap, d, dtype=self.dtype, device=self.device)
-        nv = torch.empty_like(nk)
-        nk[:, :, : self.length] = self.k_buf[:, :, : self.length]
-        nv[:, :, : self.length] = self.v_buf[:, :, : self.length]
-        self.k_buf, self.v_buf = nk, nv
+    def _resize(self, capacity: int) -> None:
+        """New buffers of `capacity` rows per (sequence, head) holding every row of the old ones (rows the decode kernel
+        appended past the host counts included)."""
+        old = self.capacity
+        for name in self._BUFFERS:
+            t = getattr(self, name)
+            nt = torch.empty((t.shape[0], t.shape[1], capacity) + tuple(t.shape[3:]), dtype=t.dtype, device=t.device)
+            nt[:, :, :old] = t
+            setattr(self, name, nt)
         self._refresh_views()
+
+    def fit(self, rows: int) -> bool:
+        """Make room for `rows` rows per (sequence, head) by amortised doubling (the copy happens off the per-token path).
+        True when the buffers were reallocated."""
+        if rows <= self.capacity:
+            return False
+        self._resize(max(rows, self.capacity + max(64, self.capacity // 2)))
+        return True
+
+    def reserve(self, extra_rows: int) -> None:
+        """Make room for `extra_rows` more rows."""
+        self.fit(self.length + extra_rows)
+
+    def _scales(self):
+        """(k_scale, v_scale) of an FP8 cache; None for 16-bit ones."""
+        return None
+
+    def decode(self, backend, q: torch.Tensor, k_new: torch.Tensor, v_new: torch.Tensor, static=None,
+               softmax_scale: float = 0.0) -> torch.Tensor:
+        """One decode step of every sequence: q [B, Hq, D], k_new / v_new [B, Hkv, D] (appended in place as each sequence's
+        next row). Returns the attention output [B, Hq, D]. `static`: the step counter and workspace of a graph-replayable
+        loop (generate.StaticDecoder), whose rows the buffers already hold; None for a host-launched step."""
+        if q.shape[0] > 1:       # an equal-length batch prefilled as one forward: one launch
+            return backend.decode_attn_batch(q, self.k_buf, self.v_buf, self.length + 1, k_new, v_new, rows=None,
+                                             **_devlen_args(self, static), softmax_scale=softmax_scale)
+        out = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+        # one sequence: the host-length launch (pkv_decode_attn), or the device-length one inside the static loop
+        backend.decode_attn(q[0], self.k_buf[0], self.v_buf[0], self.length + 1, k_new[0], v_new[0], out[0],
+                            softmax_scale=softmax_scale, **(_devlen_args(self, static) if static is not None else {}))
+        return out
 
     def advance(self, rows: int) -> None:
         """Rows were appended in place by the decode kernel."""
@@ -110,6 +166,8 @@ class PkvRaggedCacheLayer(PkvCacheLayer):
     LONGEST head's row count (what the buffers must hold); `appended` the tokens decoded so far."""
 
     def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, head_rows_host, seen_tokens: int):
+        if k_buf.shape[0] != 1:
+            raise NotImplementedError("ragged caches are batch size 1; join them (cache.join_caches) to decode them together")
         self.head_rows_host = [int(r) for r in head_rows_host]
         self.base_rows = max(self.head_rows_host)
         self.head_rows = torch.tensor(self.head_rows_host, dtype=torch.int32, device=k_buf.device)
@@ -118,6 +176,21 @@ class PkvRaggedCacheLayer(PkvCacheLayer):
     @property
     def appended(self) -> int:
         return self.length - self.base_rows
+
+    @property
+    def rows_host(self) -> list:
+        return [[r + self.appended for r in self.head_rows_host]]
+
+    @property
+    def rows_dev(self) -> torch.Tensor:
+        return self.head_rows + self.appended if self.appended else self.head_rows
+
+    def decode(self, backend, q, k_new, v_new, static=None, softmax_scale: float = 0.0) -> torch.Tensor:
+        # pkv_decode_attn_ragged: row head_rows[h] + appended + 1 (+ the step counter in the static loop)
+        out = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+        backend.decode_attn(q[0], self.k_buf[0], self.v_buf[0], self.appended + 1, k_new[0], v_new[0], out[0],
+                            softmax_scale=softmax_scale, head_rows=self.head_rows, **_devlen_args(self, static))
+        return out
 
     def head_view(self, h: int):
         """Valid rows of head h: ([rows_h, D] keys, values) of batch 0."""
@@ -147,6 +220,8 @@ class PkvBatchCacheLayer(PkvCacheLayer):
     the G query heads of its group (`pkv_decode_attn_batch_gqa`); `rows_host[b][j]` counts KV head j's rows. G = 1 (the
     default) is the per-query-head cache."""
 
+    rows_host = seq_seen = None    # held per sequence here (set in __init__), not derived from `length` as in the base class
+
     def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, rows_host, seq_seen, group: int = 1):
         self.group = int(group)
         self.rows_host = [[int(r) for r in row] for row in rows_host]
@@ -156,8 +231,8 @@ class PkvBatchCacheLayer(PkvCacheLayer):
         super().__init__(k_buf, v_buf, max(max(r) for r in self.rows_host), max(self.seq_seen))
 
     @property
-    def num_q_heads(self) -> int:
-        return self.k_buf.shape[1] * self.group
+    def rows_dev(self) -> Optional[torch.Tensor]:
+        return None if all(r == self.length for row in self.rows_host for r in row) else self.rows
 
     def _device_rows(self, device) -> torch.Tensor:
         return torch.tensor([r for row in self.rows_host for r in row], dtype=torch.int32, device=device)
@@ -181,9 +256,13 @@ class PkvBatchCacheLayer(PkvCacheLayer):
         r = self.rows_host[b][h]
         return self.k_buf[b, h, :r], self.v_buf[b, h, :r]
 
-    # -- continuous batching (generate.ContinuousDecoder): one slot rewritten in place while a decode graph holds the buffers --
-    _BUFFERS = ("k_buf", "v_buf")
+    def decode(self, backend, q, k_new, v_new, static=None, softmax_scale: float = 0.0) -> torch.Tensor:
+        # rows = layer.rows[b, h] + 1 (+ the step counter in the static loop); G > 1: each KV head read once for its group
+        fn = backend.decode_attn_batch_gqa if self.group > 1 else backend.decode_attn_batch
+        return fn(q, self.k_buf, self.v_buf, 1, k_new, v_new, rows=self.rows, **_devlen_args(self, static),
+                  softmax_scale=softmax_scale)
 
+    # -- continuous batching (generate.ContinuousDecoder): one slot rewritten in place while a decode graph holds the buffers --
     def admit(self, slot: int, src_layer, step: torch.Tensor, backend=None) -> None:
         """Copy the single-prompt layer `src_layer` (the form this batch holds: `PkvCacheLayer` / `PkvRaggedCacheLayer`, or,
         for a GQA-shared or FP8 batch, a batch-1 layer of the same group and dtype) into slot `slot`, and set the slot's
@@ -198,32 +277,18 @@ class PkvBatchCacheLayer(PkvCacheLayer):
     def grow(self, capacity: int) -> None:
         """New buffers of `capacity` rows per (sequence, head) holding every row of the old ones (the rows the decode kernel
         appended included). `rows` stays the same tensor; a decode graph over the old buffers must be captured again."""
-        old = self.capacity
-        if capacity <= old:
-            return
-        for name in self._BUFFERS:
-            t = getattr(self, name)
-            nt = torch.empty((t.shape[0], t.shape[1], capacity) + tuple(t.shape[3:]), dtype=t.dtype, device=t.device)
-            nt[:, :, :old] = t
-            setattr(self, name, nt)
-        self._refresh_views()
+        if capacity > self.capacity:
+            self._resize(capacity)
 
     def _install_item(self, slot: int, src):
         """(the `cache_install` tuple of this layer, the slot's host row counts, its tokens seen)."""
         B, H, _, D = self.k_buf.shape
         if not 0 <= int(slot) < B:
             raise ValueError(f"slot {slot} outside [0, {B})")
-        fp8 = isinstance(self, PkvFp8CacheLayer)
-        dst = (self.k_buf, self.v_buf, (self.k_scale, self.v_scale) if fp8 else None, self.rows)
+        dst = (self.k_buf, self.v_buf, self._scales(), self.rows)
         if src is None:
             return (None, None, None, 0, None, *dst), [0] * H, 0
-        if fp8:
-            ok = isinstance(src, PkvFp8CacheLayer) and src.group == self.group
-        elif self.group > 1:
-            ok = isinstance(src, PkvBatchCacheLayer) and not isinstance(src, PkvFp8CacheLayer) and src.group == self.group
-        else:
-            ok = isinstance(src, PkvCacheLayer) and not isinstance(src, PkvBatchCacheLayer)
-        if not ok:
+        if not isinstance(src, PkvCacheLayer) or _form(src) != _form(self):
             raise ValueError(f"admit: a {type(src).__name__} (group {getattr(src, 'group', 1)}) cannot enter a "
                              f"{type(self).__name__} of group {self.group}: FP8 and 16-bit caches, and caches of different "
                              "groups, do not mix")
@@ -231,21 +296,11 @@ class PkvBatchCacheLayer(PkvCacheLayer):
                 or src.device != self.device:
             raise ValueError(f"admit: the source must be one prompt of {H} heads, head_dim {D}, {self.dtype} on {self.device}; "
                              f"got {tuple(src.k_buf.shape)} {src.dtype} on {src.device}")
-        if isinstance(src, PkvRaggedCacheLayer):
-            rows_host = [r + src.appended for r in src.head_rows_host]
-            rows_dev = src.head_rows + src.appended if src.appended else src.head_rows
-            seen = src.seen_tokens
-        elif isinstance(src, PkvBatchCacheLayer):
-            rows_host = list(src.rows_host[0])
-            rows_dev = None if len(set(rows_host)) == 1 else src.rows
-            seen = src.seq_seen[0]
-        else:
-            rows_host, rows_dev, seen = [src.length] * H, None, src.seen_tokens
+        rows_host = src.rows_host[0]
         n = max(rows_host)
         if n > self.capacity:
             raise ValueError(f"admit: {n} rows exceed the capacity {self.capacity} (grow the batch first)")
-        scales = (src.k_scale, src.v_scale) if fp8 else None
-        return (src.k_buf, src.v_buf, scales, n, rows_dev, *dst), rows_host, seen
+        return (src.k_buf, src.v_buf, src._scales(), n, src.rows_dev, *dst), rows_host, src.seq_seen[0]
 
     def _book(self, slot: int, rows_host, seen: int) -> None:
         self.rows_host[slot] = list(rows_host)
@@ -302,20 +357,14 @@ class PkvFp8CacheLayer(PkvBatchCacheLayer):
         self.k_scale, self.v_scale = k_scale, v_scale
         super().__init__(k_q, v_q, rows_host, seq_seen, group)
 
-    def reserve(self, extra_rows: int) -> None:
-        need = self.length + extra_rows
-        if need <= self.capacity:
-            return
-        new_cap = max(need, self.capacity + max(64, self.capacity // 2))
-        b, h, _, d = self.k_buf.shape
-        n = self.length
-        bufs = []
-        for t in (self.k_buf, self.v_buf, self.k_scale, self.v_scale):
-            nt = torch.empty((b, h, new_cap) + tuple(t.shape[3:]), dtype=t.dtype, device=t.device)
-            nt[:, :, :n] = t[:, :, :n]
-            bufs.append(nt)
-        self.k_buf, self.v_buf, self.k_scale, self.v_scale = bufs
-        self._refresh_views()
+    def _scales(self):
+        return self.k_scale, self.v_scale
+
+    def decode(self, backend, q, k_new, v_new, static=None, softmax_scale: float = 0.0) -> torch.Tensor:
+        # the kernel quantises the new K / V row and attends it as stored
+        fn = backend.decode_attn_batch_gqa_fp8 if self.group > 1 else backend.decode_attn_batch_fp8
+        return fn(q, self.k_buf, self.v_buf, self.k_scale, self.v_scale, 1, k_new, v_new, rows=self.rows,
+                  **_devlen_args(self, static), softmax_scale=softmax_scale)
 
     @staticmethod
     def dequantize(q: torch.Tensor, scale: torch.Tensor) -> torch.Tensor:
@@ -331,9 +380,6 @@ class PkvFp8CacheLayer(PkvBatchCacheLayer):
     def update(self, key_states, value_states, *args, **kwargs):
         raise NotImplementedError("multi-token append to an FP8 cache is not built: decode it one token per step (the FP8 "
                                   "cache covers the decode path; prefill and the multi-token path stay 16-bit)")
-
-    def crop(self, max_length: int) -> None:
-        raise NotImplementedError("cropping a compacted cache is undefined (rows are in score order, not position order)")
 
     def batch_repeat_interleave(self, repeats: int) -> None:
         raise NotImplementedError("an FP8 cache holds one row count per sequence and head (beam search over FP8 caches is "
@@ -351,31 +397,15 @@ def quantize_caches_fp8(past_key_values, backend) -> int:
     converted."""
     idx, items, metas = [], [], []
     for i, l in enumerate(past_key_values.layers):
-        if isinstance(l, PkvBatchCacheLayer) and l.group > 1 and not isinstance(l, PkvFp8CacheLayer):
-            B, H, cap, D = l.k_buf.shape
-            kq = torch.empty(B, H, cap, D, dtype=torch.float8_e4m3fn, device=l.device)
-            vq = torch.empty_like(kq)
-            ks = torch.empty(B, H, cap, dtype=torch.float32, device=l.device)
-            vs = torch.empty_like(ks)
-            uniform = all(r == l.length for row in l.rows_host for r in row)
-            items.append((l.k_buf, l.v_buf, kq, vq, ks, vs, l.length, None if uniform else l.rows))
-            metas.append((kq, vq, ks, vs, l.rows_host, l.seq_seen, l.group))
-            idx.append(i)
+        if not isinstance(l, PkvCacheLayer) or isinstance(l, PkvFp8CacheLayer):
             continue
-        if not isinstance(l, PkvCacheLayer) or isinstance(l, PkvBatchCacheLayer):
-            continue
-        B, Hq, cap, D = l.k_buf.shape
-        kq = torch.empty(B, Hq, cap, D, dtype=torch.float8_e4m3fn, device=l.device)
+        B, H, cap, D = l.k_buf.shape
+        kq = torch.empty(B, H, cap, D, dtype=torch.float8_e4m3fn, device=l.device)
         vq = torch.empty_like(kq)
-        ks = torch.empty(B, Hq, cap, dtype=torch.float32, device=l.device)
+        ks = torch.empty(B, H, cap, dtype=torch.float32, device=l.device)
         vs = torch.empty_like(ks)
-        if isinstance(l, PkvRaggedCacheLayer):
-            rows_host = [[r + l.appended for r in l.head_rows_host]] * B
-            rows_dev = l.head_rows + l.appended if l.appended else l.head_rows
-        else:
-            rows_host, rows_dev = [[l.length] * Hq] * B, None
-        items.append((l.k_buf, l.v_buf, kq, vq, ks, vs, l.length, rows_dev))
-        metas.append((kq, vq, ks, vs, rows_host, [l.seen_tokens] * B))
+        items.append((l.k_buf, l.v_buf, kq, vq, ks, vs, l.length, l.rows_dev))
+        metas.append((kq, vq, ks, vs, l.rows_host, l.seq_seen, l.group))
         idx.append(i)
     if items:
         backend.cache_quantize_fp8(items)
@@ -384,28 +414,9 @@ def quantize_caches_fp8(past_key_values, backend) -> int:
     return len(idx)
 
 
-def _join_fp8(caches, reserve: int):
-    from transformers import DynamicCache
-    out = DynamicCache()
-    out.layers = []
-    for i in range(len(caches[0].layers)):
-        src = [c.layers[i] for c in caches]
-        _, hq, _, d = src[0].k_buf.shape
-        if any(l.k_buf.shape[1] != hq or l.k_buf.shape[3] != d or l.device != src[0].device for l in src):
-            raise ValueError(f"join_caches: layer {i}: head counts, head_dim or device differ between the caches")
-        rows = [list(l.rows_host[0]) for l in src]
-        cap = max(max(r) for r in rows) + int(reserve)
-        group = src[0].group
-        k = torch.empty(len(src), hq, cap, d, dtype=torch.float8_e4m3fn, device=src[0].device)
-        v = torch.empty_like(k)
-        ks = torch.empty(len(src), hq, cap, dtype=torch.float32, device=src[0].device)
-        vs = torch.empty_like(ks)
-        for b, l in enumerate(src):
-            n = l.length
-            k[b, :, :n], v[b, :, :n] = l.k_buf[0, :, :n], l.v_buf[0, :, :n]
-            ks[b, :, :n], vs[b, :, :n] = l.k_scale[0, :, :n], l.v_scale[0, :, :n]
-        out.layers.append(PkvFp8CacheLayer(k, v, ks, vs, rows, [l.seq_seen[0] for l in src], group))
-    return out
+def _form(layer) -> tuple:
+    """What decides whether two compacted layers may share a batch: FP8 or 16-bit, and the group (GQA-shared caches)."""
+    return isinstance(layer, PkvFp8CacheLayer), layer.group
 
 
 def join_caches(caches, reserve: int = 0):
@@ -419,47 +430,38 @@ def join_caches(caches, reserve: int = 0):
     if not caches:
         raise ValueError("join_caches: no caches")
     n_layers = len(caches[0].layers)
-    if len({getattr(l, "group", 1) for c in caches for l in c.layers}) > 1:
+    layers = [l for c in caches for l in c.layers]
+    if any(len(c.layers) != n_layers for c in caches) or not all(isinstance(l, PkvCacheLayer) for l in layers):
+        raise RuntimeError("join_caches needs caches prefilled by the patched forward on every layer "
+                           "(method 'fullkv' and stock caches are not compacted)")
+    forms = {_form(l) for l in layers}
+    if len({group for _, group in forms}) > 1:
         raise ValueError("join_caches: GQA-shared and per-query-head caches (or caches of different groups) cannot be joined "
                          "together (set pkv_gqa_shared the same for every prompt)")
-    fp8 = [isinstance(l, PkvFp8CacheLayer) for c in caches for l in c.layers]
-    if any(fp8):
-        if not all(fp8) or any(len(c.layers) != n_layers for c in caches):
-            raise ValueError("join_caches: FP8 and 16-bit caches cannot be joined together (set pkv_kv_cache_dtype the same "
-                             "for every prompt)")
-        if any(l.k_buf.shape[0] != 1 for c in caches for l in c.layers):
-            raise ValueError("join_caches joins single-prompt (batch 1) caches")
-        return _join_fp8(caches, reserve)
-    group = getattr(caches[0].layers[0], "group", 1) if n_layers else 1
-    single = (lambda l: isinstance(l, PkvBatchCacheLayer)) if group > 1 else (lambda l: not isinstance(l, PkvBatchCacheLayer))
-    for c in caches:
-        if len(c.layers) != n_layers or not all(isinstance(l, PkvCacheLayer) and single(l) for l in c.layers):
-            raise RuntimeError("join_caches needs caches prefilled by the patched forward on every layer "
-                               "(method 'fullkv' and stock caches are not compacted)")
-        if any(l.k_buf.shape[0] != 1 for l in c.layers):
-            raise ValueError("join_caches joins single-prompt (batch 1) caches")
+    if len(forms) > 1:
+        raise ValueError("join_caches: FP8 and 16-bit caches cannot be joined together (set pkv_kv_cache_dtype the same "
+                         "for every prompt)")
+    if any(l.k_buf.shape[0] != 1 for l in layers):
+        raise ValueError("join_caches joins single-prompt (batch 1) caches")
     out = DynamicCache()
     out.layers = []
     for i in range(n_layers):
         src = [c.layers[i] for c in caches]
-        rows = []
-        for l in src:
-            if isinstance(l, PkvRaggedCacheLayer):
-                rows.append([r + l.appended for r in l.head_rows_host])
-            elif group > 1:
-                rows.append(list(l.rows_host[0]))
-            else:
-                rows.append([l.length] * l.k_buf.shape[1])
-        _, hq, _, d = src[0].k_buf.shape
-        if any(l.k_buf.shape[1] != hq or l.k_buf.shape[3] != d or l.dtype != src[0].dtype or l.device != src[0].device for l in src):
+        l0 = src[0]
+        _, h, _, d = l0.k_buf.shape
+        if any(l.k_buf.shape[1] != h or l.k_buf.shape[3] != d or l.dtype != l0.dtype or l.device != l0.device for l in src):
             raise ValueError(f"join_caches: layer {i}: head counts, head_dim, dtype or device differ between the caches")
+        rows = [l.rows_host[0] for l in src]
         cap = max(max(r) for r in rows) + int(reserve)
-        k = torch.empty(len(src), hq, cap, d, dtype=src[0].dtype, device=src[0].device)
-        v = torch.empty_like(k)
-        for b, l in enumerate(src):
-            k[b, :, : l.length] = l.k_buf[0, :, : l.length]
-            v[b, :, : l.length] = l.v_buf[0, :, : l.length]
-        out.layers.append(PkvBatchCacheLayer(k, v, rows, [l.seen_tokens for l in src], group))
+        bufs = []
+        for name in l0._BUFFERS:
+            t0 = getattr(l0, name)
+            t = torch.empty((len(src), h, cap) + tuple(t0.shape[3:]), dtype=t0.dtype, device=t0.device)
+            for b, l in enumerate(src):
+                t[b, :, : l.length] = getattr(l, name)[0, :, : l.length]
+            bufs.append(t)
+        cls = type(l0) if isinstance(l0, PkvBatchCacheLayer) else PkvBatchCacheLayer
+        out.layers.append(cls(*bufs, rows, [l.seq_seen[0] for l in src], l0.group))
     return out
 
 

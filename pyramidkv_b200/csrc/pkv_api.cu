@@ -586,15 +586,22 @@ int pkv_decode_attn(const pkv_decode_desc* d, void* stream) {
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "decode launch");
 }
 
+// The argument checks every device-length decode entry point shares.
+static int check_devlen_args(const char* fn, int32_t num_seqs, const int32_t* rows, const int32_t* step_dev, int64_t max_length) {
+    if ((reinterpret_cast<uintptr_t>(rows) & 3u) || (reinterpret_cast<uintptr_t>(step_dev) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned int32 pointer", fn);
+    if (max_length < 1) return fail(PKV_ERR_INVALID_ARG, "%s: max_length must be >= 1", fn);
+    if (num_seqs < 1 || num_seqs > 65535) return fail(PKV_ERR_INVALID_ARG, "%s: num_seqs=%d outside [1, 65535]", fn, num_seqs);
+    return PKV_OK;
+}
+
 // The device-length decode of num_seqs sequences: pkv_decode_attn_batch, and pkv_decode_attn_graph / pkv_decode_attn_ragged
 // as its one-sequence calls.
 static int decode_devlen(const char* fn, const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
                          const int32_t* step_dev, int64_t max_length, void* stream) {
-    if ((reinterpret_cast<uintptr_t>(rows) & 3u) || (reinterpret_cast<uintptr_t>(step_dev) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned int32 pointer", fn);
-    if (max_length < 1) return fail(PKV_ERR_INVALID_ARG, "%s: max_length must be >= 1", fn);
-    if (num_seqs < 1 || num_seqs > 65535) return fail(PKV_ERR_INVALID_ARG, "%s: num_seqs=%d outside [1, 65535]", fn, num_seqs);
+    int rc = check_devlen_args(fn, num_seqs, rows, step_dev, max_length);
+    if (rc) return rc;
     DecodeArgs a;
-    int rc = resolve_decode(d, &a, true, max_length, num_seqs);
+    rc = resolve_decode(d, &a, true, max_length, num_seqs);
     if (rc) return rc;
     if (num_seqs > 1 && (cache_stride_b < int64_t(a.Hq) * a.cache_sh || cache_stride_b % 8))
         return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_b=%lld is below num_q_heads*cache_stride_h=%lld or not a multiple of 8", fn,
@@ -617,13 +624,12 @@ int pkv_decode_attn_batch_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_
                               const int32_t* step_dev, int64_t max_length, float* k_scale, float* v_scale, int64_t scale_stride_h,
                               int64_t scale_stride_b, void* stream) {
     const char* fn = "pkv_decode_attn_batch_fp8";
-    if ((reinterpret_cast<uintptr_t>(rows) & 3u) || (reinterpret_cast<uintptr_t>(step_dev) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned int32 pointer", fn);
-    if (max_length < 1) return fail(PKV_ERR_INVALID_ARG, "%s: max_length must be >= 1", fn);
-    if (num_seqs < 1 || num_seqs > 65535) return fail(PKV_ERR_INVALID_ARG, "%s: num_seqs=%d outside [1, 65535]", fn, num_seqs);
+    int rc = check_devlen_args(fn, num_seqs, rows, step_dev, max_length);
+    if (rc) return rc;
     if (!k_scale || !v_scale) return fail(PKV_ERR_INVALID_ARG, "%s: null scale pointer", fn);
     if ((reinterpret_cast<uintptr_t>(k_scale) & 3u) || (reinterpret_cast<uintptr_t>(v_scale) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned scale pointer", fn);
     DecodeArgs a;
-    int rc = resolve_decode(d, &a, true, max_length, num_seqs);
+    rc = resolve_decode(d, &a, true, max_length, num_seqs);
     if (rc) return rc;
     if (a.cache_sh % 16) return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_h=%lld bytes is not a multiple of 16", fn, (long long)a.cache_sh);
     if (num_seqs > 1 && (cache_stride_b < int64_t(a.Hq) * a.cache_sh || cache_stride_b % 16))
@@ -648,10 +654,9 @@ int pkv_decode_attn_batch_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_
 // GQA-shared caches: the checks of pkv_decode_attn_batch(_fp8) with KV-head strides; `elem` = bytes per cached element.
 static int resolve_decode_gqa(const char* fn, const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
                               const int32_t* step_dev, int64_t max_length, int elem, DecodeArgs* a) {
-    if ((reinterpret_cast<uintptr_t>(rows) & 3u) || (reinterpret_cast<uintptr_t>(step_dev) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned int32 pointer", fn);
-    if (max_length < 1) return fail(PKV_ERR_INVALID_ARG, "%s: max_length must be >= 1", fn);
-    if (num_seqs < 1 || num_seqs > 65535) return fail(PKV_ERR_INVALID_ARG, "%s: num_seqs=%d outside [1, 65535]", fn, num_seqs);
-    int rc = resolve_decode(d, a, true, max_length, num_seqs);
+    int rc = check_devlen_args(fn, num_seqs, rows, step_dev, max_length);
+    if (rc) return rc;
+    rc = resolve_decode(d, a, true, max_length, num_seqs);
     if (rc) return rc;
     if (a->G != 2 && a->G != 4 && a->G != 8)
         return fail(PKV_ERR_UNSUPPORTED, "%s: group size num_q_heads/num_kv_heads = %d: the grouped kernels are built for 2, 4 and 8", fn, a->G);

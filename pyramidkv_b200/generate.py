@@ -34,7 +34,7 @@ from typing import Optional
 
 import torch
 
-from .cache import PkvBatchCacheLayer, PkvCacheLayer, PkvRaggedCacheLayer, admit_cache, join_caches, park_cache
+from .cache import PkvBatchCacheLayer, PkvCacheLayer, admit_cache, join_caches, park_cache
 
 
 @dataclass
@@ -54,32 +54,32 @@ class StaticDecoder:
 
     def __init__(self, model, cache, first_token: torch.Tensor, max_steps: int, use_graph: Optional[bool] = None,
                  eos_token_id=None, pad_token_id: int = 0):
-        self.model, self.cache, self.max_steps = model, cache, int(max_steps)
         layers = [l for l in cache.layers if isinstance(l, PkvCacheLayer)]
         if len(layers) != model.config.num_hidden_layers:
             raise RuntimeError("StaticDecoder needs a cache prefilled by the patched forward on every layer "
                                "(method 'fullkv' and stock caches go through model.generate)")
-        self.layers = layers
+        for l in layers:
+            l.reserve(int(max_steps))                      # off the per-token path: no reallocation while the graph lives
+        self._setup(model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id)
+        self.done = None if self.eos is None else (self.ids == self.eos[None, :]).any(dim=1, keepdim=True)   # [B, 1]
+
+    def _setup(self, model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id) -> None:
+        """The state both decoders hold: the step counter and workspace the decode launches read, the per-sequence input
+        ids and positions, the token buffer [B, max_steps] and its cursor, and the EOS ids."""
+        self.model, self.cache, self.layers, self.max_steps = model, cache, layers, int(max_steps)
         dev = layers[0].device
         bsz = layers[0].k_buf.shape[0]
-        if isinstance(layers[0], PkvRaggedCacheLayer) and bsz != 1:
-            raise NotImplementedError("ragged caches are batch size 1; join them (cache.join_caches) to decode them together")
-        for l in layers:
-            l.reserve(self.max_steps)                      # off the per-token path: no reallocation while the graph lives
-        backend = model.model.layers[0].self_attn.kv_cluster.backend
-        hq, d = layers[0].k_buf.shape[1] * getattr(layers[0], "group", 1), layers[0].k_buf.shape[3]   # query heads
+        self.backend = model.model.layers[0].self_attn.kv_cluster.backend
         self.state = _StaticState(step=torch.zeros(1, dtype=torch.int32, device=dev),
-                                  workspace=backend.decode_workspace(bsz * hq, d, dev))
+                                  workspace=self.backend.decode_workspace(bsz * layers[0].num_q_heads, layers[0].k_buf.shape[3], dev))
         self.ids = first_token.reshape(bsz, 1).to(device=dev, dtype=torch.long).clone()
-        seen = layers[0].seq_seen if isinstance(layers[0], PkvBatchCacheLayer) else [layers[0].seen_tokens] * bsz
-        self.pos = torch.tensor(seen, dtype=torch.long, device=dev).reshape(bsz, 1)
+        self.pos = torch.tensor(layers[0].seq_seen, dtype=torch.long, device=dev).reshape(bsz, 1)
         self.cursor = torch.zeros(1, dtype=torch.long, device=dev)
         self.tokens = torch.zeros(bsz, self.max_steps, dtype=torch.long, device=dev)
-        self.eos = self.done = None
+        self.eos = None
         if eos_token_id is not None:
             eos = eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id]
             self.eos = torch.tensor([int(e) for e in eos], dtype=torch.long, device=dev)
-            self.done = (self.ids == self.eos[None, :]).any(dim=1, keepdim=True)      # [B, 1]
         self.pad_token_id = int(pad_token_id)
         self.taken = 0
         self.graph = None
@@ -154,7 +154,7 @@ class StaticDecoder:
         if getattr(self.cache, "_pkv_static", None) is self.state:
             del self.cache._pkv_static
         for l in self.layers:
-            if kept is not None and isinstance(l, PkvBatchCacheLayer):
+            if kept is not None:
                 l.settle(kept)
             else:
                 l.advance(self.taken)
@@ -270,38 +270,18 @@ class ContinuousDecoder(StaticDecoder):
 
     def __init__(self, model, cache, first_token: torch.Tensor, left, chunk: int, use_graph: Optional[bool] = None,
                  eos_token_id=None, pad_token_id: int = 0):
-        self.model, self.cache, self.max_steps = model, cache, max(1, int(chunk))
         layers = [l for l in cache.layers if isinstance(l, PkvBatchCacheLayer)]
         if len(layers) != model.config.num_hidden_layers or len(layers) != len(cache.layers):
             raise RuntimeError("ContinuousDecoder needs a batched cache (cache.join_caches) on every layer")
-        self.layers = layers
-        dev = layers[0].device
-        bsz = layers[0].k_buf.shape[0]
-        self.backend = model.model.layers[0].self_attn.kv_cluster.backend
-        hq, d = layers[0].num_q_heads, layers[0].k_buf.shape[3]
-        self.state = _StaticState(step=torch.zeros(1, dtype=torch.int32, device=dev),
-                                  workspace=self.backend.decode_workspace(bsz * hq, d, dev))
+        self._setup(model, cache, layers, first_token, max(1, int(chunk)), use_graph, eos_token_id, pad_token_id)
         # every layer's row counts are rows of one tensor, so one op per step stops them growing for the done slots
         self.rows_all = torch.stack([l.rows for l in layers])
         for i, l in enumerate(layers):
             l.rows = self.rows_all[i]
-        self.ids = first_token.reshape(bsz, 1).to(device=dev, dtype=torch.long).clone()
-        self.pos = torch.tensor(layers[0].seq_seen, dtype=torch.long, device=dev).reshape(bsz, 1)
-        self.cursor = torch.zeros(1, dtype=torch.long, device=dev)
-        self.tokens = torch.zeros(bsz, self.max_steps, dtype=torch.long, device=dev)
-        self.left = torch.tensor([int(n) for n in left], dtype=torch.long, device=dev).reshape(bsz, 1)
-        self.eos = None
-        if eos_token_id is not None:
-            eos = eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id]
-            self.eos = torch.tensor([int(e) for e in eos], dtype=torch.long, device=dev)
+        self.left = torch.tensor([int(n) for n in left], dtype=torch.long, device=self.ids.device).reshape(self.ids.shape[0], 1)
         self.done = self.left <= 0
-        self.pad_token_id = int(pad_token_id)
-        self.taken = 0
-        self.graph = None
         self.captures = 0
         self.parked = set()
-        self.use_graph = (dev.type == "cuda") if use_graph is None else bool(use_graph)
-        cache._pkv_static = self.state
 
     def _step(self) -> None:
         nxt = torch.where(self.done, self.pad_token_id, self._greedy_token())
@@ -337,10 +317,7 @@ class ContinuousDecoder(StaticDecoder):
         `reserve`). True when a buffer was reallocated (the graph is then captured again on the next chunk)."""
         grew = False
         for l, s in zip(self.layers, src_cache.layers):
-            need = s.length + int(new_tokens)
-            if need > l.capacity:
-                l.grow(max(need, l.capacity + max(64, l.capacity // 2)))
-                grew = True
+            grew |= l.fit(max(s.rows_host[0]) + int(new_tokens))
         if grew:
             self.graph = None
         return grew
@@ -415,7 +392,7 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
         ms = (time.perf_counter() - t0) * 1e3
         stats["prefill_ms"][i] = ms
         stats["prefill_s"] += ms / 1e3
-        stats["cache_rows_first_last"][i] = [int(cache.layers[0].length), int(cache.layers[-1].length)]
+        stats["cache_rows_first_last"][i] = [max(cache.layers[0].rows_host[0]), max(cache.layers[-1].rows_host[0])]
         return first, cache
 
     B = min(int(num_slots), len(ids))

@@ -426,59 +426,73 @@ def decode_attn_batch(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor,
     [B*Hq] (or [B, Hq]) or None (every sequence holds `length` rows). The launch is sized for `max_length` rows (default:
     the capacity) and is graph-replayable; every sequence's output and appended row are bit-identical to `decode_attn` in
     the graph form (or the ragged form, for per-head rows) on that sequence alone. Returns out [B, Hq, D]."""
-    _require_cuda(q, k_buf, v_buf, k_new, v_new, rows, step, workspace, out)
-    if k_buf.dim() != 4 or k_buf.shape != v_buf.shape or k_buf.stride() != v_buf.stride():
-        raise ValueError("k_buf / v_buf must be [B, Hq, capacity, D] tensors of equal shape and strides")
-    B, Hq, cap, D = k_buf.shape
-    if k_buf.stride(3) != 1 or k_buf.stride(2) != D:
-        raise ValueError("k_buf / v_buf: every head's rows must be contiguous [capacity, D]")
-    if q.shape != (B, Hq, D):
-        raise ValueError(f"q must be [B, Hq, D] = {(B, Hq, D)}, got {tuple(q.shape)}")
-    if not q.is_contiguous():
-        q = q.contiguous()
+    return _decode_batch("pkv_decode_attn_batch", "decode_attn_batch", q, k_buf, v_buf, None, length, k_new, v_new,
+                         rows, step, max_length, workspace, out, softmax_scale)
+
+
+def _decode_batch(entry, what, q, k_buf, v_buf, scales, length, k_new, v_new, rows, step, max_length, workspace, out,
+                  softmax_scale, gqa: bool = False) -> torch.Tensor:
+    """The checks and the descriptor of the four batched decode launches, then the launch of the C entry point `entry`.
+    `scales`: (k_scale, v_scale) of an FP8 cache, or None. `gqa`: a GQA-shared cache (k_buf / v_buf [B, Hkv, capacity, D],
+    q [B, Hq, D])."""
+    _require_cuda(q, k_buf, v_buf, k_new, v_new, rows, step, workspace, out, *(scales or ()))
+    if scales is not None:
+        _check_fp8_buffers(k_buf, v_buf, scales[0], scales[1], what)
+    elif k_buf.dim() != 4 or k_buf.shape != v_buf.shape or k_buf.stride() != v_buf.stride() or k_buf.stride(3) != 1 \
+            or k_buf.stride(2) != k_buf.shape[3]:
+        raise ValueError(f"{what}: k_buf / v_buf must be [B, H, capacity, D] tensors of equal shape and strides, rows contiguous")
+    B, H, cap, D = k_buf.shape
+    heads = "Hkv" if gqa else "Hq"        # the heads of the cache
+    if q.dim() != 3 or q.shape[0] != B or q.shape[2] != D or (q.shape[1] % H if gqa else q.shape[1] != H):
+        raise ValueError(f"{what}: q must be [B, Hq, D] with B = {B}, D = {D} and Hq "
+                         f"{'a multiple of Hkv = ' if gqa else '= '}{H}, got {tuple(q.shape)}")
+    Hq = q.shape[1]
+    q = q.contiguous()
     if out is None:
         out = torch.empty(B, Hq, D, dtype=q.dtype, device=q.device)
     elif out.shape != (B, Hq, D) or not out.is_contiguous() or out.dtype != q.dtype:
-        raise ValueError("out must be a contiguous [B, Hq, D] tensor of q's dtype")
+        raise ValueError(f"{what}: out must be a contiguous [B, Hq, D] tensor of q's dtype")
     max_length = int(max_length) or cap
     if not 1 <= length <= max_length <= cap:
-        raise ValueError(f"cache capacity {cap} exceeded or bad row counts (length {length}, max_length {max_length})")
+        raise ValueError(f"{what}: cache capacity {cap} exceeded or bad row counts (length {length}, max_length {max_length})")
     if step is not None and (step.dtype != torch.int32 or step.numel() != 1):
         raise ValueError("step must be an int32 device tensor with one element")
     if rows is not None:
-        if rows.dtype != torch.int32 or rows.numel() != B * Hq or not rows.is_contiguous():
-            raise ValueError(f"rows must be a contiguous int32 device tensor of B*Hq = {B * Hq} elements")
+        if rows.dtype != torch.int32 or rows.numel() != B * H or not rows.is_contiguous():
+            raise ValueError(f"{what}: rows must be a contiguous int32 device tensor of B*{heads} = {B * H} elements")
         if not torch.cuda.is_current_stream_capturing():
             # (one device read; a captured launch relies on the caller, and the kernel reads and writes no row of a
             # (sequence, head) whose count exceeds max_length)
             most = int(rows.max()) + int(length) + (int(step) if step is not None else 0)
             if most > max_length:
-                raise ValueError(f"cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
+                raise ValueError(f"{what}: cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
     d = DecodeDesc()
     d.struct_bytes = C.sizeof(DecodeDesc)
-    d.dtype, d.num_q_heads, d.head_dim = _dtype_code(q), Hq, D
+    d.dtype, d.num_q_heads, d.num_kv_heads, d.head_dim = _dtype_code(q), B * Hq, H, D
     d.device = q.device.index if q.device.index is not None else torch.cuda.current_device()
     d.length = int(length)
     d.q, d.k_cache, d.v_cache, d.cache_stride_h, d.out = q.data_ptr(), k_buf.data_ptr(), v_buf.data_ptr(), k_buf.stride(1), out.data_ptr()
     keep = [q, out]
     if k_new is not None:
-        if k_new.dim() != 3 or k_new.shape[0] != B or k_new.shape[2] != D or v_new is None or v_new.shape != k_new.shape:
-            raise ValueError("k_new / v_new must be [B, Hkv, D]")
+        if k_new.dim() != 3 or k_new.shape[0] != B or k_new.shape[2] != D or (gqa and k_new.shape[1] != H) or v_new is None \
+                or v_new.shape != k_new.shape or k_new.dtype != q.dtype or v_new.dtype != q.dtype:
+            raise ValueError(f"{what}: k_new / v_new must be [B, Hkv, D] tensors of q's dtype"
+                             + (f", Hkv = {H}" if gqa else ""))
         k_new, v_new = k_new.contiguous(), v_new.contiguous()
         d.num_kv_heads = k_new.shape[1]
         d.k_new, d.v_new = k_new.data_ptr(), v_new.data_ptr()
         keep += [k_new, v_new]
-    else:
-        d.num_kv_heads = Hq
-    d.num_q_heads = B * Hq                 # workspace query: one set of split partials per (sequence, head)
-    nbytes = int(_lib.lib().pkv_decode_workspace_bytes(C.byref(d)))
+    nbytes = int(_lib.lib().pkv_decode_workspace_bytes(C.byref(d)))      # one set of split partials per (sequence, query head)
     d.num_q_heads = Hq
     ws = workspace if workspace is not None else _workspace(q.device, nbytes)
     d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel() * ws.element_size()
     d.softmax_scale = float(softmax_scale)
-    _lib.check(_lib.lib().pkv_decode_attn_batch(C.byref(d), B, k_buf.stride(0), rows.data_ptr() if rows is not None else None,
-                                                step.data_ptr() if step is not None else None, max_length,
-                                                torch.cuda.current_stream(q.device).cuda_stream))
+    args = (C.byref(d), B, k_buf.stride(0), rows.data_ptr() if rows is not None else None,
+            step.data_ptr() if step is not None else None, max_length)
+    if scales is not None:
+        ks, vs = scales
+        args += (ks.data_ptr(), vs.data_ptr(), ks.stride(1), ks.stride(0))
+    _lib.check(getattr(_lib.lib(), entry)(*args, torch.cuda.current_stream(q.device).cuda_stream))
     return out
 
 
@@ -546,118 +560,11 @@ def decode_attn_batch_fp8(q: torch.Tensor, k_q: torch.Tensor, v_q: torch.Tensor,
     k_scale / v_scale float32 [B, Hq, capacity]; q [B, Hq, D] and k_new / v_new [B, Hkv, D] in bf16 / fp16. The new row
     is quantised, stored (bytes and scale) and attended as stored. The same row counts, launch sizing and graph
     replayability as `decode_attn_batch`; one sequence is B = 1 (step None for a host launch). Returns out [B, Hq, D]."""
-    _require_cuda(q, k_q, v_q, k_scale, v_scale, k_new, v_new, rows, step, workspace, out)
-    _check_fp8_buffers(k_q, v_q, k_scale, v_scale, "decode_attn_batch_fp8")
-    B, Hq, cap, D = k_q.shape
-    if q.shape != (B, Hq, D):
-        raise ValueError(f"q must be [B, Hq, D] = {(B, Hq, D)}, got {tuple(q.shape)}")
-    if not q.is_contiguous():
-        q = q.contiguous()
-    if out is None:
-        out = torch.empty(B, Hq, D, dtype=q.dtype, device=q.device)
-    elif out.shape != (B, Hq, D) or not out.is_contiguous() or out.dtype != q.dtype:
-        raise ValueError("out must be a contiguous [B, Hq, D] tensor of q's dtype")
-    max_length = int(max_length) or cap
-    if not 1 <= length <= max_length <= cap:
-        raise ValueError(f"cache capacity {cap} exceeded or bad row counts (length {length}, max_length {max_length})")
-    if step is not None and (step.dtype != torch.int32 or step.numel() != 1):
-        raise ValueError("step must be an int32 device tensor with one element")
-    if rows is not None:
-        if rows.dtype != torch.int32 or rows.numel() != B * Hq or not rows.is_contiguous():
-            raise ValueError(f"rows must be a contiguous int32 device tensor of B*Hq = {B * Hq} elements")
-        if not torch.cuda.is_current_stream_capturing():
-            most = int(rows.max()) + int(length) + (int(step) if step is not None else 0)
-            if most > max_length:
-                raise ValueError(f"cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
-    d = DecodeDesc()
-    d.struct_bytes = C.sizeof(DecodeDesc)
-    d.dtype, d.num_q_heads, d.head_dim = _dtype_code(q), Hq, D
-    d.device = q.device.index if q.device.index is not None else torch.cuda.current_device()
-    d.length = int(length)
-    d.q, d.k_cache, d.v_cache, d.cache_stride_h, d.out = q.data_ptr(), k_q.data_ptr(), v_q.data_ptr(), k_q.stride(1), out.data_ptr()
-    keep = [q, out]
-    if k_new is not None:
-        if k_new.dim() != 3 or k_new.shape[0] != B or k_new.shape[2] != D or v_new is None or v_new.shape != k_new.shape \
-                or k_new.dtype != q.dtype or v_new.dtype != q.dtype:
-            raise ValueError("k_new / v_new must be [B, Hkv, D] tensors of q's dtype")
-        k_new, v_new = k_new.contiguous(), v_new.contiguous()
-        d.num_kv_heads = k_new.shape[1]
-        d.k_new, d.v_new = k_new.data_ptr(), v_new.data_ptr()
-        keep += [k_new, v_new]
-    else:
-        d.num_kv_heads = Hq
-    d.num_q_heads = B * Hq                 # workspace query: one set of split partials per (sequence, head)
-    nbytes = int(_lib.lib().pkv_decode_workspace_bytes(C.byref(d)))
-    d.num_q_heads = Hq
-    ws = workspace if workspace is not None else _workspace(q.device, nbytes)
-    d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel() * ws.element_size()
-    d.softmax_scale = float(softmax_scale)
-    _lib.check(_lib.lib().pkv_decode_attn_batch_fp8(C.byref(d), B, k_q.stride(0), rows.data_ptr() if rows is not None else None,
-                                                    step.data_ptr() if step is not None else None, max_length,
-                                                    k_scale.data_ptr(), v_scale.data_ptr(), k_scale.stride(1), k_scale.stride(0),
-                                                    torch.cuda.current_stream(q.device).cuda_stream))
-    return out
+    return _decode_batch("pkv_decode_attn_batch_fp8", "decode_attn_batch_fp8", q, k_q, v_q, (k_scale, v_scale), length,
+                         k_new, v_new, rows, step, max_length, workspace, out, softmax_scale)
 
 
 # ---- GQA-shared caches (PKV_FLAG_GQA_SHARED): one cache per KV head, decoded once per group ----
-def _decode_gqa(what, q, k_buf, v_buf, length, k_new, v_new, rows, step, max_length, workspace, out, softmax_scale, scales=None):
-    _require_cuda(q, k_buf, v_buf, k_new, v_new, rows, step, workspace, out, *(scales or ()))
-    if scales is not None:
-        _check_fp8_buffers(k_buf, v_buf, scales[0], scales[1], what)
-    elif k_buf.dim() != 4 or k_buf.shape != v_buf.shape or k_buf.stride() != v_buf.stride() or k_buf.stride(3) != 1 \
-            or k_buf.stride(2) != k_buf.shape[3]:
-        raise ValueError(f"{what}: k_buf / v_buf must be [B, Hkv, capacity, D] tensors of equal shape and strides, rows contiguous")
-    B, Hkv, cap, D = k_buf.shape
-    if q.dim() != 3 or q.shape[0] != B or q.shape[2] != D or q.shape[1] % Hkv:
-        raise ValueError(f"{what}: q must be [B, Hq, D] with Hq a multiple of Hkv = {Hkv}, got {tuple(q.shape)}")
-    Hq = q.shape[1]
-    q = q.contiguous()
-    if out is None:
-        out = torch.empty(B, Hq, D, dtype=q.dtype, device=q.device)
-    elif out.shape != (B, Hq, D) or not out.is_contiguous() or out.dtype != q.dtype:
-        raise ValueError(f"{what}: out must be a contiguous [B, Hq, D] tensor of q's dtype")
-    max_length = int(max_length) or cap
-    if not 1 <= length <= max_length <= cap:
-        raise ValueError(f"{what}: cache capacity {cap} exceeded or bad row counts (length {length}, max_length {max_length})")
-    if step is not None and (step.dtype != torch.int32 or step.numel() != 1):
-        raise ValueError("step must be an int32 device tensor with one element")
-    if rows is not None:
-        if rows.dtype != torch.int32 or rows.numel() != B * Hkv or not rows.is_contiguous():
-            raise ValueError(f"{what}: rows must be a contiguous int32 device tensor of B*Hkv = {B * Hkv} elements")
-        if not torch.cuda.is_current_stream_capturing():
-            most = int(rows.max()) + int(length) + (int(step) if step is not None else 0)
-            if most > max_length:
-                raise ValueError(f"{what}: cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
-    d = DecodeDesc()
-    d.struct_bytes = C.sizeof(DecodeDesc)
-    d.dtype, d.num_q_heads, d.num_kv_heads, d.head_dim = _dtype_code(q), B * Hq, Hkv, D
-    d.device = q.device.index if q.device.index is not None else torch.cuda.current_device()
-    nbytes = int(_lib.lib().pkv_decode_workspace_bytes(C.byref(d)))      # one set of split partials per (sequence, query head)
-    d.num_q_heads = Hq
-    d.length = int(length)
-    d.q, d.k_cache, d.v_cache, d.cache_stride_h, d.out = q.data_ptr(), k_buf.data_ptr(), v_buf.data_ptr(), k_buf.stride(1), out.data_ptr()
-    keep = [q, out]
-    if k_new is not None:
-        if k_new.dim() != 3 or k_new.shape != (B, Hkv, D) or v_new is None or v_new.shape != k_new.shape \
-                or k_new.dtype != q.dtype or v_new.dtype != q.dtype:
-            raise ValueError(f"{what}: k_new / v_new must be [B, Hkv, D] = {(B, Hkv, D)} tensors of q's dtype")
-        k_new, v_new = k_new.contiguous(), v_new.contiguous()
-        d.k_new, d.v_new = k_new.data_ptr(), v_new.data_ptr()
-        keep += [k_new, v_new]
-    ws = workspace if workspace is not None else _workspace(q.device, nbytes)
-    d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel() * ws.element_size()
-    d.softmax_scale = float(softmax_scale)
-    common = (C.byref(d), B, k_buf.stride(0), rows.data_ptr() if rows is not None else None,
-              step.data_ptr() if step is not None else None, max_length)
-    stream = torch.cuda.current_stream(q.device).cuda_stream
-    if scales is None:
-        _lib.check(_lib.lib().pkv_decode_attn_batch_gqa(*common, stream))
-    else:
-        ks, vs = scales
-        _lib.check(_lib.lib().pkv_decode_attn_batch_gqa_fp8(*common, ks.data_ptr(), vs.data_ptr(), ks.stride(1), ks.stride(0), stream))
-    return out
-
-
 def decode_attn_batch_gqa(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor, length: int,
                           k_new: Optional[torch.Tensor] = None, v_new: Optional[torch.Tensor] = None,
                           rows: Optional[torch.Tensor] = None, step: Optional[torch.Tensor] = None, max_length: int = 0,
@@ -667,8 +574,8 @@ def decode_attn_batch_gqa(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Ten
     head, read once for the Hq / Hkv query heads of its group; q / out [B, Hq, D]; k_new / v_new [B, Hkv, D]; `rows` int32
     [B*Hkv]. Query head h's output and the appended row are bit-identical to `decode_attn_batch` over the cache
     repeat-interleaved along the heads. Workspace: `decode_workspace_bytes(B*Hq, D)`."""
-    return _decode_gqa("decode_attn_batch_gqa", q, k_buf, v_buf, length, k_new, v_new, rows, step, max_length, workspace, out,
-                       softmax_scale)
+    return _decode_batch("pkv_decode_attn_batch_gqa", "decode_attn_batch_gqa", q, k_buf, v_buf, None, length, k_new,
+                         v_new, rows, step, max_length, workspace, out, softmax_scale, gqa=True)
 
 
 def decode_attn_batch_gqa_fp8(q: torch.Tensor, k_q: torch.Tensor, v_q: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor,
@@ -678,8 +585,8 @@ def decode_attn_batch_gqa_fp8(q: torch.Tensor, k_q: torch.Tensor, v_q: torch.Ten
                               softmax_scale: float = 0.0) -> torch.Tensor:
     """`decode_attn_batch_fp8` over GQA-shared FP8 caches (`pkv_decode_attn_batch_gqa_fp8`): k_q / v_q float8_e4m3fn
     [B, Hkv, capacity, D], k_scale / v_scale float32 [B, Hkv, capacity]; otherwise as `decode_attn_batch_gqa`."""
-    return _decode_gqa("decode_attn_batch_gqa_fp8", q, k_q, v_q, length, k_new, v_new, rows, step, max_length, workspace, out,
-                       softmax_scale, scales=(k_scale, v_scale))
+    return _decode_batch("pkv_decode_attn_batch_gqa_fp8", "decode_attn_batch_gqa_fp8", q, k_q, v_q, (k_scale, v_scale),
+                         length, k_new, v_new, rows, step, max_length, workspace, out, softmax_scale, gqa=True)
 
 
 # ---- continuous batching: admission into one slot of a batched cache (include/pkv.h: pkv_cache_install) ----
