@@ -210,9 +210,8 @@ constexpr int kPoolMaxW = 64;
 // (5, 7) or 0 = any odd size. The specialised path (WT = 8, KS > 0) is the one the reference's defaults hit.
 // MEAN: the window rows are averaged instead of summed (`.mean(dim=-2)`, AdaKV / HeadKV calcul_attn_sore,
 // pyramidkv_utils.py:661 / :795): fp32 sum times the exact power of two 1/W, one rounding.
-// OCC: CTAs per SM the register allocation aims at (1 = no cap beyond 256 threads per CTA)
-template <typename T, int WT, int KS, bool MEAN = false, int LB = 1, int OCC = 1>
-__global__ void __launch_bounds__(256, OCC) softmax_pool_kernel(const PoolParams p, const __grid_constant__ PoolLayers<LB> ly) {
+template <typename T, int WT, int KS, bool MEAN = false, int LB = 1>
+__global__ void __launch_bounds__(256) softmax_pool_kernel(const PoolParams p, const __grid_constant__ PoolLayers<LB> ly) {
     __shared__ StatR stat[kPoolMaxW];
     __shared__ __align__(16) StatP stat_p[kPoolMaxW / 2];    // the same statistics as packed row pairs {-m, -m'}, {-l, -l'}, {r, r'}: fp32 pair operands as loaded
     __shared__ __align__(16) float sbuf[kPoolTok + 2 * kPoolMaxPad];
@@ -461,15 +460,16 @@ cudaError_t launch_softmax_pool_layers(const EvictArgs* as, int n, int batch_gri
             count_launch();
             if (e != cudaSuccess) return e;
         }
-        // 48 registers (5 CTAs per SM) by default; PKV_BATCH_POOL_OCC = 4 / 6 select the 64- / 40-register builds for A/B runs.
-        static const int occ = []() { const char* e = getenv("PKV_BATCH_POOL_OCC"); return e ? atoi(e) : 5; }();
-#define PKV_POOL_LAUNCH_B(T, O)                                                                                     \
+        // The builds without a register cap (about 60 registers, four CTAs per SM): the stage is bound by the dependency latency of
+        // the window sums, and capping at 48 or 40 registers for five or six CTAs per SM costs more of each thread's ILP than the
+        // extra CTAs hide (H100: 0.28 instead of 0.32 ms per 32 x 32K batch, DESIGN.md section 4.1).
+#define PKV_POOL_LAUNCH_B(T)                                                                                        \
     (a.W != 8 ? cudaLaunchKernelEx(&cfg, softmax_pool_kernel<T, 0, 0, false, kMaxLayerBatch>, p, ly)                \
-     : ks == 7 ? cudaLaunchKernelEx(&cfg, softmax_pool_kernel<T, 8, 7, false, kMaxLayerBatch, O>, p, ly)            \
+     : ks == 7 ? cudaLaunchKernelEx(&cfg, softmax_pool_kernel<T, 8, 7, false, kMaxLayerBatch>, p, ly)               \
      : ks == 5 ? cudaLaunchKernelEx(&cfg, softmax_pool_kernel<T, 8, 5, false, kMaxLayerBatch>, p, ly)               \
                : cudaLaunchKernelEx(&cfg, softmax_pool_kernel<T, 8, 0, false, kMaxLayerBatch>, p, ly))
-        if (a.dtype == PKV_BF16) e = occ == 5 ? PKV_POOL_LAUNCH_B(__nv_bfloat16, 5) : occ == 6 ? PKV_POOL_LAUNCH_B(__nv_bfloat16, 6) : PKV_POOL_LAUNCH_B(__nv_bfloat16, 1);
-        else e = PKV_POOL_LAUNCH_B(__half, 1);
+        if (a.dtype == PKV_BF16) e = PKV_POOL_LAUNCH_B(__nv_bfloat16);
+        else e = PKV_POOL_LAUNCH_B(__half);
 #undef PKV_POOL_LAUNCH_B
         count_launch();
         return e != cudaSuccess ? e : cudaGetLastError();
