@@ -397,6 +397,46 @@ int pkv_decode_attn_ragged(const pkv_decode_desc* d, const int32_t* head_rows, c
 int pkv_update_flatten_view(void* dst, const void* src, const void* state, const int32_t* head_lens, const int32_t* cu_lens,
                             int32_t num_heads, int32_t row_bytes, int32_t device, void* stream);
 
+/* ---- sampled decoding: one token per row of logits, in one launch for the batch (DESIGN.md §4.6) ----
+ * Row b (logits[b*logits_stride .. + vocab), dtype bf16 / fp16) is drawn with its own device parameters temperature[b] = T
+ * (fp32), top_k[b], top_p[b] (fp32), seed[b] and token index t = token_index[b]:
+ *  1. T == 0 or top_k == 1: the argmax of the logits, first index among ties (torch.argmax); no random numbers.
+ *  2. x_i = f32(logit_i) / T (IEEE fp32 division).
+ *  3. top_k in [2, vocab): kappa = the top_k-th largest x; every token with x_i >= kappa is kept (ties at kappa included).
+ *  4. top_p < 1: the kept tokens in (x descending, index ascending) order; the shortest prefix whose mass (softmax of x over
+ *     the kept set) reaches top_p, at least one token. The masses are expf(x_i - max x) summed exactly in 64-bit fixed
+ *     point (2^-40 units), so the prefix equals the exact one unless a prefix mass at the boundary lies within a relative
+ *     1e-5 of top_p.
+ *  5. token = argmax over the kept set of x_i + g_i (lowest index among ties), g_i = -log(-log(u_i)), u_i = (2*(r >> 9) + 1)
+ *     * 2^-24 with r = word (i & 3) of Philox4x32-10(counter = {i >> 2, 0, lo32(t), hi32(t)}, key = {lo32(seed),
+ *     hi32(seed)}): a draw from softmax(x) over the kept set that depends only on the logits, the parameters, seed and t.
+ *  6. A row whose largest logit is NaN (torch.argmax's order: NaN above everything) or whose largest x is not finite
+ *     (+-inf, or an overflow of the division) gets the argmax of rule 1.
+ * Parameters are read on the device, so they are not checked at the call: a row with T < 0, top_k < 0 or top_p outside
+ * (0, 1] (or NaN) gets token -1. The token goes to tokens[b*tokens_stride + column]; with PKV_SAMPLE_ADVANCE, token_index[b]
+ * is incremented after the draw. No allocation, no synchronisation, fixed launch arguments: the launch replays in a CUDA
+ * graph with all per-request state in device memory. PKV_ERR_INVALID_ARG: batch outside [1, 2^20], vocab outside
+ * [1, 2^24], logits_stride < vocab, column outside [0, tokens_stride), null or misaligned pointers (2 bytes for the
+ * logits, 4 for temperature / top_k / top_p, 8 for seed / token_index / tokens), unknown flags. */
+#define PKV_SAMPLE_ADVANCE 1u
+typedef struct pkv_sample_desc {
+    uint32_t struct_bytes;  /* = sizeof(pkv_sample_desc) */
+    int32_t dtype;          /* pkv_dtype of the logits */
+    int32_t device;
+    int32_t batch;          /* rows */
+    int64_t vocab;          /* logits per row */
+    const void* logits; int64_t logits_stride;   /* elements between rows */
+    const float* temperature;   /* [batch] device arrays */
+    const int32_t* top_k;       /* 0: off */
+    const float* top_p;         /* 1: off */
+    const uint64_t* seed;
+    int64_t* token_index;
+    int64_t* tokens; int64_t tokens_stride; int64_t column;   /* int64 [batch, tokens_stride] */
+    uint32_t flags;         /* PKV_SAMPLE_ADVANCE */
+    uint32_t reserved;
+} pkv_sample_desc;
+int pkv_sample_tokens(const pkv_sample_desc* d, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

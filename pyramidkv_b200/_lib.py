@@ -22,7 +22,7 @@ EXPORTS = [
     "pkv_ragged_place_window", "pkv_decode_attn_ragged", "pkv_evict_single_launch", "pkv_stage_scan_pool",
     "pkv_evict_prefill_batch", "pkv_evict_batch_supported", "pkv_stage_batch", "pkv_decode_attn_batch",
     "pkv_decode_attn_batch_fp8", "pkv_cache_quantize_fp8", "pkv_decode_attn_batch_gqa", "pkv_decode_attn_batch_gqa_fp8",
-    "pkv_evict_pooled_kv_offset", "pkv_cache_install",
+    "pkv_evict_pooled_kv_offset", "pkv_cache_install", "pkv_sample_tokens",
 ]
 FLAG_GQA_SHARED = 128          # pkv_evict_desc.flags: one compacted cache per KV head
 
@@ -68,6 +68,19 @@ class RopeDesc(C.Structure):
         ("q", C.c_void_p), ("q_stride_h", C.c_int64), ("q_stride_s", C.c_int64),
         ("k", C.c_void_p), ("k_stride_h", C.c_int64), ("k_stride_s", C.c_int64),
         ("cos", C.c_void_p), ("sin", C.c_void_p), ("cs_stride_s", C.c_int64),
+    ]
+
+
+SAMPLE_ADVANCE = 1            # pkv_sample_desc.flags: token_index[b] += 1 after the draw
+
+
+class SampleDesc(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("dtype", C.c_int32), ("device", C.c_int32), ("batch", C.c_int32),
+        ("vocab", C.c_int64), ("logits", C.c_void_p), ("logits_stride", C.c_int64),
+        ("temperature", C.c_void_p), ("top_k", C.c_void_p), ("top_p", C.c_void_p), ("seed", C.c_void_p),
+        ("token_index", C.c_void_p), ("tokens", C.c_void_p), ("tokens_stride", C.c_int64), ("column", C.c_int64),
+        ("flags", C.c_uint32), ("reserved", C.c_uint32),
     ]
 
 
@@ -153,6 +166,8 @@ def lib() -> C.CDLL:
     # [2*layers] pointers; capacities and rows [layers] int64; rows_dev, dst_rows [layers] pointers), step_dev, stream
     L.pkv_cache_install.argtypes = [C.c_int32] * 7 + [p] * 11
     L.pkv_cache_install.restype = i32
+    L.pkv_sample_tokens.argtypes = [C.POINTER(SampleDesc), p]
+    L.pkv_sample_tokens.restype = i32
     if L.pkv_version() != 3:
         raise RuntimeError(f"libpkv ABI version {L.pkv_version()} != 3; rebuild with `python -m pyramidkv_b200.build --force`")
     _lib = L

@@ -891,6 +891,38 @@ int pkv_update_flatten_view(void* dst, const void* src, const void* state, const
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "flatten append launch");
 }
 
+int pkv_sample_tokens(const pkv_sample_desc* d, void* stream) {
+    const char* fn = "pkv_sample_tokens";
+    if (!d) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
+    if (d->struct_bytes != sizeof(pkv_sample_desc))
+        return fail(PKV_ERR_INVALID_ARG, "pkv_sample_desc.struct_bytes=%u, library expects %zu (ABI mismatch)", d->struct_bytes, sizeof(pkv_sample_desc));
+    if (d->dtype != PKV_BF16 && d->dtype != PKV_FP16) return fail(PKV_ERR_UNSUPPORTED_DTYPE, "%s: dtype %d: only bf16 (0) and fp16 (1) logits", fn, d->dtype);
+    if (d->batch < 1 || d->batch > (1 << 20)) return fail(PKV_ERR_INVALID_ARG, "%s: batch=%d outside [1, 2^20]", fn, d->batch);
+    if (d->vocab < 1 || d->vocab > (int64_t(1) << 24)) return fail(PKV_ERR_INVALID_ARG, "%s: vocab=%lld outside [1, 2^24]", fn, (long long)d->vocab);
+    if (d->logits_stride < d->vocab) return fail(PKV_ERR_INVALID_ARG, "%s: logits_stride=%lld < vocab=%lld", fn, (long long)d->logits_stride, (long long)d->vocab);
+    if (d->column < 0 || d->column >= d->tokens_stride)
+        return fail(PKV_ERR_INVALID_ARG, "%s: column=%lld outside [0, tokens_stride=%lld)", fn, (long long)d->column, (long long)d->tokens_stride);
+    if (d->flags & ~PKV_SAMPLE_ADVANCE) return fail(PKV_ERR_INVALID_ARG, "%s: unknown flags 0x%x", fn, d->flags);
+    auto bad = [](const void* p, uintptr_t align) { return !p || (reinterpret_cast<uintptr_t>(p) & (align - 1)); };
+    if (bad(d->logits, 2)) return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned logits (2 bytes)", fn);
+    if (bad(d->temperature, 4) || bad(d->top_k, 4) || bad(d->top_p, 4))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned temperature / top_k / top_p (4 bytes)", fn);
+    if (bad(d->seed, 8) || bad(d->token_index, 8) || bad(d->tokens, 8))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned seed / token_index / tokens (8 bytes)", fn);
+    const DevInfo* di = nullptr;
+    int rc = device_info(d->device, &di);
+    if (rc) return rc;
+    SampleArgs a;
+    a.dtype = d->dtype; a.B = d->batch; a.V = int(d->vocab);
+    a.logits = static_cast<const uint16_t*>(d->logits); a.ld = d->logits_stride;
+    a.temperature = d->temperature; a.top_k = d->top_k; a.top_p = d->top_p; a.seed = d->seed; a.token_index = d->token_index;
+    a.tokens = d->tokens; a.tokens_ld = d->tokens_stride; a.col = d->column;
+    a.advance = (d->flags & PKV_SAMPLE_ADVANCE) != 0;
+    DeviceGuard guard(d->device);
+    const cudaError_t e = launch_sample(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "sample launch");
+}
+
 int pkv_cache_append(const pkv_decode_desc* d, void* stream) {
     DecodeArgs a;
     int rc = resolve_decode(d, &a, false);

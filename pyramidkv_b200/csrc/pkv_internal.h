@@ -178,6 +178,22 @@ struct InstallArgs {
 };
 cudaError_t launch_install(const InstallArgs& a, int row_bytes, int num_sms, cudaStream_t st);
 
+// one sampled token per row of logits (pkv_sample.cu): one CTA per row
+struct SampleArgs {
+    int dtype, B, V;
+    const uint16_t* logits;
+    int64_t ld;                 // elements between rows
+    const float* temperature;   // per-row device parameters [B]
+    const int32_t* top_k;
+    const float* top_p;
+    const uint64_t* seed;
+    int64_t* token_index;
+    int64_t* tokens;            // token of row b at tokens[b * tokens_ld + col]
+    int64_t tokens_ld, col;
+    bool advance;               // token_index[b] += 1 after the draw
+};
+cudaError_t launch_sample(const SampleArgs& a, cudaStream_t st);
+
 // RoPE in place on Q and K (pkv_rope.cu)
 struct RopeArgs {
     int dtype, Hq, Hkv, D;

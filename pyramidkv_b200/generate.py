@@ -25,16 +25,82 @@ launch per layer.
 `greedy_generate_continuous` keeps a fixed number of slots busy: when a sequence stops (EOS or its own `max_new_tokens`),
 the next waiting prompt is prefilled and copied into its slot in place (`pkv_cache_install`, one launch for every layer),
 while the captured step graph keeps replaying unchanged.
+
+All three loops are greedy by default. `sampling=SamplingParams(...)` (or one per prompt) draws each token instead - the
+prefill's with token index t = 0, decode step n's with t = n - with temperature, top-k, top-p and a per-request seed, one
+`pkv_sample_tokens` launch per step for the whole batch in place of the argmax (DESIGN.md §4.6). A request's tokens depend
+only on its logits, its parameters and its seed, not on its batch position, slot or the graph.
 """
 from __future__ import annotations
 
 import time
 from dataclasses import dataclass
-from typing import Optional
+from typing import List, Optional
 
 import torch
 
 from .cache import PkvBatchCacheLayer, PkvCacheLayer, admit_cache, join_caches, park_cache
+
+
+@dataclass(frozen=True)
+class SamplingParams:
+    """One request's sampling settings, applied in HF's warper order: temperature, top-k, top-p, then the draw.
+    temperature 0 or top_k 1: the greedy token. top_k 0 and top_p 1 switch those filters off. The temperature is used as an
+    fp32 value; the 64-bit seed and the token index key the Philox stream of the Gumbel-max draw (DESIGN.md §4.6)."""
+    temperature: float = 1.0
+    top_k: int = 0
+    top_p: float = 1.0
+    seed: int = 0
+
+    def __post_init__(self):
+        if not float(self.temperature) >= 0.0:
+            raise ValueError(f"SamplingParams: temperature must be >= 0, got {self.temperature}")
+        if int(self.top_k) != self.top_k or int(self.top_k) < 0:
+            raise ValueError(f"SamplingParams: top_k must be an integer >= 0, got {self.top_k}")
+        if not 0.0 < float(self.top_p) <= 1.0:
+            raise ValueError(f"SamplingParams: top_p must be in (0, 1], got {self.top_p}")
+        if int(self.seed) != self.seed or not 0 <= int(self.seed) < 2 ** 64:
+            raise ValueError(f"SamplingParams: seed must be an integer in [0, 2^64), got {self.seed}")
+
+
+def _seed_i64(seed: int) -> int:
+    seed = int(seed)
+    return seed - 2 ** 64 if seed >= 2 ** 63 else seed      # the same 64 bits in an int64 tensor
+
+
+class SamplingState:
+    """The per-row device state `sample_tokens` reads: parameters and the token index of each row (sequence or slot).
+    Rows are rewritten in place (`set_row`), so a captured graph keeps its pointers."""
+
+    def __init__(self, params: List[SamplingParams], device, index: int = 0):
+        self.temperature = torch.tensor([float(p.temperature) for p in params], dtype=torch.float32, device=device)
+        self.top_k = torch.tensor([min(int(p.top_k), 2 ** 31 - 1) for p in params], dtype=torch.int32, device=device)
+        self.top_p = torch.tensor([float(p.top_p) for p in params], dtype=torch.float32, device=device)
+        self.seed = torch.tensor([_seed_i64(p.seed) for p in params], dtype=torch.int64, device=device)
+        self.index = torch.full((len(params),), int(index), dtype=torch.int64, device=device)
+
+    def set_row(self, row: int, p: SamplingParams, index: int) -> None:
+        self.temperature[row] = float(p.temperature)
+        self.top_k[row] = min(int(p.top_k), 2 ** 31 - 1)
+        self.top_p[row] = float(p.top_p)
+        self.seed[row] = _seed_i64(p.seed)
+        self.index[row] = int(index)
+
+
+def _sampling_list(sampling, n: int, what: str):
+    """None, one SamplingParams for every prompt, or one per prompt -> None or a list of n."""
+    if sampling is None:
+        return None
+    if isinstance(sampling, SamplingParams):
+        return [sampling] * n
+    out = list(sampling)
+    if len(out) != n or not all(isinstance(p, SamplingParams) for p in out):
+        raise ValueError(f"{what}: sampling must be a SamplingParams or one per prompt ({n})")
+    return out
+
+
+def _backend(model):
+    return model.model.layers[0].self_attn.kv_cluster.backend
 
 
 @dataclass
@@ -50,22 +116,24 @@ class StaticDecoder:
     PkvCacheLayer entries - one prompt, an equal-length batch prefilled as one forward, or prompts joined by
     `cache.join_caches`; first_token: the token the prefill produced per sequence ([B] or [B, 1] int64).
     eos_token_id (int or list): a sequence that produced one is done - it keeps decoding in lock-step, but its tokens are
-    `pad_token_id` from then on (on the device: `done` [B]); None masks nothing."""
+    `pad_token_id` from then on (on the device: `done` [B]); None masks nothing. sampling: None (greedy: the argmax) or one
+    SamplingParams per sequence, whose first decode step draws with token index 1 (the prefill's token is t = 0)."""
 
     def __init__(self, model, cache, first_token: torch.Tensor, max_steps: int, use_graph: Optional[bool] = None,
-                 eos_token_id=None, pad_token_id: int = 0):
+                 eos_token_id=None, pad_token_id: int = 0, sampling: Optional[List[SamplingParams]] = None):
         layers = [l for l in cache.layers if isinstance(l, PkvCacheLayer)]
         if len(layers) != model.config.num_hidden_layers:
             raise RuntimeError("StaticDecoder needs a cache prefilled by the patched forward on every layer "
                                "(method 'fullkv' and stock caches go through model.generate)")
         for l in layers:
             l.reserve(int(max_steps))                      # off the per-token path: no reallocation while the graph lives
-        self._setup(model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id)
+        self._setup(model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling)
         self.done = None if self.eos is None else (self.ids == self.eos[None, :]).any(dim=1, keepdim=True)   # [B, 1]
 
-    def _setup(self, model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id) -> None:
+    def _setup(self, model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling) -> None:
         """The state both decoders hold: the step counter and workspace the decode launches read, the per-sequence input
-        ids and positions, the token buffer [B, max_steps] and its cursor, and the EOS ids."""
+        ids and positions, the token buffer [B, max_steps] and its cursor, the EOS ids and, when sampling, the per-sequence
+        sampling state with the buffer the sampled tokens land in."""
         self.model, self.cache, self.layers, self.max_steps = model, cache, layers, int(max_steps)
         dev = layers[0].device
         bsz = layers[0].k_buf.shape[0]
@@ -84,10 +152,17 @@ class StaticDecoder:
         self.taken = 0
         self.graph = None
         self.use_graph = (dev.type == "cuda") if use_graph is None else bool(use_graph)
+        self.sampling = None
+        if sampling is not None:
+            if len(sampling) != bsz:
+                raise ValueError(f"{len(sampling)} SamplingParams for {bsz} sequences")
+            self.sampling = SamplingState(sampling, dev, index=1)
+            self.sampled = torch.zeros(bsz, 1, dtype=torch.long, device=dev)
         cache._pkv_static = self.state
 
     def _greedy_token(self) -> torch.Tensor:
-        """The forward of one token per sequence through every layer (appending to the cache); the argmax [B, 1]."""
+        """The forward of one token per sequence through every layer (appending to the cache); the argmax [B, 1], or with
+        sampling the drawn tokens (one `sample_tokens` launch for every sequence; each token index advances by one)."""
         m = self.model.model
         h = m.embed_tokens(self.ids)
         pos_emb = m.rotary_emb(h, position_ids=self.pos)
@@ -96,6 +171,9 @@ class StaticDecoder:
                       past_key_values=self.cache, use_cache=True)
         h = m.norm(h)
         logits = self.model.lm_head(h[:, -1, :])
+        if self.sampling is not None:
+            self.backend.sample_tokens(logits, self.sampling, self.sampled, 0)
+            return self.sampled
         return logits.argmax(dim=-1, keepdim=True)                      # [B, 1]
 
     # one greedy step; every tensor it touches is static, every launch argument constant
@@ -112,7 +190,8 @@ class StaticDecoder:
 
     def _counters(self) -> list:
         """The device tensors a step advances (restored after the warm-up step of a capture)."""
-        return [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done) if t is not None]
+        idx = self.sampling.index if self.sampling is not None else None
+        return [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done, idx) if t is not None]
 
     def _capture(self) -> None:
         # warm up on a side stream (lazy initialisation, cuBLAS workspaces), restore the counters, then capture
@@ -162,15 +241,21 @@ class StaticDecoder:
         self.taken = 0
 
 
-def _prefill(model, input_ids: torch.Tensor):
-    """Prefill (+ eviction in every patched layer) of one prompt: (first token [1, 1], cache)."""
+def _prefill(model, input_ids: torch.Tensor, sampling: Optional[SamplingParams] = None):
+    """Prefill (+ eviction in every patched layer) of one prompt: (first token [1, 1], cache). The token is the argmax, or
+    with `sampling` drawn with token index 0."""
     from transformers import DynamicCache
     if hasattr(model, "prepare_inputs_for_generation"):
         for layer in model.model.layers:                 # what the patched prepare_inputs does on an empty cache (llama_model.py:2609-2612)
             layer.self_attn.kv_seq_len = 0
     cache = DynamicCache(config=model.config)
     out = model(input_ids=input_ids, past_key_values=cache, use_cache=True, logits_to_keep=1)
-    return out.logits[:, -1, :].argmax(dim=-1, keepdim=True), cache
+    if sampling is None:
+        return out.logits[:, -1, :].argmax(dim=-1, keepdim=True), cache
+    logits = out.logits[:, -1, :]
+    first = torch.zeros(1, 1, dtype=torch.long, device=logits.device)
+    _backend(model).sample_tokens(logits, SamplingState([sampling], logits.device, index=0), first, 0, advance=False)
+    return first, cache
 
 
 def _eos_set(eos_token_id) -> set:
@@ -181,8 +266,10 @@ def _eos_set(eos_token_id) -> set:
 
 @torch.no_grad()
 def greedy_generate(model, input_ids: torch.Tensor, max_new_tokens: int, use_graph: Optional[bool] = None,
-                    return_cache: bool = False, eos_token_id=None, check_every: int = 16):
-    """Prefill (+ eviction in every patched layer) then up to `max_new_tokens - 1` static decode steps.
+                    return_cache: bool = False, eos_token_id=None, check_every: int = 16,
+                    sampling: Optional[SamplingParams] = None):
+    """Prefill (+ eviction in every patched layer) then up to `max_new_tokens - 1` static decode steps. Greedy unless
+    `sampling` (a SamplingParams) is given: every token is then drawn with it (DESIGN.md §4.6).
     Returns sequences [1, prompt + generated] like `generate(...).sequences` (and the cache on request).
     `eos_token_id` (int or list, as the reference runner passes it: run_longbench.py:270-272) ends the generation with the first
     such token (kept, like HF); the device never waits for the host, so the tokens are inspected every `check_every` steps
@@ -190,10 +277,13 @@ def greedy_generate(model, input_ids: torch.Tensor, max_new_tokens: int, use_gra
     if input_ids.dim() != 2 or input_ids.shape[0] != 1:
         raise NotImplementedError("batch size 1 (as in the reference: README.md:47); greedy_generate_batch decodes several prompts together")
     eos = _eos_set(eos_token_id)
-    first, cache = _prefill(model, input_ids)
+    if sampling is not None and not isinstance(sampling, SamplingParams):
+        raise ValueError("greedy_generate: sampling must be a SamplingParams")
+    first, cache = _prefill(model, input_ids, sampling)
     toks = [first]
     if max_new_tokens > 1 and not (eos and int(first) in eos):
-        dec = StaticDecoder(model, cache, first, max_new_tokens - 1, use_graph=use_graph)
+        dec = StaticDecoder(model, cache, first, max_new_tokens - 1, use_graph=use_graph,
+                            sampling=None if sampling is None else [sampling])
         if not eos:
             toks.append(dec.run(max_new_tokens - 1).clone())
         else:
@@ -216,19 +306,21 @@ def greedy_generate(model, input_ids: torch.Tensor, max_new_tokens: int, use_gra
 
 @torch.no_grad()
 def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None, pad_token_id: int = 0,
-                          use_graph: Optional[bool] = None, check_every: int = 16, return_cache: bool = False):
+                          use_graph: Optional[bool] = None, check_every: int = 16, return_cache: bool = False, sampling=None):
     """Greedy generation for several prompts of any lengths (1-D or [1, S] id tensors): each prompt is prefilled alone
     exactly as `greedy_generate` does, the compacted caches are joined, and up to `max_new_tokens - 1` steps decode all of
     them together (`StaticDecoder` over the joined cache). Each sequence stops at its first `eos_token_id` (kept, like HF);
     the loop ends once all are done, which the host checks every `check_every` steps. Returns one 1-D tensor per prompt,
-    prompt + generated (and the joined cache on request, its per-sequence rows ending at each EOS)."""
+    prompt + generated (and the joined cache on request, its per-sequence rows ending at each EOS). Greedy unless `sampling`
+    (one SamplingParams for all prompts, or one per prompt) is given: each prompt's tokens are then drawn with its own."""
     ids = [p.reshape(1, -1) for p in prompts]
     if not ids:
         raise ValueError("greedy_generate_batch: no prompts")
     eos = _eos_set(eos_token_id)
+    samp = _sampling_list(sampling, len(ids), "greedy_generate_batch")
     firsts, caches = [], []
-    for p in ids:
-        f, c = _prefill(model, p)
+    for i, p in enumerate(ids):
+        f, c = _prefill(model, p, None if samp is None else samp[i])
         firsts.append(f)
         caches.append(c)
     first = torch.cat(firsts)                                            # [B, 1]
@@ -240,7 +332,7 @@ def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None
     gen = torch.empty(len(ids), 0, dtype=torch.long)
     if steps and not all(t in eos for t in first_host):
         dec = StaticDecoder(model, cache, first, steps, use_graph=use_graph, eos_token_id=sorted(eos) if eos else None,
-                            pad_token_id=pad_token_id)
+                            pad_token_id=pad_token_id, sampling=samp)
         while dec.taken < steps:
             dec.run(min(max(1, check_every) if eos else steps, steps - dec.taken))
             if eos and bool(dec.done.all()):                            # one device-to-host read per chunk
@@ -269,11 +361,11 @@ class ContinuousDecoder(StaticDecoder):
     when an admission needs more rows; the graph is then captured again."""
 
     def __init__(self, model, cache, first_token: torch.Tensor, left, chunk: int, use_graph: Optional[bool] = None,
-                 eos_token_id=None, pad_token_id: int = 0):
+                 eos_token_id=None, pad_token_id: int = 0, sampling: Optional[List[SamplingParams]] = None):
         layers = [l for l in cache.layers if isinstance(l, PkvBatchCacheLayer)]
         if len(layers) != model.config.num_hidden_layers or len(layers) != len(cache.layers):
             raise RuntimeError("ContinuousDecoder needs a batched cache (cache.join_caches) on every layer")
-        self._setup(model, cache, layers, first_token, max(1, int(chunk)), use_graph, eos_token_id, pad_token_id)
+        self._setup(model, cache, layers, first_token, max(1, int(chunk)), use_graph, eos_token_id, pad_token_id, sampling)
         # every layer's row counts are rows of one tensor, so one op per step stops them growing for the done slots
         self.rows_all = torch.stack([l.rows for l in layers])
         for i, l in enumerate(layers):
@@ -322,9 +414,14 @@ class ContinuousDecoder(StaticDecoder):
             self.graph = None
         return grew
 
-    def admit(self, slot: int, src_cache, first_token: torch.Tensor, left: int) -> None:
-        """Slot `slot` continues the prefilled prompt `src_cache` (first token `first_token`, `left` decode steps)."""
+    def admit(self, slot: int, src_cache, first_token: torch.Tensor, left: int, sampling: Optional[SamplingParams] = None) -> None:
+        """Slot `slot` continues the prefilled prompt `src_cache` (first token `first_token`, `left` decode steps); a sampling
+        decoder takes the request's `sampling` parameters, its next token drawn with token index 1."""
+        if (sampling is None) != (self.sampling is None):
+            raise ValueError("admit: pass sampling parameters exactly when the decoder samples")
         admit_cache(self.cache, slot, src_cache, self.state.step, self.backend)
+        if sampling is not None:
+            self.sampling.set_row(slot, sampling, 1)
         self.ids[slot] = first_token.reshape(-1)[:1].to(self.ids.device)
         self.pos[slot] = self.layers[0].seq_seen[slot]
         self.left[slot] = int(left)
@@ -354,7 +451,8 @@ def _sync(device: torch.device) -> None:
 
 @torch.no_grad()
 def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, eos_token_id=None, pad_token_id: int = 0,
-                               use_graph: Optional[bool] = None, check_every: int = 16, return_stats: bool = False):
+                               use_graph: Optional[bool] = None, check_every: int = 16, return_stats: bool = False,
+                               sampling=None):
     """Greedy generation for any number of prompts (1-D or [1, S] id tensors) through `num_slots` sequences decoded together
     (continuous batching). `max_new_tokens`: an int, or one per prompt. The first `num_slots` prompts are prefilled one at a
     time and joined exactly as in `greedy_generate_batch`; decoding then runs in chunks of `check_every` steps. After each
@@ -364,7 +462,9 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     format of `greedy_generate_batch`), and with `return_stats` a dict: decode_steps, live_slot_steps (the sum over steps
     of the slots holding an unfinished sequence), admissions (prompts admitted after the start), regrowths, graph_captures,
     prefill_s / decode_s (host wall time of the prefills and of the rest of the loop) and per prompt `prefill_ms` and
-    `cache_rows_first_last` (rows of its first and last layer after the prefill)."""
+    `cache_rows_first_last` (rows of its first and last layer after the prefill). Greedy unless `sampling` (one
+    SamplingParams for all prompts, or one per prompt) is given: each request's tokens are then drawn with its own, and
+    equal those it gets from `greedy_generate_batch` with the same parameters wherever its logits are equal there."""
     ids = [p.reshape(1, -1) for p in prompts]
     if not ids:
         raise ValueError("greedy_generate_continuous: no prompts")
@@ -374,6 +474,7 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     if int(num_slots) < 1:
         raise ValueError(f"greedy_generate_continuous: num_slots must be >= 1, got {num_slots}")
     eos = _eos_set(eos_token_id)
+    samp = _sampling_list(sampling, len(ids), "greedy_generate_continuous")
     chunk = max(1, int(check_every))
     dev = ids[0].device
     gen = [[] for _ in ids]                        # generated tokens per prompt, the prefill's first token included
@@ -387,7 +488,7 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     def prefill(i):
         _sync(dev)
         t0 = time.perf_counter()
-        first, cache = _prefill(model, ids[i])
+        first, cache = _prefill(model, ids[i], None if samp is None else samp[i])
         gen[i].append(int(first))                  # waits for the prefill
         ms = (time.perf_counter() - t0) * 1e3
         stats["prefill_ms"][i] = ms
@@ -401,7 +502,8 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     del caches
     slot_req = list(range(B))
     dec = ContinuousDecoder(model, cache, torch.cat(firsts), [0 if finished(b) else caps[b] - 1 for b in range(B)], chunk,
-                            use_graph=use_graph, eos_token_id=sorted(eos) if eos else None, pad_token_id=pad_token_id)
+                            use_graph=use_graph, eos_token_id=sorted(eos) if eos else None, pad_token_id=pad_token_id,
+                            sampling=None if samp is None else samp[:B])
     waiting = B
     while True:
         for s in range(B):
@@ -415,7 +517,7 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
                 if finished(i):
                     continue
                 stats["regrowths"] += int(dec.grow_for(single, caps[i]))
-                dec.admit(s, single, first, caps[i] - 1)
+                dec.admit(s, single, first, caps[i] - 1, None if samp is None else samp[i])
                 stats["admissions"] += 1
                 slot_req[s] = i
             if slot_req[s] is None:

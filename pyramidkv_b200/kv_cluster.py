@@ -97,6 +97,10 @@ class CudaBackend:
     def rope_inplace(self, q, k, cos, sin):
         ops.rope_inplace(q, k, cos, sin)
 
+    # -- sampled decoding: one token per row of logits, per-row parameters in device memory --
+    def sample_tokens(self, logits, params, out, col, advance=True):
+        ops.sample_tokens(logits, params, out, col, advance)
+
     # -- ragged per-head budgets (AdaKV / HeadKV): scores first, budgets from the host, then select + gather --
     def ragged_begin(self, q, k, v, window_size, kernel_size, pooling):
         """Stages 1-2 (window logits, softmax + pool) into a workspace that stays alive until ragged_finish."""

@@ -683,3 +683,34 @@ def cache_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k_new: torch.Tens
     d.k_new, d.v_new = k_new.data_ptr(), v_new.data_ptr()
     d.k_cache, d.v_cache, d.cache_stride_h = k_cache.data_ptr(), v_cache.data_ptr(), k_cache.stride(0)
     _lib.check(_lib.lib().pkv_cache_append(C.byref(d), torch.cuda.current_stream(k_cache.device).cuda_stream))
+
+
+# ---- sampled decoding (include/pkv.h: pkv_sample_tokens, DESIGN.md §4.6) ----
+def sample_tokens(logits: torch.Tensor, params, out: torch.Tensor, col: int, advance: bool = True) -> None:
+    """One token per row of `logits` [B, V] (bf16 / fp16, rows may be strided) into out[:, col] (int64 [B, *]), in ONE
+    launch: temperature, top-k, top-p and a Gumbel-max draw keyed by Philox4x32-10 (seed, token index), each row with its
+    own parameters. `params` holds the per-row DEVICE tensors `temperature` (float32 [B]), `top_k` (int32), `top_p`
+    (float32), `seed` (int64, the 64 seed bits) and `index` (int64, the row's token index t; incremented in place when
+    `advance`) - generate.SamplingState. Nothing is read back: the launch replays in a CUDA graph."""
+    _require_cuda(logits, out, params.temperature, params.top_k, params.top_p, params.seed, params.index)
+    if logits.dim() != 2 or logits.stride(1) != 1:
+        raise ValueError(f"sample_tokens: logits must be [B, V] with contiguous rows, got {tuple(logits.shape)}")
+    B, V = logits.shape
+    if out.dim() != 2 or out.dtype != torch.long or out.shape[0] != B or out.stride(1) != 1:
+        raise ValueError(f"sample_tokens: out must be an int64 [B={B}, n] tensor with contiguous rows")
+    for name, dt in (("temperature", torch.float32), ("top_k", torch.int32), ("top_p", torch.float32), ("seed", torch.int64),
+                     ("index", torch.int64)):
+        t = getattr(params, name)
+        if t.dtype != dt or t.numel() != B or not t.is_contiguous() or t.device != logits.device:
+            raise ValueError(f"sample_tokens: params.{name} must be a contiguous {dt} tensor of B = {B} elements on {logits.device}")
+    d = _lib.SampleDesc()
+    d.struct_bytes = C.sizeof(_lib.SampleDesc)
+    d.dtype = _dtype_code(logits)
+    d.device = logits.device.index if logits.device.index is not None else torch.cuda.current_device()
+    d.batch, d.vocab = B, V
+    d.logits, d.logits_stride = logits.data_ptr(), logits.stride(0) if B > 1 else V
+    d.temperature, d.top_k, d.top_p = params.temperature.data_ptr(), params.top_k.data_ptr(), params.top_p.data_ptr()
+    d.seed, d.token_index = params.seed.data_ptr(), params.index.data_ptr()
+    d.tokens, d.tokens_stride, d.column = out.data_ptr(), out.stride(0) if B > 1 else out.shape[1], int(col)
+    d.flags = _lib.SAMPLE_ADVANCE if advance else 0
+    _lib.check(_lib.lib().pkv_sample_tokens(C.byref(d), torch.cuda.current_stream(logits.device).cuda_stream))
