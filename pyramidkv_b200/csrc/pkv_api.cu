@@ -555,14 +555,13 @@ static int resolve_decode(const pkv_decode_desc* d, DecodeArgs* a, bool need_q, 
     a->dtype = d->dtype; a->Hq = d->num_q_heads; a->Hkv = d->num_kv_heads; a->G = a->Hq / a->Hkv; a->D = d->head_dim;
     a->T = d->length;
     a->q = static_cast<const uint16_t*>(d->q); a->k_new = static_cast<const uint16_t*>(d->k_new); a->v_new = static_cast<const uint16_t*>(d->v_new);
-    a->k_cache = static_cast<uint16_t*>(d->k_cache); a->v_cache = static_cast<uint16_t*>(d->v_cache); a->out = static_cast<uint16_t*>(d->out);
+    a->k_cache = d->k_cache; a->v_cache = d->v_cache; a->out = static_cast<uint16_t*>(d->out);
     a->cache_sh = d->cache_stride_h;
     a->scale = d->softmax_scale != 0.f ? d->softmax_scale : 1.0f / sqrtf(float(d->head_dim));
     a->num_sms = di->sms;
     a->nsplit = decode_num_splits(a->Hq, rows_bound, a->num_sms);
     a->ws = static_cast<float*>(d->workspace);
     a->num_seqs = num_seqs;
-    a->cache_sb = int64_t(a->Hq) * a->cache_sh;
     a->max_rows = rows_bound;
     if (need_q && a->nsplit > 1) {
         const uint64_t need = uint64_t(num_seqs) * a->Hq * a->nsplit * (2 + a->D) * sizeof(float);
@@ -577,15 +576,6 @@ uint64_t pkv_decode_workspace_bytes(const pkv_decode_desc* d) {
     return uint64_t(d->num_q_heads) * 64 * (2 + uint64_t(d->head_dim)) * sizeof(float);
 }
 
-int pkv_decode_attn(const pkv_decode_desc* d, void* stream) {
-    DecodeArgs a;
-    int rc = resolve_decode(d, &a, true);
-    if (rc) return rc;
-    DeviceGuard guard(d->device);
-    const cudaError_t e = launch_decode(a, static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "decode launch");
-}
-
 // The argument checks every device-length decode entry point shares.
 static int check_devlen_args(const char* fn, int32_t num_seqs, const int32_t* rows, const int32_t* step_dev, int64_t max_length) {
     if ((reinterpret_cast<uintptr_t>(rows) & 3u) || (reinterpret_cast<uintptr_t>(step_dev) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned int32 pointer", fn);
@@ -594,116 +584,79 @@ static int check_devlen_args(const char* fn, int32_t num_seqs, const int32_t* ro
     return PKV_OK;
 }
 
-// The device-length decode of num_seqs sequences: pkv_decode_attn_batch, and pkv_decode_attn_graph / pkv_decode_attn_ragged
-// as its one-sequence calls.
-static int decode_devlen(const char* fn, const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
-                         const int32_t* step_dev, int64_t max_length, void* stream) {
-    int rc = check_devlen_args(fn, num_seqs, rows, step_dev, max_length);
+// E4M3 caches: one fp32 scale per row for K and for V, `stride_h` / `stride_b` floats between heads / sequences
+struct DecodeScales {
+    float *k, *v;
+    int64_t stride_h, stride_b;
+};
+
+// The decode of every cache form behind the seven entry points: num_seqs sequences with a cache per query head, or with a
+// GQA-shared cache per KV head (`shared`), of 16-bit rows or of E4M3 rows (`scales`). host_length: pkv_decode_attn, the
+// `length` rows of one sequence (num_seqs, rows, step_dev and max_length are not used); otherwise every device-length
+// argument is checked.
+static int decode(const char* fn, const pkv_decode_desc* d, bool shared, const DecodeScales* scales, bool host_length, int32_t num_seqs,
+                  int64_t cache_stride_b, const int32_t* rows, const int32_t* step_dev, int64_t max_length, void* stream) {
+    int rc = host_length ? PKV_OK : check_devlen_args(fn, num_seqs, rows, step_dev, max_length);
     if (rc) return rc;
+    if (scales && (!scales->k || !scales->v)) return fail(PKV_ERR_INVALID_ARG, "%s: null scale pointer", fn);
+    if (scales && ((reinterpret_cast<uintptr_t>(scales->k) & 3u) || (reinterpret_cast<uintptr_t>(scales->v) & 3u)))
+        return fail(PKV_ERR_INVALID_ARG, "%s: misaligned scale pointer", fn);
     DecodeArgs a;
-    rc = resolve_decode(d, &a, true, max_length, num_seqs);
+    rc = resolve_decode(d, &a, true, host_length ? 0 : max_length, num_seqs);
     if (rc) return rc;
-    if (num_seqs > 1 && (cache_stride_b < int64_t(a.Hq) * a.cache_sh || cache_stride_b % 8))
-        return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_b=%lld is below num_q_heads*cache_stride_h=%lld or not a multiple of 8", fn,
-                    (long long)cache_stride_b, (long long)(int64_t(a.Hq) * a.cache_sh));
-    if (num_seqs > 1) a.cache_sb = cache_stride_b;
-    a.devlen = true;
+    if (shared && a.G != 2 && a.G != 4 && a.G != 8)
+        return fail(PKV_ERR_UNSUPPORTED, "%s: group size num_q_heads/num_kv_heads = %d: the grouped kernels are built for 2, 4 and 8", fn, a.G);
+    const int64_t align = scales ? 16 : 8;   // cache strides in elements that keep every row 16-byte aligned
+    if (a.cache_sh % align) return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_h=%lld is not a multiple of 16 bytes", fn, (long long)a.cache_sh);
+    const int heads = shared ? a.Hkv : a.Hq;   // cache heads per sequence
+    a.cache_sb = heads * a.cache_sh;
+    if (num_seqs > 1) {
+        if (cache_stride_b < a.cache_sb || cache_stride_b % align)
+            return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_b=%lld is below num_%s_heads*cache_stride_h=%lld or not a multiple of 16 bytes", fn,
+                        (long long)cache_stride_b, shared ? "kv" : "q", (long long)a.cache_sb);
+        a.cache_sb = cache_stride_b;
+    }
+    if (scales) {
+        if (scales->stride_h < max_length || (num_seqs > 1 && scales->stride_b < heads * scales->stride_h))
+            return fail(PKV_ERR_INVALID_ARG, "%s: scale strides (%lld, %lld) hold fewer than max_length=%lld rows per cache head", fn,
+                        (long long)scales->stride_h, (long long)scales->stride_b, (long long)max_length);
+        a.k_scale = scales->k;
+        a.v_scale = scales->v;
+        a.scale_sh = scales->stride_h;
+        a.scale_sb = num_seqs > 1 ? scales->stride_b : heads * scales->stride_h;
+    }
+    a.heads_per_cache = shared ? a.G : 1;
     a.rows = rows;
     a.step_dev = step_dev;
     DeviceGuard guard(d->device);
     const cudaError_t e = launch_decode(a, static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "decode launch");
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, fn);
 }
+
+int pkv_decode_attn(const pkv_decode_desc* d, void* stream) { return decode("pkv_decode_attn", d, false, nullptr, true, 1, 0, nullptr, nullptr, 0, stream); }
 
 int pkv_decode_attn_batch(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
                           const int32_t* step_dev, int64_t max_length, void* stream) {
-    return decode_devlen("pkv_decode_attn_batch", d, num_seqs, cache_stride_b, rows, step_dev, max_length, stream);
+    return decode("pkv_decode_attn_batch", d, false, nullptr, false, num_seqs, cache_stride_b, rows, step_dev, max_length, stream);
 }
 
 int pkv_decode_attn_batch_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
                               const int32_t* step_dev, int64_t max_length, float* k_scale, float* v_scale, int64_t scale_stride_h,
                               int64_t scale_stride_b, void* stream) {
-    const char* fn = "pkv_decode_attn_batch_fp8";
-    int rc = check_devlen_args(fn, num_seqs, rows, step_dev, max_length);
-    if (rc) return rc;
-    if (!k_scale || !v_scale) return fail(PKV_ERR_INVALID_ARG, "%s: null scale pointer", fn);
-    if ((reinterpret_cast<uintptr_t>(k_scale) & 3u) || (reinterpret_cast<uintptr_t>(v_scale) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned scale pointer", fn);
-    DecodeArgs a;
-    rc = resolve_decode(d, &a, true, max_length, num_seqs);
-    if (rc) return rc;
-    if (a.cache_sh % 16) return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_h=%lld bytes is not a multiple of 16", fn, (long long)a.cache_sh);
-    if (num_seqs > 1 && (cache_stride_b < int64_t(a.Hq) * a.cache_sh || cache_stride_b % 16))
-        return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_b=%lld is below num_q_heads*cache_stride_h=%lld or not a multiple of 16", fn,
-                    (long long)cache_stride_b, (long long)(int64_t(a.Hq) * a.cache_sh));
-    if (scale_stride_h < max_length || (num_seqs > 1 && scale_stride_b < int64_t(a.Hq) * scale_stride_h))
-        return fail(PKV_ERR_INVALID_ARG, "%s: scale strides (%lld, %lld) hold fewer than max_length=%lld rows per head", fn,
-                    (long long)scale_stride_h, (long long)scale_stride_b, (long long)max_length);
-    if (num_seqs > 1) a.cache_sb = cache_stride_b;
-    a.devlen = true;
-    a.rows = rows;
-    a.step_dev = step_dev;
-    a.k_scale = k_scale;
-    a.v_scale = v_scale;
-    a.scale_sh = scale_stride_h;
-    a.scale_sb = num_seqs > 1 ? scale_stride_b : int64_t(a.Hq) * scale_stride_h;
-    DeviceGuard guard(d->device);
-    const cudaError_t e = launch_decode_fp8(a, static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "fp8 decode launch");
-}
-
-// GQA-shared caches: the checks of pkv_decode_attn_batch(_fp8) with KV-head strides; `elem` = bytes per cached element.
-static int resolve_decode_gqa(const char* fn, const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
-                              const int32_t* step_dev, int64_t max_length, int elem, DecodeArgs* a) {
-    int rc = check_devlen_args(fn, num_seqs, rows, step_dev, max_length);
-    if (rc) return rc;
-    rc = resolve_decode(d, a, true, max_length, num_seqs);
-    if (rc) return rc;
-    if (a->G != 2 && a->G != 4 && a->G != 8)
-        return fail(PKV_ERR_UNSUPPORTED, "%s: group size num_q_heads/num_kv_heads = %d: the grouped kernels are built for 2, 4 and 8", fn, a->G);
-    const int64_t align = 16 / elem;   // cache strides in elements that keep every row 16-byte aligned
-    if (a->cache_sh % align) return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_h=%lld is not a multiple of 16 bytes", fn, (long long)a->cache_sh);
-    a->cache_sb = int64_t(a->Hkv) * a->cache_sh;
-    if (num_seqs > 1) {
-        if (cache_stride_b < a->cache_sb || cache_stride_b % align)
-            return fail(PKV_ERR_INVALID_ARG, "%s: cache_stride_b=%lld is below num_kv_heads*cache_stride_h=%lld or not a multiple of 16 bytes", fn,
-                        (long long)cache_stride_b, (long long)a->cache_sb);
-        a->cache_sb = cache_stride_b;
-    }
-    a->devlen = true;
-    a->rows = rows;
-    a->step_dev = step_dev;
-    return PKV_OK;
+    const DecodeScales scales{k_scale, v_scale, scale_stride_h, scale_stride_b};
+    return decode("pkv_decode_attn_batch_fp8", d, false, &scales, false, num_seqs, cache_stride_b, rows, step_dev, max_length, stream);
 }
 
 int pkv_decode_attn_batch_gqa(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
                               const int32_t* step_dev, int64_t max_length, void* stream) {
-    DecodeArgs a;
-    const int rc = resolve_decode_gqa("pkv_decode_attn_batch_gqa", d, num_seqs, cache_stride_b, rows, step_dev, max_length, 2, &a);
-    if (rc) return rc;
-    DeviceGuard guard(d->device);
-    const cudaError_t e = launch_decode_gqa(a, static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "grouped decode launch");
+    return decode("pkv_decode_attn_batch_gqa", d, true, nullptr, false, num_seqs, cache_stride_b, rows, step_dev, max_length, stream);
 }
 
 int pkv_decode_attn_batch_gqa_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
                                   const int32_t* step_dev, int64_t max_length, float* k_scale, float* v_scale,
                                   int64_t scale_stride_h, int64_t scale_stride_b, void* stream) {
-    const char* fn = "pkv_decode_attn_batch_gqa_fp8";
-    if (!k_scale || !v_scale) return fail(PKV_ERR_INVALID_ARG, "%s: null scale pointer", fn);
-    if ((reinterpret_cast<uintptr_t>(k_scale) & 3u) || (reinterpret_cast<uintptr_t>(v_scale) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned scale pointer", fn);
-    DecodeArgs a;
-    const int rc = resolve_decode_gqa(fn, d, num_seqs, cache_stride_b, rows, step_dev, max_length, 1, &a);
-    if (rc) return rc;
-    if (scale_stride_h < max_length || (num_seqs > 1 && scale_stride_b < int64_t(a.Hkv) * scale_stride_h))
-        return fail(PKV_ERR_INVALID_ARG, "%s: scale strides (%lld, %lld) hold fewer than max_length=%lld rows per KV head", fn,
-                    (long long)scale_stride_h, (long long)scale_stride_b, (long long)max_length);
-    a.k_scale = k_scale;
-    a.v_scale = v_scale;
-    a.scale_sh = scale_stride_h;
-    a.scale_sb = num_seqs > 1 ? scale_stride_b : int64_t(a.Hkv) * scale_stride_h;
-    DeviceGuard guard(d->device);
-    const cudaError_t e = launch_decode_gqa_fp8(a, static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "grouped fp8 decode launch");
+    const DecodeScales scales{k_scale, v_scale, scale_stride_h, scale_stride_b};
+    return decode("pkv_decode_attn_batch_gqa_fp8", d, true, &scales, false, num_seqs, cache_stride_b, rows, step_dev, max_length, stream);
 }
 
 int pkv_cache_quantize_fp8(int32_t dtype, int32_t num_seqs, int32_t num_heads, int32_t head_dim, int32_t device, int32_t num_layers,
@@ -817,7 +770,7 @@ int pkv_cache_install(int32_t elem_bytes, int32_t num_seqs, int32_t num_heads, i
 
 int pkv_decode_attn_graph(const pkv_decode_desc* d, const int32_t* step_dev, int64_t max_length, void* stream) {
     if (!step_dev) return fail(PKV_ERR_INVALID_ARG, "pkv_decode_attn_graph: null step counter");
-    return decode_devlen("pkv_decode_attn_graph", d, 1, 0, nullptr, step_dev, max_length, stream);
+    return decode("pkv_decode_attn_graph", d, false, nullptr, false, 1, 0, nullptr, step_dev, max_length, stream);
 }
 
 int pkv_rope_inplace(const pkv_rope_desc* d, void* stream) {
@@ -874,7 +827,7 @@ int pkv_ragged_place_window(const pkv_evict_desc* d, const int32_t* caps, void* 
 
 int pkv_decode_attn_ragged(const pkv_decode_desc* d, const int32_t* head_rows, const int32_t* step_dev, int64_t max_length, void* stream) {
     if (!head_rows) return fail(PKV_ERR_INVALID_ARG, "pkv_decode_attn_ragged: null head_rows");
-    return decode_devlen("pkv_decode_attn_ragged", d, 1, 0, head_rows, step_dev, max_length, stream);
+    return decode("pkv_decode_attn_ragged", d, false, nullptr, false, 1, 0, head_rows, step_dev, max_length, stream);
 }
 
 int pkv_update_flatten_view(void* dst, const void* src, const void* state, const int32_t* head_lens, const int32_t* cu_lens,

@@ -1,15 +1,18 @@
-// pkv_decode.cu — decode step over the compacted per-query-head cache: in-place append + attention.
+// pkv_decode.cu — decode step over the compacted cache: in-place append + attention, one kernel for every cache form.
 //
 // Replaces, per layer and token: DynamicCache.update's torch.cat of the whole layer cache
 // (cache_utils_think.py:383-384, called at llama_model.py:170 / :288 / :403), the two transposes and the
 // attention launch (eager llama_model.py:174-183, sdpa :291-313, flash :411-445 -> flash_attn_func :77).
 // q_len == 1 and every cached row is visible, so there is no mask. One launch for T <= 256 rows per
 // head; longer caches are split along T (flash-decoding) and merged by a second small kernel.
-// Several sequences decoded in lock-step share one launch: the grid is (split, q head, sequence), and every
+// Several sequences decoded in lock-step share one launch: the grid is (split, cache head part, sequence), and every
 // (sequence, head) divides its own rows among the splits a one-sequence launch would use.
-// HBM-bound: reads 2*Hq*T*D*2 bytes per sequence; each row is fetched with 128-bit loads, D/8 lanes per row.
+// HBM-bound: reads 2*T*D*elem bytes per cache head and sequence; each row is fetched with 128-bit loads, D/8 lanes per row
+// for 16-bit rows, D/16 for E4M3 rows (the per-row K scale multiplies the finished dot product and the V scale is folded
+// into the softmax weight, so neither costs a multiply per element).
 #include "pkv_common.cuh"
 #include "pkv_internal.h"
+#include "pkv_rows.cuh"
 
 namespace pkv {
 namespace {
@@ -18,255 +21,191 @@ constexpr int kDecodeThreads = 256;
 constexpr int kDecodeWarps = kDecodeThreads / 32;
 constexpr int kDecodeUnroll = 4;
 
-__host__ __device__ inline int64_t splits_for(int64_t Hq, int64_t T, int64_t num_sms) { return decode_splits_for(Hq, T, num_sms); }
-
 struct DecodeParams {
     const uint16_t *q, *k_new, *v_new;   // q [num_seqs][Hq][D], k_new / v_new [num_seqs][Hkv][D]
-    uint16_t *k_cache, *v_cache, *out;   // caches at + s*cache_sb + h*cache_sh; out [num_seqs][Hq][D]
-    int64_t cache_sh, cache_sb, T, chunk, max_rows;
+    void *k_cache, *v_cache;             // cache head c of sequence s at + s*cache_sb + c*cache_sh elements
+    uint16_t* out;                       // [num_seqs][Hq][D]
+    float *k_scale, *v_scale;            // E4M3 rows: at + s*scale_sb + c*scale_sh
+    int64_t cache_sh, cache_sb, scale_sh, scale_sb, T, max_rows;
     int G, nsplit, num_sms;
-    int Hq;     // query heads per sequence (the grouped kernel's split rule; the per-head kernel reads gridDim.y)
+    int Hq;     // query heads per sequence: the split rule
     float scale;
     float* ws;  // [num_seqs*Hq][nsplit][2 + D] partial (m, l, acc) when nsplit > 1
-    const int32_t* step_dev;  // DEVLEN kernels: rows = T + *step_dev (graph-replayable decode; the grid is sized for the maximum)
-    const int32_t* rows;      // DEVLEN kernels: + rows[s*Hq + h] (rows of each sequence and head: joined prompts, AdaKV / HeadKV)
+    const int32_t* step_dev;  // rows = T + *step_dev (graph-replayable decode; the grid is sized for the maximum)
+    const int32_t* rows;      // + rows[s*(cache heads) + c] (rows of each sequence and cache head: joined prompts, AdaKV / HeadKV)
 };
 
+// Row formats. A lane holds kElems elements of a row (one 128-bit load). score() and weight() give the softmax input of a
+// row and the factor of its V elements, with the roundings the fp32 online softmax below is defined by.
 template <typename T>
-__device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
-    const uint32_t u[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        f[2 * e] = DT<T>::to_f32(uint16_t(u[e] & 0xffffu));
-        f[2 * e + 1] = DT<T>::to_f32(uint16_t(u[e] >> 16));
-    }
-}
+struct Rows16 {   // bf16 / fp16 rows, as the eviction wrote them
+    using Elem = uint16_t;
+    static constexpr int kElems = 8;
+    static constexpr bool kE4M3 = false;
+    static __device__ __forceinline__ void widen(const uint4& v, float (&f)[kElems]) { unpack8<T>(v, f); }
+    static __device__ __forceinline__ float score(float dot, float /*k_scale*/, float scale) { return __fmul_rn(dot, scale); }
+    static __device__ __forceinline__ float weight(float pe, float /*v_scale*/) { return pe; }
+};
+struct RowsE4M3 {   // E4M3 rows with one fp32 scale per row for K and for V (pkv_rows.cuh)
+    using Elem = uint8_t;
+    static constexpr int kElems = 16;
+    static constexpr bool kE4M3 = true;
+    static __device__ __forceinline__ void widen(const uint4& v, float (&f)[kElems]) { fp8x16_to_f32(v, f); }
+    static __device__ __forceinline__ float score(float dot, float k_scale, float scale) { return __fmul_rn(__fmul_rn(dot, k_scale), scale); }
+    static __device__ __forceinline__ float weight(float pe, float v_scale) { return __fmul_rn(pe, v_scale); }
+};
 
-// DEVLEN = false: the row count is the launch parameter p.T. DEVLEN = true: p.T is the row count at step 0 and the
-// current step is read from device memory, so that ONE captured launch (CUDA graph) serves every decode step; the grid
-// is sized for the cache capacity, and the rows are divided in-kernel among the splits a host launch for the current row
-// count would use (the others stay empty), so both forms add the same terms in the same order: the same output bits.
-// The split count comes from the per-sequence head count gridDim.y, so a sequence gets the same bits in a batch as alone.
-// A row count outside [1, max_rows] (the capacity the launch was checked against) is treated as 0: nothing is read or
-// written but the output, which becomes NaN.
-template <typename T, int D, bool DEVLEN>
+// One CTA per (split, cache head part, sequence) attends GH query heads over the rows of its split, loading each row once.
+// GH = 1: a cache per query head (h = blockIdx.y; the new row comes from kv head h / G). GH > 1: a GQA-shared cache per KV
+// head c, read by its G query heads, GH of them per CTA: blockIdx.y = c * (G / GH) + part, and part 0 appends the new row.
+//
+// The row count is T (+ *step_dev) (+ rows[...]), read on the device, so that ONE captured launch (CUDA graph) serves every
+// decode step; the grid is sized for the capacity, and the rows are divided in-kernel among the splits a launch for the
+// current row count would use (the others stay empty), so every launch adds the same terms in the same order: the same
+// output bits. The split count is that of Hq query heads, so a sequence gets the same bits in a batch as alone, and every
+// head of a shared cache the bits it gets from the repeat-interleaved cache. A row count outside [1, max_rows] (the capacity
+// the launch was checked against) is treated as 0: nothing is read or written but the output, which becomes NaN.
+//
+// Registers: the GH = 1 forms must stay within the ceilings of their occupancy, 80 per thread for 16-bit rows (3 CTAs per
+// SM; 74-75 now) and 128 for E4M3 rows (2 CTAs per SM; at 128 now, no headroom). ptxas -v prints the counts.
+template <typename T, int D, typename Rows, int GH>
 __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodeParams p) {
-    constexpr int LPR = D / 8;     // lanes per cached row
-    constexpr int RPW = 32 / LPR;  // rows per warp step
-    __shared__ float s_m[kDecodeWarps], s_l[kDecodeWarps];
-    __shared__ float s_acc[kDecodeWarps][D];
+    using Elem = typename Rows::Elem;
+    constexpr int E = Rows::kElems;
+    constexpr int LPR = D / E;        // lanes per cached row
+    constexpr int RPW = 32 / LPR;     // rows per warp step
+    constexpr bool kShared = GH > 1;
+    __shared__ float s_m[GH][kDecodeWarps], s_l[GH][kDecodeWarps];
+    __shared__ float s_acc[GH][kDecodeWarps][D];
+    __shared__ uint4 s_new[2][LPR];   // E4M3: the appended K and V rows and their scales, as stored
+    __shared__ float s_new_scale[2];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int split = blockIdx.x, h = blockIdx.y, g = h / p.G;
-    const int64_t sh = int64_t(blockIdx.z) * gridDim.y + h;            // (sequence, head) index
-    const int64_t sg = int64_t(blockIdx.z) * (gridDim.y / p.G) + g;    // (sequence, kv head) index
     const int sub = lane / LPR, piece = lane % LPR;
-    uint16_t* kc = p.k_cache + int64_t(blockIdx.z) * p.cache_sb + int64_t(h) * p.cache_sh;
-    uint16_t* vc = p.v_cache + int64_t(blockIdx.z) * p.cache_sb + int64_t(h) * p.cache_sh;
-    const uint16_t* k_new = p.k_new + sg * D;
-    const uint16_t* v_new = p.v_new + sg * D;
-    int64_t rows = p.T, chunk = p.chunk;
-    if constexpr (DEVLEN) {
-        if (p.step_dev) rows += int64_t(__ldg(p.step_dev));
-        if (p.rows) rows += int64_t(__ldg(p.rows + sh));
-        if (rows < 1 || rows > p.max_rows) rows = 0;
-        const int64_t ns = min(int64_t(p.nsplit), splits_for(gridDim.y, rows, p.num_sms));
-        chunk = (rows + ns - 1) / ns;
-    }
+    const int Hkv = p.Hq / p.G, parts = kShared ? p.G / GH : 1;
+    const int split = blockIdx.x, c = blockIdx.y / parts, part = blockIdx.y % parts;
+    const int64_t sc = int64_t(blockIdx.z) * (kShared ? Hkv : p.Hq) + c;                               // (sequence, cache head)
+    const int64_t sk = int64_t(blockIdx.z) * Hkv + (kShared ? c : c / p.G);                           // (sequence, kv head)
+    const int64_t sh0 = int64_t(blockIdx.z) * p.Hq + (kShared ? int64_t(c) * p.G : c) + part * GH;   // (sequence, first query head)
+    const int64_t cache_off = int64_t(blockIdx.z) * p.cache_sb + int64_t(c) * p.cache_sh;
+    const int64_t scale_off = int64_t(blockIdx.z) * p.scale_sb + int64_t(c) * p.scale_sh;
+    Elem* kc = static_cast<Elem*>(p.k_cache) + cache_off;
+    Elem* vc = static_cast<Elem*>(p.v_cache) + cache_off;
+    const uint16_t* k_new = p.k_new + sk * D;
+    const uint16_t* v_new = p.v_new + sk * D;
+    int64_t rows = p.T;
+    if (p.step_dev) rows += int64_t(__ldg(p.step_dev));
+    if (p.rows) rows += int64_t(__ldg(p.rows + sc));
+    if (rows < 1 || rows > p.max_rows) rows = 0;
+    const int64_t ns = min(int64_t(p.nsplit), decode_splits_for(p.Hq, rows, p.num_sms));
+    const int64_t chunk = (rows + ns - 1) / ns;
     const int64_t r_begin = int64_t(split) * chunk;
     const int64_t r_end = min(rows, r_begin + chunk);   // may be <= r_begin (empty split): the partial is (-inf, 0, 0)
-    const bool has_new = p.k_new != nullptr;
     const int64_t new_row = rows - 1;
+    const bool own_new = p.k_new != nullptr && new_row >= r_begin && new_row < r_end;   // uniform over the CTA
 
-    // fused append: the CTA that owns the last row stores the new token's K/V (this head's copy)
-    if (has_new && new_row >= r_begin && new_row < r_end && warp == 0 && lane < LPR) {
-        *reinterpret_cast<uint4*>(kc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(k_new + lane * 8);
-        *reinterpret_cast<uint4*>(vc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(v_new + lane * 8);
+    // fused append: the CTA that owns the last row stores the new token's K/V
+    if constexpr (Rows::kE4M3) {
+        // warp 0 quantises the new K row (lane groups 0, 2, ...) and V row (1, 3, ...); groups 0 and 1 store them, and every
+        // part keeps them in shared memory to attend the row exactly as the cache holds it
+        if (own_new && warp == 0) {
+            const int which = sub & 1;
+            float x[16];
+            load16<T>((which ? v_new : k_new) + piece * 16, x);
+            const float amax = row_amax<LPR>(x);
+            float s;
+            const uint4 qv = quantize16(x, amax, s);
+            if (sub < 2) {
+                if (part == 0) *reinterpret_cast<uint4*>((which ? vc : kc) + new_row * D + piece * 16) = qv;
+                s_new[which][piece] = qv;
+                if (piece == 0) {
+                    if (part == 0) (which ? p.v_scale : p.k_scale)[scale_off + new_row] = s;
+                    s_new_scale[which] = s;
+                }
+            }
+        }
+        __syncthreads();
+    } else {
+        if (own_new && part == 0 && warp == 0 && lane < LPR) {
+            *reinterpret_cast<uint4*>(kc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(k_new + lane * 8);
+            *reinterpret_cast<uint4*>(vc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(v_new + lane * 8);
+        }
     }
 
-    float qf[8];
-    unpack8<T>(*reinterpret_cast<const uint4*>(p.q + sh * D + piece * 8), qf);
-
-    float m = -INFINITY, l = 0.f, acc[8];
+    float qf[GH][E], m[GH], l[GH], acc[GH][E];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+    for (int i = 0; i < GH; ++i) {
+#pragma unroll
+        for (int b = 0; b < E; b += 8) unpack8<T>(*reinterpret_cast<const uint4*>(p.q + (sh0 + i) * D + piece * E + b), qf[i] + b);
+        m[i] = -INFINITY;
+        l[i] = 0.f;
+#pragma unroll
+        for (int e = 0; e < E; ++e) acc[i][e] = 0.f;
+    }
 
     // warp-uniform trip count (the shuffles below need every lane); rows are checked per lane group
     for (int64_t rb = r_begin + warp * RPW; rb < r_end; rb += int64_t(kDecodeWarps) * RPW * kDecodeUnroll) {
         uint4 kv[kDecodeUnroll], vv[kDecodeUnroll];
+        float ks[kDecodeUnroll], vs[kDecodeUnroll];   // E4M3 row scales
         bool ok[kDecodeUnroll];
 #pragma unroll
         for (int u = 0; u < kDecodeUnroll; ++u) {
             const int64_t r = rb + sub + int64_t(u) * kDecodeWarps * RPW;
             kv[u] = make_uint4(0, 0, 0, 0);
             vv[u] = make_uint4(0, 0, 0, 0);
+            ks[u] = vs[u] = 0.f;
             ok[u] = r < r_end;
             if (ok[u]) {
-                const bool is_new = has_new && r == new_row;   // read the appended row from its source
-                const uint16_t* kr = is_new ? k_new : kc + r * D;
-                const uint16_t* vr = is_new ? v_new : vc + r * D;
-                kv[u] = *reinterpret_cast<const uint4*>(kr + piece * 8);
-                vv[u] = *reinterpret_cast<const uint4*>(vr + piece * 8);
+                const bool is_new = own_new && r == new_row;   // the appended row: from its source
+                if constexpr (Rows::kE4M3) {
+                    if (is_new) {
+                        kv[u] = s_new[0][piece];
+                        vv[u] = s_new[1][piece];
+                        ks[u] = s_new_scale[0];
+                        vs[u] = s_new_scale[1];
+                    } else {
+                        kv[u] = *reinterpret_cast<const uint4*>(kc + r * D + piece * E);
+                        vv[u] = *reinterpret_cast<const uint4*>(vc + r * D + piece * E);
+                        ks[u] = p.k_scale[scale_off + r];
+                        vs[u] = p.v_scale[scale_off + r];
+                    }
+                } else {
+                    const uint16_t* kr = is_new ? k_new : kc + r * D;
+                    const uint16_t* vr = is_new ? v_new : vc + r * D;
+                    kv[u] = *reinterpret_cast<const uint4*>(kr + piece * E);
+                    vv[u] = *reinterpret_cast<const uint4*>(vr + piece * E);
+                }
             }
         }
 #pragma unroll
         for (int u = 0; u < kDecodeUnroll; ++u) {
-            float kf[8], vf[8];
-            unpack8<T>(kv[u], kf);
-            unpack8<T>(vv[u], vf);
-            float dot = 0.f;
-#pragma unroll
-            for (int e = 0; e < 8; ++e) dot = fmaf(qf[e], kf[e], dot);
-#pragma unroll
-            for (int o = 1; o < LPR; o <<= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
-            if (ok[u]) {   // uniform within the LPR-lane row group
-                const float s = dot * p.scale;
-                const float mn = fmaxf(m, s);
-                const float corr = expf(m - mn), pe = expf(s - mn);
-                l = l * corr + pe;
-#pragma unroll
-                for (int e = 0; e < 8; ++e) acc[e] = acc[e] * corr + pe * vf[e];
-                m = mn;
-            }
-        }
-    }
-
-    // merge the RPW row groups of the warp (same dims, different rows)
-#pragma unroll
-    for (int o = LPR; o < 32; o <<= 1) {
-        const float m2 = __shfl_xor_sync(0xffffffffu, m, o);
-        const float l2 = __shfl_xor_sync(0xffffffffu, l, o);
-        const float mn = fmaxf(m, m2);
-        const float c1 = (mn == -INFINITY) ? 0.f : expf(m - mn), c2 = (mn == -INFINITY) ? 0.f : expf(m2 - mn);
-        l = l * c1 + l2 * c2;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            const float a2 = __shfl_xor_sync(0xffffffffu, acc[e], o);
-            acc[e] = acc[e] * c1 + a2 * c2;
-        }
-        m = mn;
-    }
-    if (sub == 0) {
-        if (piece == 0) { s_m[warp] = m; s_l[warp] = l; }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) s_acc[warp][piece * 8 + e] = acc[e];
-    }
-    __syncthreads();
-    if (tid < D) {
-        float mn = -INFINITY;
-#pragma unroll
-        for (int w = 0; w < kDecodeWarps; ++w) mn = fmaxf(mn, s_m[w]);
-        float lt = 0.f, at = 0.f;
-#pragma unroll
-        for (int w = 0; w < kDecodeWarps; ++w) {
-            const float c = (s_m[w] == -INFINITY) ? 0.f : expf(s_m[w] - mn);
-            lt += s_l[w] * c;
-            at += s_acc[w][tid] * c;
-        }
-        if (p.nsplit == 1) {
-            p.out[sh * D + tid] = DT<T>::from_f32(at / lt);
-        } else {
-            float* w = p.ws + (sh * p.nsplit + split) * (2 + D);
-            if (tid == 0) { w[0] = mn; w[1] = lt; }
-            w[2 + tid] = at;
-        }
-    }
-}
-
-// decode_kernel<T, D, true> over a GQA-shared cache ([num_seqs][Hkv][capacity][D], rows[s*Hkv + j]): the CTA of (split, KV
-// head j, sequence) loads every row of its split once and runs, for each of the GH query heads h0..h0+GH-1 of the group, the
-// arithmetic decode_kernel runs for that head on the repeat-interleaved cache - the same rows per warp and lane group, the same
-// dot-product and online-softmax order, the same merges - so each head's output is bit-identical to it. The split count is
-// the per-query-head kernel's for Hq heads, and the partials are written per query head for decode_combine_kernel.
-// GH < G: the group is covered by G / GH CTAs (blockIdx.y = j * (G / GH) + part); part 0 appends the new row.
-template <typename T, int D, int GH>
-__global__ void __launch_bounds__(kDecodeThreads) decode_gqa_kernel(const DecodeParams p) {
-    constexpr int LPR = D / 8;
-    constexpr int RPW = 32 / LPR;
-    __shared__ float s_m[GH][kDecodeWarps], s_l[GH][kDecodeWarps];
-    __shared__ float s_acc[GH][kDecodeWarps][D];
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int parts = p.G / GH, split = blockIdx.x, j = blockIdx.y / parts, part = blockIdx.y % parts;
-    const int Hkv = p.Hq / p.G;
-    const int64_t sg = int64_t(blockIdx.z) * Hkv + j;                          // (sequence, kv head) index
-    const int64_t sh0 = int64_t(blockIdx.z) * p.Hq + int64_t(j) * p.G + part * GH;   // (sequence, first query head) index
-    const int sub = lane / LPR, piece = lane % LPR;
-    uint16_t* kc = p.k_cache + int64_t(blockIdx.z) * p.cache_sb + int64_t(j) * p.cache_sh;
-    uint16_t* vc = p.v_cache + int64_t(blockIdx.z) * p.cache_sb + int64_t(j) * p.cache_sh;
-    const uint16_t* k_new = p.k_new + sg * D;
-    const uint16_t* v_new = p.v_new + sg * D;
-    int64_t rows = p.T;
-    if (p.step_dev) rows += int64_t(__ldg(p.step_dev));
-    if (p.rows) rows += int64_t(__ldg(p.rows + sg));
-    if (rows < 1 || rows > p.max_rows) rows = 0;
-    const int64_t ns = min(int64_t(p.nsplit), splits_for(p.Hq, rows, p.num_sms));
-    const int64_t chunk = (rows + ns - 1) / ns;
-    const int64_t r_begin = int64_t(split) * chunk;
-    const int64_t r_end = min(rows, r_begin + chunk);
-    const bool has_new = p.k_new != nullptr;
-    const int64_t new_row = rows - 1;
-
-    // fused append, once per KV head
-    if (has_new && part == 0 && new_row >= r_begin && new_row < r_end && warp == 0 && lane < LPR) {
-        *reinterpret_cast<uint4*>(kc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(k_new + lane * 8);
-        *reinterpret_cast<uint4*>(vc + new_row * D + lane * 8) = *reinterpret_cast<const uint4*>(v_new + lane * 8);
-    }
-
-    float qf[GH][8], m[GH], l[GH], acc[GH][8];
-#pragma unroll
-    for (int i = 0; i < GH; ++i) {
-        unpack8<T>(*reinterpret_cast<const uint4*>(p.q + (sh0 + i) * D + piece * 8), qf[i]);
-        m[i] = -INFINITY;
-        l[i] = 0.f;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) acc[i][e] = 0.f;
-    }
-
-    for (int64_t rb = r_begin + warp * RPW; rb < r_end; rb += int64_t(kDecodeWarps) * RPW * kDecodeUnroll) {
-        uint4 kv[kDecodeUnroll], vv[kDecodeUnroll];
-        bool ok[kDecodeUnroll];
-#pragma unroll
-        for (int u = 0; u < kDecodeUnroll; ++u) {
-            const int64_t r = rb + sub + int64_t(u) * kDecodeWarps * RPW;
-            kv[u] = make_uint4(0, 0, 0, 0);
-            vv[u] = make_uint4(0, 0, 0, 0);
-            ok[u] = r < r_end;
-            if (ok[u]) {
-                const bool is_new = has_new && r == new_row;
-                const uint16_t* kr = is_new ? k_new : kc + r * D;
-                const uint16_t* vr = is_new ? v_new : vc + r * D;
-                kv[u] = *reinterpret_cast<const uint4*>(kr + piece * 8);
-                vv[u] = *reinterpret_cast<const uint4*>(vr + piece * 8);
-            }
-        }
-#pragma unroll
-        for (int u = 0; u < kDecodeUnroll; ++u) {
-            float kf[8], vf[8];
-            unpack8<T>(kv[u], kf);
-            unpack8<T>(vv[u], vf);
+            float kf[E], vf[E];
+            Rows::widen(kv[u], kf);
+            Rows::widen(vv[u], vf);
 #pragma unroll
             for (int i = 0; i < GH; ++i) {
                 float dot = 0.f;
 #pragma unroll
-                for (int e = 0; e < 8; ++e) dot = fmaf(qf[i][e], kf[e], dot);
+                for (int e = 0; e < E; ++e) dot = fmaf(qf[i][e], kf[e], dot);
 #pragma unroll
                 for (int o = 1; o < LPR; o <<= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
-                if (ok[u]) {
-                    // Explicit roundings: the forms the compiler picks for decode_kernel (with the G heads unrolled it may
-                    // contract a*b + c*d around the other product, or fuse dot * scale into s - mn), so the bits match it.
-                    const float s = __fmul_rn(dot, p.scale);
+                if (ok[u]) {   // uniform within the LPR-lane row group
+                    // Explicit roundings, so that the compiler cannot contract differently for different GH (a*b + c*d around
+                    // either product, or dot * scale into s - mn): every head gets the bits of its per-query-head cache.
+                    const float s = Rows::score(dot, ks[u], p.scale);
                     const float mn = fmaxf(m[i], s);
                     const float corr = expf(m[i] - mn), pe = expf(s - mn);
                     l[i] = __fmaf_rn(l[i], corr, pe);
+                    const float pv = Rows::weight(pe, vs[u]);
 #pragma unroll
-                    for (int e = 0; e < 8; ++e) acc[i][e] = __fmaf_rn(acc[i][e], corr, __fmul_rn(pe, vf[e]));
+                    for (int e = 0; e < E; ++e) acc[i][e] = __fmaf_rn(acc[i][e], corr, __fmul_rn(pv, vf[e]));
                     m[i] = mn;
                 }
             }
         }
     }
 
+    // merge the RPW row groups of each warp (same dims, different rows), then the warps
 #pragma unroll
     for (int i = 0; i < GH; ++i) {
 #pragma unroll
@@ -277,7 +216,7 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_gqa_kernel(const Decode
             const float c1 = (mn == -INFINITY) ? 0.f : expf(m[i] - mn), c2 = (mn == -INFINITY) ? 0.f : expf(m2 - mn);
             l[i] = __fmaf_rn(l[i], c1, __fmul_rn(l2, c2));
 #pragma unroll
-            for (int e = 0; e < 8; ++e) {
+            for (int e = 0; e < E; ++e) {
                 const float a2 = __shfl_xor_sync(0xffffffffu, acc[i][e], o);
                 acc[i][e] = __fmaf_rn(acc[i][e], c1, __fmul_rn(a2, c2));
             }
@@ -286,7 +225,7 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_gqa_kernel(const Decode
         if (sub == 0) {
             if (piece == 0) { s_m[i][warp] = m[i]; s_l[i][warp] = l[i]; }
 #pragma unroll
-            for (int e = 0; e < 8; ++e) s_acc[i][warp][piece * 8 + e] = acc[i][e];
+            for (int e = 0; e < E; ++e) s_acc[i][warp][piece * E + e] = acc[i][e];
         }
     }
     __syncthreads();
@@ -330,14 +269,14 @@ __global__ void decode_combine_kernel(const DecodeParams p) {   // one CTA per (
 }
 
 template <int D>
-__global__ void append_kernel(const DecodeParams p) {  // (host-length only; the graph path appends inside decode_kernel)
+__global__ void append_kernel(const DecodeParams p) {  // (pkv_cache_append; decode_kernel appends the new row itself)
     constexpr int LPR = D / 8;
     const int h = blockIdx.x, g = h / p.G, lane = threadIdx.x;
     if (lane >= 2 * LPR) return;
     const bool is_v = lane >= LPR;
     const int piece = lane % LPR;
     const uint16_t* src = (is_v ? p.v_new : p.k_new) + int64_t(g) * D + piece * 8;
-    uint16_t* dst = (is_v ? p.v_cache : p.k_cache) + int64_t(h) * p.cache_sh + (p.T - 1) * D + piece * 8;
+    uint16_t* dst = static_cast<uint16_t*>(is_v ? p.v_cache : p.k_cache) + int64_t(h) * p.cache_sh + (p.T - 1) * D + piece * 8;
     *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(src);
 }
 
@@ -345,10 +284,11 @@ DecodeParams make_params(const DecodeArgs& a) {
     DecodeParams p;
     p.q = a.q; p.k_new = a.k_new; p.v_new = a.v_new;
     p.k_cache = a.k_cache; p.v_cache = a.v_cache; p.out = a.out;
-    p.cache_sh = a.cache_sh; p.cache_sb = a.cache_sb; p.T = a.T; p.max_rows = a.max_rows;
+    p.k_scale = a.k_scale; p.v_scale = a.v_scale;
+    p.cache_sh = a.cache_sh; p.cache_sb = a.cache_sb; p.scale_sh = a.scale_sh; p.scale_sb = a.scale_sb;
+    p.T = a.T; p.max_rows = a.max_rows;
     p.G = a.G; p.nsplit = a.nsplit; p.num_sms = a.num_sms;
     p.Hq = a.Hq;
-    p.chunk = (a.T + a.nsplit - 1) / a.nsplit;
     p.scale = a.scale;
     p.ws = a.ws;
     p.step_dev = a.step_dev;
@@ -356,12 +296,21 @@ DecodeParams make_params(const DecodeArgs& a) {
     return p;
 }
 
-template <typename T, int D>
+template <typename T, int D, typename Rows>
 cudaError_t launch_decode_t(const DecodeArgs& a, cudaStream_t st) {
     const DecodeParams p = make_params(a);
-    const dim3 grid(unsigned(a.nsplit), unsigned(a.Hq), unsigned(a.num_seqs));
-    if (a.devlen) decode_kernel<T, D, true><<<grid, kDecodeThreads, 0, st>>>(p);
-    else decode_kernel<T, D, false><<<grid, kDecodeThreads, 0, st>>>(p);
+    // query heads per CTA: 1 on a cache per query head; on a shared cache the whole group, for E4M3 at most 4 (the registers
+    // of eight heads do not fit)
+    const int GH = a.heads_per_cache == 1 ? 1 : Rows::kE4M3 ? min(a.G, 4) : a.G;
+    const dim3 grid(unsigned(a.nsplit), unsigned(a.Hq / GH), unsigned(a.num_seqs));
+    if (GH == 1) decode_kernel<T, D, Rows, 1><<<grid, kDecodeThreads, 0, st>>>(p);
+    else if (GH == 2) decode_kernel<T, D, Rows, 2><<<grid, kDecodeThreads, 0, st>>>(p);
+    else if (GH == 4) decode_kernel<T, D, Rows, 4><<<grid, kDecodeThreads, 0, st>>>(p);
+    else if (!Rows::kE4M3 && GH == 8) {
+        if constexpr (!Rows::kE4M3) decode_kernel<T, D, Rows, 8><<<grid, kDecodeThreads, 0, st>>>(p);
+    } else {
+        return cudaErrorInvalidValue;   // no instantiation for this group size
+    }
     count_launch();
     if (a.nsplit > 1) {
         decode_combine_kernel<T, D><<<unsigned(int64_t(a.num_seqs) * a.Hq), D, 0, st>>>(p);
@@ -371,44 +320,17 @@ cudaError_t launch_decode_t(const DecodeArgs& a, cudaStream_t st) {
 }
 
 template <typename T, int D>
-cudaError_t launch_decode_gqa_t(const DecodeArgs& a, cudaStream_t st) {
-    const DecodeParams p = make_params(a);
-    const dim3 grid(unsigned(a.nsplit), unsigned(a.Hkv), unsigned(a.num_seqs));
-    if (a.G == 2) decode_gqa_kernel<T, D, 2><<<grid, kDecodeThreads, 0, st>>>(p);
-    else if (a.G == 4) decode_gqa_kernel<T, D, 4><<<grid, kDecodeThreads, 0, st>>>(p);
-    else decode_gqa_kernel<T, D, 8><<<grid, kDecodeThreads, 0, st>>>(p);
-    count_launch();
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess || a.nsplit == 1) return e;
-    return launch_decode_combine(a, st);
+cudaError_t launch_decode_rows(const DecodeArgs& a, cudaStream_t st) {
+    return a.k_scale ? launch_decode_t<T, D, RowsE4M3>(a, st) : launch_decode_t<T, D, Rows16<T>>(a, st);
 }
 
 }  // namespace
 
-cudaError_t launch_decode_gqa(const DecodeArgs& a, cudaStream_t st) {
-    if (a.dtype == PKV_BF16) return a.D == 128 ? launch_decode_gqa_t<__nv_bfloat16, 128>(a, st) : launch_decode_gqa_t<__nv_bfloat16, 64>(a, st);
-    return a.D == 128 ? launch_decode_gqa_t<__half, 128>(a, st) : launch_decode_gqa_t<__half, 64>(a, st);
-}
-
-int decode_num_splits(int Hq, int64_t T, int num_sms) { return int(splits_for(Hq, T, num_sms)); }
+int decode_num_splits(int Hq, int64_t T, int num_sms) { return int(decode_splits_for(Hq, T, num_sms)); }
 
 cudaError_t launch_decode(const DecodeArgs& a, cudaStream_t st) {
-    if (a.dtype == PKV_BF16) return a.D == 128 ? launch_decode_t<__nv_bfloat16, 128>(a, st) : launch_decode_t<__nv_bfloat16, 64>(a, st);
-    return a.D == 128 ? launch_decode_t<__half, 128>(a, st) : launch_decode_t<__half, 64>(a, st);
-}
-
-cudaError_t launch_decode_combine(const DecodeArgs& a, cudaStream_t st) {
-    const DecodeParams p = make_params(a);
-    const unsigned grid = unsigned(int64_t(a.num_seqs) * a.Hq);
-    if (a.dtype == PKV_BF16) {
-        if (a.D == 128) decode_combine_kernel<__nv_bfloat16, 128><<<grid, 128, 0, st>>>(p);
-        else decode_combine_kernel<__nv_bfloat16, 64><<<grid, 64, 0, st>>>(p);
-    } else {
-        if (a.D == 128) decode_combine_kernel<__half, 128><<<grid, 128, 0, st>>>(p);
-        else decode_combine_kernel<__half, 64><<<grid, 64, 0, st>>>(p);
-    }
-    count_launch();
-    return cudaGetLastError();
+    if (a.dtype == PKV_BF16) return a.D == 128 ? launch_decode_rows<__nv_bfloat16, 128>(a, st) : launch_decode_rows<__nv_bfloat16, 64>(a, st);
+    return a.D == 128 ? launch_decode_rows<__half, 128>(a, st) : launch_decode_rows<__half, 64>(a, st);
 }
 
 cudaError_t launch_append(const DecodeArgs& a, cudaStream_t st) {

@@ -105,28 +105,30 @@ int fused_tiles_per_cta(const EvictArgs& a);   // largest number of 128-token ti
 // kernel follows as its own launch. false: stages 1-4, everything in one launch.
 cudaError_t launch_evict_fused(const EvictArgs& a, bool pool_only, cudaStream_t st);
 
+// One decode step over a compacted cache of any form. The row count of each (sequence, cache head) is read on the device:
+// T (+ *step_dev) (+ rows[s*(cache heads) + c]); counts outside [1, max_rows] are not attended (NaN output, nothing written).
 struct DecodeArgs {
     int dtype, Hq, Hkv, G, D;
-    int64_t T;  // valid rows after append
+    int64_t T;  // valid rows after append (at step 0)
     const uint16_t *q, *k_new, *v_new;
-    uint16_t *k_cache, *v_cache, *out;
+    void *k_cache, *v_cache;
+    uint16_t* out;
     int64_t cache_sh;
     int64_t cache_sb = 0;   // elements between the caches of consecutive sequences
     int num_seqs = 1;
-    int64_t max_rows = 0;   // devlen: row counts outside [1, max_rows] are not attended (NaN output, nothing written)
-    bool devlen = false;    // row counts are read on the device (graph-replayable form): T (+ *step_dev) (+ rows[s*Hq + h])
+    int heads_per_cache = 1;   // 1: a cache per query head; G: a GQA-shared cache per KV head ([num_seqs][Hkv][capacity][D])
+    int64_t max_rows = 0;
     float* ws;
     float scale;
     int nsplit;
     int num_sms;
     const int32_t* step_dev = nullptr;  // device step counter added to T inside the kernel
-    const int32_t* rows = nullptr;      // [num_seqs*Hq] per (sequence, head) row counts added to T inside the kernel
-    // FP8 cache (launch_decode_fp8): k_cache / v_cache hold E4M3 bytes, one fp32 scale per (sequence, head, row)
+    const int32_t* rows = nullptr;      // [num_seqs * cache heads] row counts added to T inside the kernel
+    // E4M3 cache when k_scale is set: k_cache / v_cache hold E4M3 bytes, one fp32 scale per (sequence, cache head, row)
     float *k_scale = nullptr, *v_scale = nullptr;
     int64_t scale_sh = 0, scale_sb = 0;   // floats between the scales of consecutive heads / sequences
-    bool gqa = false;   // launch_decode_fp8: the cache is GQA-shared (launch_decode_gqa_fp8)
 };
-// split count for T rows (decode_num_splits); shared by the host launch and the device-length decode kernels
+// split count for T rows (decode_num_splits); shared by the launch and the decode kernel
 __host__ __device__ inline int64_t decode_splits_for(int64_t Hq, int64_t T, int64_t num_sms) {
     int64_t ns = (T + 255) / 256;                       // ~256 rows (32 per warp) per CTA
     const int64_t cap = (num_sms * 4 + Hq - 1) / Hq;    // at most ~4 CTAs per SM in flight
@@ -136,16 +138,11 @@ __host__ __device__ inline int64_t decode_splits_for(int64_t Hq, int64_t T, int6
     return ns;
 }
 int decode_num_splits(int Hq, int64_t T, int num_sms);
+// decode_kernel for the cache form (16-bit or E4M3 rows, per query head or GQA-shared), plus the merge of the split partials
 cudaError_t launch_decode(const DecodeArgs& a, cudaStream_t st);
-cudaError_t launch_decode_combine(const DecodeArgs& a, cudaStream_t st);   // merges the split partials in a.ws into a.out
 cudaError_t launch_append(const DecodeArgs& a, cudaStream_t st);
-// GQA-shared caches ([num_seqs][Hkv][capacity][D], rows[s*Hkv + j]): one CTA per (split, KV head, sequence) computes the G query
-// heads of the group; device-length form only. The split rule and the partials stay those of Hq query heads.
-cudaError_t launch_decode_gqa(const DecodeArgs& a, cudaStream_t st);
 
-// ---- FP8 (E4M3) compacted cache (pkv_fp8.cu) ----
-cudaError_t launch_decode_fp8(const DecodeArgs& a, cudaStream_t st);   // device-length form only (a.devlen)
-cudaError_t launch_decode_gqa_fp8(const DecodeArgs& a, cudaStream_t st);   // GQA-shared FP8 caches (launch_decode_gqa)
+// ---- conversion of the compacted cache to FP8 (E4M3) rows (pkv_fp8.cu) ----
 struct QuantLayer {
     const uint16_t* src[2];   // K, V: 16-bit [num_seqs][H][src_cap][D]
     uint8_t* dst[2];          // K, V: E4M3 [num_seqs][H][dst_cap][D]
