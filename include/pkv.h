@@ -312,6 +312,38 @@ int pkv_decode_attn_batch_gqa(const pkv_decode_desc* d, int32_t num_seqs, int64_
 int pkv_decode_attn_batch_gqa_fp8(const pkv_decode_desc* d, int32_t num_seqs, int64_t cache_stride_b, const int32_t* rows,
                                   const int32_t* step_dev, int64_t max_length, float* k_scale, float* v_scale,
                                   int64_t scale_stride_h, int64_t scale_stride_b, void* stream);
+/* The decode step with a decode window: each (sequence, cache head) keeps its P prompt rows plus a ring of its last
+ * `window` = R appended rows, so generation of any length needs P + R rows. Any cache form: a cache per query head or a
+ * GQA-shared one (`gqa_shared`), 16-bit rows or E4M3 rows (`k_scale` / `v_scale` non-NULL, with the layout, quantisation
+ * and strides of pkv_decode_attn_batch_fp8). The logical row count n = d->length (+ *step_dev) (+ rows[s*H + c]) is that
+ * of pkv_decode_attn_batch / _gqa / _fp8 (H = num_q_heads, or num_kv_heads when gqa_shared), and P = prompt_rows[s*H + c]
+ * (DEVICE int32). While n <= P + R the step is exactly the unwindowed one: it stores the new row at n - 1 and attends
+ * rows [0, n). Once n > P + R, the j-th appended row (j = n - 1 - P) is stored at P + j mod R, replacing the oldest, and
+ * rows [0, P + R) are attended, in physical order, the new row as stored; positions are those the caller rotated K with.
+ * Every output, appended row and scale is then bit-identical to pkv_decode_attn_batch / _gqa / _fp8 / _gqa_fp8 run
+ * without k_new on the same buffer with the new row already at its ring slot and P + min(n - P, R) rows. A count n < 1,
+ * P < 0 or an attended count above max_length reads and writes no row; its output is NaN. The caller keeps max_length
+ * >= P + R for every (sequence, cache head) whose ring fills (it cannot be checked on the host for device P), as it keeps
+ * the counts of `rows` within max_length. Graph-replayable like pkv_decode_attn_batch: n and P are read on the device.
+ * Workspace: pkv_decode_workspace_bytes with num_q_heads = num_seqs*num_q_heads. PKV_ERR_INVALID_ARG, in addition to the
+ * errors of the entry point of the same cache form: w NULL or w->struct_bytes != sizeof(pkv_decode_window), window < 1,
+ * prompt_rows NULL or not 4-byte aligned. */
+typedef struct pkv_decode_window {
+    uint32_t struct_bytes;
+    int32_t num_seqs;
+    int64_t cache_stride_b;     /* elements (E4M3: bytes) between the caches of consecutive sequences */
+    int32_t gqa_shared;         /* 0: a cache per query head; 1: one per KV head (group in {2, 4, 8}) */
+    int32_t reserved;
+    const int32_t* rows;        /* optional DEVICE int32 [num_seqs*H], as pkv_decode_attn_batch */
+    const int32_t* prompt_rows; /* DEVICE int32 [num_seqs*H]: P of each (sequence, cache head) */
+    const int32_t* step_dev;    /* optional DEVICE int32 step counter */
+    int64_t max_length;         /* the rows the launch is sized for: cache_stride_h >= max_length*head_dim */
+    float* k_scale;             /* E4M3 rows: fp32 row scales [num_seqs, H, capacity]; NULL for 16-bit rows */
+    float* v_scale;
+    int64_t scale_stride_h, scale_stride_b;
+    int64_t window;             /* R >= 1 */
+} pkv_decode_window;
+int pkv_decode_attn_window(const pkv_decode_desc* d, const pkv_decode_window* w, void* stream);
 /* Conversion of the compacted 16-bit caches of num_layers layers (one prompt, or one equal-length batch of num_seqs
  * sequences) to the FP8 format above, in one launch per 32 layers; the per-layer tables travel as kernel parameters.
  * Layer l: src[2l] / src[2l+1] = K / V, 16-bit contiguous [num_seqs, num_heads, src_capacity[l], head_dim]; dst[2l] /

@@ -22,7 +22,7 @@ EXPORTS = [
     "pkv_ragged_place_window", "pkv_decode_attn_ragged", "pkv_evict_single_launch", "pkv_stage_scan_pool",
     "pkv_evict_prefill_batch", "pkv_evict_batch_supported", "pkv_stage_batch", "pkv_decode_attn_batch",
     "pkv_decode_attn_batch_fp8", "pkv_cache_quantize_fp8", "pkv_decode_attn_batch_gqa", "pkv_decode_attn_batch_gqa_fp8",
-    "pkv_evict_pooled_kv_offset", "pkv_cache_install", "pkv_sample_tokens",
+    "pkv_evict_pooled_kv_offset", "pkv_cache_install", "pkv_sample_tokens", "pkv_decode_attn_window",
 ]
 FLAG_GQA_SHARED = 128          # pkv_evict_desc.flags: one compacted cache per KV head
 
@@ -58,6 +58,16 @@ class DecodeDesc(C.Structure):
         ("k_cache", C.c_void_p), ("v_cache", C.c_void_p), ("cache_stride_h", C.c_int64),
         ("out", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_uint64),
         ("softmax_scale", C.c_float), ("reserved", C.c_uint32),
+    ]
+
+
+class DecodeWindow(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("num_seqs", C.c_int32), ("cache_stride_b", C.c_int64),
+        ("gqa_shared", C.c_int32), ("reserved", C.c_int32),
+        ("rows", C.c_void_p), ("prompt_rows", C.c_void_p), ("step_dev", C.c_void_p), ("max_length", C.c_int64),
+        ("k_scale", C.c_void_p), ("v_scale", C.c_void_p), ("scale_stride_h", C.c_int64), ("scale_stride_b", C.c_int64),
+        ("window", C.c_int64),
     ]
 
 
@@ -159,6 +169,8 @@ def lib() -> C.CDLL:
     L.pkv_decode_attn_batch_gqa.restype = i32
     L.pkv_decode_attn_batch_gqa_fp8.argtypes = [C.POINTER(DecodeDesc), C.c_int32, i64, p, p, i64, p, p, i64, i64, p]
     L.pkv_decode_attn_batch_gqa_fp8.restype = i32
+    L.pkv_decode_attn_window.argtypes = [C.POINTER(DecodeDesc), C.POINTER(DecodeWindow), p]
+    L.pkv_decode_attn_window.restype = i32
     # tables: src / dst / scales [2*layers] pointers, capacities and rows [layers] int64, rows_dev [layers] pointers or NULL
     L.pkv_cache_quantize_fp8.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p, p, p, p, p, p, p, p]
     L.pkv_cache_quantize_fp8.restype = i32

@@ -22,8 +22,8 @@ from typing import Callable, Optional
 import torch
 from transformers.modeling_utils import ALL_ATTENTION_FUNCTIONS
 
-from .cache import (PkvBatchCacheLayer, PkvCacheLayer, PkvRaggedCacheLayer, gqa_shared, install_layer, kv_cache_dtype,
-                    layer_is_empty, quantize_caches_fp8)
+from .cache import (PkvBatchCacheLayer, PkvCacheLayer, PkvRaggedCacheLayer, decode_window, gqa_shared, install_layer,
+                    kv_cache_dtype, layer_is_empty, quantize_caches_fp8)
 from .kv_cluster import INIT_BY_METHOD, flush_pending
 
 DEFAULT_DECODE_RESERVE = 256   # rows of head-room behind the compacted prompt (grows by doubling)
@@ -111,6 +111,9 @@ def make_forward(method: str, modeling, original_forward):
                                                          attention_mask, **kwargs)
             cluster.inputs_ready = True      # the launch in front of the eviction is the dense attention: it only reads q / k / v
             reserve = int(getattr(self.config, "pkv_decode_reserve", DEFAULT_DECODE_RESERVE))
+            window = decode_window(self.config)
+            if window is not None:       # knob pkv_decode_window: at most R decoded rows behind the prompt
+                reserve = min(reserve, window)
             group = num_q_heads // key_states.shape[1] if gqa_shared(self.config) else 1
             if group > 1 and getattr(cluster, "ragged", False):
                 raise NotImplementedError(f"pkv_gqa_shared: {method} sets a budget per QUERY head, which one cache per KV head "
@@ -120,7 +123,11 @@ def make_forward(method: str, modeling, original_forward):
                 if bsz != 1:
                     raise NotImplementedError("AdaKV / HeadKV are batch size 1 (pyramidkv_utils.py:723)")
                 k_buf, v_buf, head_rows = cluster.evict_ragged(query_states[0], key_states[0], value_states[0], reserve=reserve)
-                install_layer(past_key_values, self.layer_idx, PkvRaggedCacheLayer(k_buf[None], v_buf[None], head_rows, seen_tokens=q_len))
+                if window is not None:   # the per-(sequence, head) row-count form carries the window
+                    layer = PkvBatchCacheLayer(k_buf[None], v_buf[None], [[int(r) for r in head_rows]], [q_len], window=window)
+                else:
+                    layer = PkvRaggedCacheLayer(k_buf[None], v_buf[None], head_rows, seen_tokens=q_len)
+                install_layer(past_key_values, self.layer_idx, layer)
                 _maybe_quantize(self, past_key_values, cluster)
                 attn_output = attn_output.reshape(*input_shape, -1).contiguous()
                 return self.o_proj(attn_output), attn_weights
@@ -142,9 +149,10 @@ def make_forward(method: str, modeling, original_forward):
                 k_buf, v_buf = bufs[0][0][None], bufs[0][1][None]
             else:
                 k_buf, v_buf = torch.stack([t[0] for t in bufs]), torch.stack([t[1] for t in bufs])
-            if group > 1:
-                # knob pkv_gqa_shared: one cache per KV head, held in the per-(sequence, head) row-count form
-                layer = PkvBatchCacheLayer(k_buf, v_buf, [[rows] * k_buf.shape[1]] * bsz, [q_len] * bsz, group=group)
+            if group > 1 or window is not None:
+                # knob pkv_gqa_shared: one cache per KV head; knob pkv_decode_window: a ring of decoded rows. Both are held in
+                # the per-(sequence, head) row-count form
+                layer = PkvBatchCacheLayer(k_buf, v_buf, [[rows] * k_buf.shape[1]] * bsz, [q_len] * bsz, group=group, window=window)
             else:
                 layer = PkvCacheLayer(k_buf, v_buf, rows, seen_tokens=q_len)
             install_layer(past_key_values, self.layer_idx, layer)

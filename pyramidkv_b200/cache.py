@@ -27,6 +27,7 @@ class PkvCacheLayer(DynamicLayer):
 
     is_sliding = False
     group = 1                        # query heads per cache head (> 1: a GQA-shared cache, `PkvBatchCacheLayer`)
+    window = None                    # decode window R (knob `pkv_decode_window`; `PkvBatchCacheLayer` only)
     _BUFFERS = ("k_buf", "v_buf")    # the [B, H, capacity, ...] tensors a resize or a join copies
 
     def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, length: int, seen_tokens: int):
@@ -218,35 +219,68 @@ class PkvBatchCacheLayer(PkvCacheLayer):
 
     `group` G > 1: a GQA-shared cache (knob `pkv_gqa_shared`): one cache per KV head, [B, Hkv, capacity, D], read once for
     the G query heads of its group (`pkv_decode_attn_batch_gqa`); `rows_host[b][j]` counts KV head j's rows. G = 1 (the
-    default) is the per-query-head cache."""
+    default) is the per-query-head cache.
+
+    `window` R (knob `pkv_decode_window`): (sequence b, head h) keeps its `prompt_rows_host[b][h]` = P prompt rows and a ring
+    of its last R appended rows, the j-th at row P + j mod R (`pkv_decode_attn_window`). `generated[b]` counts the rows
+    sequence b appended; `rows_host[b][h]` = P + min(generated[b], R) are the rows the buffers hold, in ring order (not
+    token order) past P, while the device `rows` hold the logical counts P + generated[b] the kernel derives the ring slot
+    from. `prompt_rows` is the device copy of P (int32 [B*H]). None: no window."""
 
     rows_host = seq_seen = None    # held per sequence here (set in __init__), not derived from `length` as in the base class
 
-    def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, rows_host, seq_seen, group: int = 1):
+    def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, rows_host, seq_seen, group: int = 1, window: Optional[int] = None,
+                 prompt_rows=None, generated=None):
         self.group = int(group)
         self.rows_host = [[int(r) for r in row] for row in rows_host]
         self.seq_seen = [int(s) for s in seq_seen]
         assert len(self.rows_host) == len(self.seq_seen) == k_buf.shape[0] and all(len(r) == k_buf.shape[1] for r in self.rows_host)
+        self.window = None if window is None else int(window)
+        if self.window is not None:
+            # a cache that enters the window with rows of its own (the prefill's, or a joined cache's) counts them as its prompt
+            self.prompt_rows_host = [list(r) for r in (prompt_rows if prompt_rows is not None else self.rows_host)]
+            self.generated = [int(g) for g in generated] if generated is not None else [0] * len(self.rows_host)
+            self.prompt_rows = self._device_counts(self.prompt_rows_host, k_buf.device)
         self.rows = self._device_rows(k_buf.device)
         super().__init__(k_buf, v_buf, max(max(r) for r in self.rows_host), max(self.seq_seen))
 
     @property
     def rows_dev(self) -> Optional[torch.Tensor]:
+        if self.window is not None:      # the rows the buffers hold (the device `rows` are the logical counts)
+            return self._device_counts(self.rows_host, self.device)
         return None if all(r == self.length for row in self.rows_host for r in row) else self.rows
 
+    @staticmethod
+    def _device_counts(rows, device) -> torch.Tensor:
+        return torch.tensor([r for row in rows for r in row], dtype=torch.int32, device=device)
+
     def _device_rows(self, device) -> torch.Tensor:
-        return torch.tensor([r for row in self.rows_host for r in row], dtype=torch.int32, device=device)
+        if self.window is None:
+            return self._device_counts(self.rows_host, device)
+        return self._device_counts([[p + g for p in row] for row, g in zip(self.prompt_rows_host, self.generated)], device)
 
     def settle(self, appended) -> None:
-        """Sequence b appended `appended[b]` rows to every head (in place, by the decode kernel)."""
+        """Sequence b appended `appended[b]` rows to every head (in place, by the decode kernel). With a window the buffers
+        hold P + min(generated, R) of them."""
         assert len(appended) == len(self.rows_host)
         for b, n in enumerate(appended):
-            self.rows_host[b] = [r + int(n) for r in self.rows_host[b]]
+            if self.window is None:
+                self.rows_host[b] = [r + int(n) for r in self.rows_host[b]]
+            else:
+                self.generated[b] += int(n)
+                self.rows_host[b] = [p + min(self.generated[b], self.window) for p in self.prompt_rows_host[b]]
             self.seq_seen[b] += int(n)
         self.rows = self._device_rows(self.device)     # a new tensor: launches already queued keep reading the old one
         self.length = max(max(r) for r in self.rows_host)
         self.seen_tokens = max(self.seq_seen)
         self._refresh_views()
+
+    def reserve(self, extra_rows: int) -> None:
+        """Make room for `extra_rows` more appended rows; with a window never more than P + R rows per (sequence, head)."""
+        if self.window is None:
+            return super().reserve(extra_rows)
+        self.fit(max(p + min(g + int(extra_rows), self.window)
+                     for row, g in zip(self.prompt_rows_host, self.generated) for p in row))
 
     def advance(self, rows: int) -> None:
         self.settle([rows] * len(self.rows_host))
@@ -258,6 +292,10 @@ class PkvBatchCacheLayer(PkvCacheLayer):
 
     def decode(self, backend, q, k_new, v_new, static=None, softmax_scale: float = 0.0) -> torch.Tensor:
         # rows = layer.rows[b, h] + 1 (+ the step counter in the static loop); G > 1: each KV head read once for its group
+        if self.window is not None:
+            return backend.decode_attn_window(q, self.k_buf, self.v_buf, 1, k_new, v_new, self.prompt_rows, self.window,
+                                              rows=self.rows, **_devlen_args(self, static), softmax_scale=softmax_scale,
+                                              scales=self._scales(), gqa=self.group > 1)
         fn = backend.decode_attn_batch_gqa if self.group > 1 else backend.decode_attn_batch
         return fn(q, self.k_buf, self.v_buf, 1, k_new, v_new, rows=self.rows, **_devlen_args(self, static),
                   softmax_scale=softmax_scale)
@@ -289,9 +327,10 @@ class PkvBatchCacheLayer(PkvCacheLayer):
         if src is None:
             return (None, None, None, 0, None, *dst), [0] * H, 0
         if not isinstance(src, PkvCacheLayer) or _form(src) != _form(self):
-            raise ValueError(f"admit: a {type(src).__name__} (group {getattr(src, 'group', 1)}) cannot enter a "
-                             f"{type(self).__name__} of group {self.group}: FP8 and 16-bit caches, and caches of different "
-                             "groups, do not mix")
+            raise ValueError(f"admit: a {type(src).__name__} (group {getattr(src, 'group', 1)}, decode window "
+                             f"{getattr(src, 'window', None)}) cannot enter a {type(self).__name__} of group {self.group}, "
+                             f"decode window {self.window}: FP8 and 16-bit caches, and caches of different groups or decode "
+                             "windows, do not mix")
         if src.k_buf.shape[0] != 1 or src.k_buf.shape[1] != H or src.k_buf.shape[3] != D or src.dtype != self.dtype \
                 or src.device != self.device:
             raise ValueError(f"admit: the source must be one prompt of {H} heads, head_dim {D}, {self.dtype} on {self.device}; "
@@ -305,11 +344,20 @@ class PkvBatchCacheLayer(PkvCacheLayer):
     def _book(self, slot: int, rows_host, seen: int) -> None:
         self.rows_host[slot] = list(rows_host)
         self.seq_seen[slot] = int(seen)
+        if self.window is not None:
+            # the admitted rows are the slot's prompt (a parked slot: none); written in place for a captured decode graph
+            H = len(rows_host)
+            self.prompt_rows_host[slot] = list(rows_host)
+            self.generated[slot] = 0
+            self.prompt_rows[slot * H:(slot + 1) * H].copy_(torch.tensor(rows_host, dtype=torch.int32))
         self.length = max(max(r) for r in self.rows_host)
         self.seen_tokens = max(self.seq_seen)
         self._refresh_views()
 
     def update(self, key_states, value_states, *args, **kwargs):
+        if self.window is not None:
+            raise NotImplementedError("multi-token append under the decode window (pkv_decode_window) is not built: decode one "
+                                      "token per step")
         raise NotImplementedError("multi-token append to a joined batch is not defined: its sequences hold different row counts "
                                   "(decode it one token per step: generate.StaticDecoder / greedy_generate_batch)")
 
@@ -332,6 +380,17 @@ def kv_cache_dtype(config) -> Optional[str]:
     return v
 
 
+def decode_window(config) -> Optional[int]:
+    """The knob `pkv_decode_window` of a model config: None (the default: every decoded row stays) or R >= 1, the decoded rows
+    each sequence keeps behind its compacted prompt (the oldest is overwritten first)."""
+    v = getattr(config, "pkv_decode_window", None)
+    if v is None:
+        return None
+    if isinstance(v, bool) or not isinstance(v, int) or v < 1:
+        raise ValueError(f"pkv_decode_window={v!r}: expected None or an int >= 1")
+    return int(v)
+
+
 def gqa_shared(config) -> bool:
     """The knob `pkv_gqa_shared` of a model config (default False): one selection and one compacted cache per KV head."""
     v = getattr(config, "pkv_gqa_shared", False)
@@ -352,16 +411,18 @@ class PkvFp8CacheLayer(PkvBatchCacheLayer):
     _BUFFERS = ("k_buf", "v_buf", "k_scale", "v_scale")
 
     def __init__(self, k_q: torch.Tensor, v_q: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor, rows_host, seq_seen,
-                 group: int = 1):
+                 group: int = 1, **window):
         assert k_q.dtype == torch.float8_e4m3fn and k_scale.shape == k_q.shape[:3] and v_scale.shape == k_scale.shape
         self.k_scale, self.v_scale = k_scale, v_scale
-        super().__init__(k_q, v_q, rows_host, seq_seen, group)
+        super().__init__(k_q, v_q, rows_host, seq_seen, group, **window)
 
     def _scales(self):
         return self.k_scale, self.v_scale
 
     def decode(self, backend, q, k_new, v_new, static=None, softmax_scale: float = 0.0) -> torch.Tensor:
         # the kernel quantises the new K / V row and attends it as stored
+        if self.window is not None:
+            return super().decode(backend, q, k_new, v_new, static, softmax_scale)
         fn = backend.decode_attn_batch_gqa_fp8 if self.group > 1 else backend.decode_attn_batch_fp8
         return fn(q, self.k_buf, self.v_buf, self.k_scale, self.v_scale, 1, k_new, v_new, rows=self.rows,
                   **_devlen_args(self, static), softmax_scale=softmax_scale)
@@ -405,18 +466,26 @@ def quantize_caches_fp8(past_key_values, backend) -> int:
         ks = torch.empty(B, H, cap, dtype=torch.float32, device=l.device)
         vs = torch.empty_like(ks)
         items.append((l.k_buf, l.v_buf, kq, vq, ks, vs, l.length, l.rows_dev))
-        metas.append((kq, vq, ks, vs, l.rows_host, l.seq_seen, l.group))
+        metas.append(((kq, vq, ks, vs, l.rows_host, l.seq_seen, l.group), _window_args(l)))
         idx.append(i)
     if items:
         backend.cache_quantize_fp8(items)
-    for i, m in zip(idx, metas):
-        past_key_values.layers[i] = PkvFp8CacheLayer(*m)
+    for i, (m, w) in zip(idx, metas):
+        past_key_values.layers[i] = PkvFp8CacheLayer(*m, **w)
     return len(idx)
 
 
 def _form(layer) -> tuple:
-    """What decides whether two compacted layers may share a batch: FP8 or 16-bit, and the group (GQA-shared caches)."""
-    return isinstance(layer, PkvFp8CacheLayer), layer.group
+    """What decides whether two compacted layers may share a batch: FP8 or 16-bit, the group (GQA-shared caches) and the
+    decode window."""
+    return isinstance(layer, PkvFp8CacheLayer), layer.group, layer.window
+
+
+def _window_args(layer) -> dict:
+    """The decode-window state of a layer as `PkvBatchCacheLayer` keyword arguments."""
+    if layer.window is None:
+        return {}
+    return dict(window=layer.window, prompt_rows=layer.prompt_rows_host, generated=layer.generated)
 
 
 def join_caches(caches, reserve: int = 0):
@@ -435,7 +504,10 @@ def join_caches(caches, reserve: int = 0):
         raise RuntimeError("join_caches needs caches prefilled by the patched forward on every layer "
                            "(method 'fullkv' and stock caches are not compacted)")
     forms = {_form(l) for l in layers}
-    if len({group for _, group in forms}) > 1:
+    if len({window for _, _, window in forms}) > 1:
+        raise ValueError("join_caches: caches of different decode windows cannot be joined together (set pkv_decode_window the "
+                         "same for every prompt)")
+    if len({group for _, group, _ in forms}) > 1:
         raise ValueError("join_caches: GQA-shared and per-query-head caches (or caches of different groups) cannot be joined "
                          "together (set pkv_gqa_shared the same for every prompt)")
     if len(forms) > 1:
@@ -453,6 +525,8 @@ def join_caches(caches, reserve: int = 0):
             raise ValueError(f"join_caches: layer {i}: head counts, head_dim, dtype or device differ between the caches")
         rows = [l.rows_host[0] for l in src]
         cap = max(max(r) for r in rows) + int(reserve)
+        if l0.window is not None:    # at most P + R rows per (sequence, head)
+            cap = max(p + min(l.generated[0] + int(reserve), l.window) for l in src for p in l.prompt_rows_host[0])
         bufs = []
         for name in l0._BUFFERS:
             t0 = getattr(l0, name)
@@ -461,7 +535,10 @@ def join_caches(caches, reserve: int = 0):
                 t[b, :, : l.length] = getattr(l, name)[0, :, : l.length]
             bufs.append(t)
         cls = type(l0) if isinstance(l0, PkvBatchCacheLayer) else PkvBatchCacheLayer
-        out.layers.append(cls(*bufs, rows, [l.seq_seen[0] for l in src], l0.group))
+        win = {}
+        if l0.window is not None:
+            win = dict(window=l0.window, prompt_rows=[l.prompt_rows_host[0] for l in src], generated=[l.generated[0] for l in src])
+        out.layers.append(cls(*bufs, rows, [l.seq_seen[0] for l in src], l0.group, **win))
     return out
 
 

@@ -595,7 +595,8 @@ struct DecodeScales {
 // `length` rows of one sequence (num_seqs, rows, step_dev and max_length are not used); otherwise every device-length
 // argument is checked.
 static int decode(const char* fn, const pkv_decode_desc* d, bool shared, const DecodeScales* scales, bool host_length, int32_t num_seqs,
-                  int64_t cache_stride_b, const int32_t* rows, const int32_t* step_dev, int64_t max_length, void* stream) {
+                  int64_t cache_stride_b, const int32_t* rows, const int32_t* step_dev, int64_t max_length, void* stream,
+                  int64_t window = 0, const int32_t* prompt_rows = nullptr) {
     int rc = host_length ? PKV_OK : check_devlen_args(fn, num_seqs, rows, step_dev, max_length);
     if (rc) return rc;
     if (scales && (!scales->k || !scales->v)) return fail(PKV_ERR_INVALID_ARG, "%s: null scale pointer", fn);
@@ -628,6 +629,8 @@ static int decode(const char* fn, const pkv_decode_desc* d, bool shared, const D
     a.heads_per_cache = shared ? a.G : 1;
     a.rows = rows;
     a.step_dev = step_dev;
+    a.window = window;
+    a.prompt_rows = prompt_rows;
     DeviceGuard guard(d->device);
     const cudaError_t e = launch_decode(a, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, fn);
@@ -657,6 +660,18 @@ int pkv_decode_attn_batch_gqa_fp8(const pkv_decode_desc* d, int32_t num_seqs, in
                                   int64_t scale_stride_h, int64_t scale_stride_b, void* stream) {
     const DecodeScales scales{k_scale, v_scale, scale_stride_h, scale_stride_b};
     return decode("pkv_decode_attn_batch_gqa_fp8", d, true, &scales, false, num_seqs, cache_stride_b, rows, step_dev, max_length, stream);
+}
+
+int pkv_decode_attn_window(const pkv_decode_desc* d, const pkv_decode_window* w, void* stream) {
+    const char* fn = "pkv_decode_attn_window";
+    if (!w || w->struct_bytes != sizeof(pkv_decode_window))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null pkv_decode_window or struct_bytes != %zu (ABI mismatch)", fn, sizeof(pkv_decode_window));
+    if (w->window < 1) return fail(PKV_ERR_INVALID_ARG, "%s: window=%lld must be >= 1", fn, (long long)w->window);
+    if (!w->prompt_rows || (reinterpret_cast<uintptr_t>(w->prompt_rows) & 3u)) return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned prompt_rows", fn);
+    if ((w->k_scale == nullptr) != (w->v_scale == nullptr)) return fail(PKV_ERR_INVALID_ARG, "%s: null scale pointer", fn);
+    const DecodeScales scales{w->k_scale, w->v_scale, w->scale_stride_h, w->scale_stride_b};
+    return decode(fn, d, w->gqa_shared != 0, w->k_scale ? &scales : nullptr, false, w->num_seqs, w->cache_stride_b, w->rows,
+                  w->step_dev, w->max_length, stream, w->window, w->prompt_rows);
 }
 
 int pkv_cache_quantize_fp8(int32_t dtype, int32_t num_seqs, int32_t num_heads, int32_t head_dim, int32_t device, int32_t num_layers,

@@ -33,6 +33,8 @@ struct DecodeParams {
     float* ws;  // [num_seqs*Hq][nsplit][2 + D] partial (m, l, acc) when nsplit > 1
     const int32_t* step_dev;  // rows = T + *step_dev (graph-replayable decode; the grid is sized for the maximum)
     const int32_t* rows;      // + rows[s*(cache heads) + c] (rows of each sequence and cache head: joined prompts, AdaKV / HeadKV)
+    int64_t window;           // decode window R (0: off): rows past prompt_rows[s*(cache heads) + c] form a ring of R rows
+    const int32_t* prompt_rows;
 };
 
 // Row formats. A lane holds kElems elements of a row (one 128-bit load). score() and weight() give the softmax input of a
@@ -65,10 +67,13 @@ struct RowsE4M3 {   // E4M3 rows with one fp32 scale per row for K and for V (pk
 // output bits. The split count is that of Hq query heads, so a sequence gets the same bits in a batch as alone, and every
 // head of a shared cache the bits it gets from the repeat-interleaved cache. A row count outside [1, max_rows] (the capacity
 // the launch was checked against) is treated as 0: nothing is read or written but the output, which becomes NaN.
+// With a decode window (window > 0, pkv_decode_attn_window) the count n past P = prompt_rows[...] wraps: once n > P + window
+// the new row goes to P + (n-1-P) mod window and P + window rows are attended, with the split rule of that count.
 //
 // Registers: the GH = 1 forms must stay within the ceilings of their occupancy, 80 per thread for 16-bit rows (3 CTAs per
-// SM; 74-75 now) and 128 for E4M3 rows (2 CTAs per SM; at 128 now, no headroom). ptxas -v prints the counts.
-template <typename T, int D, typename Rows, int GH>
+// SM; 64-79 now) and 128 for E4M3 rows (2 CTAs per SM; at 128 now, no headroom). ptxas -v prints the counts. The window is a
+// template parameter so that the launches without one keep the code (and the speed) they had before it existed.
+template <typename T, int D, typename Rows, int GH, bool kWindow>
 __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodeParams p) {
     using Elem = typename Rows::Elem;
     constexpr int E = Rows::kElems;
@@ -93,15 +98,25 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
     Elem* vc = static_cast<Elem*>(p.v_cache) + cache_off;
     const uint16_t* k_new = p.k_new + sk * D;
     const uint16_t* v_new = p.v_new + sk * D;
-    int64_t rows = p.T;
+    int64_t rows = p.T;   // logical row count n: the new row is the n-th
     if (p.step_dev) rows += int64_t(__ldg(p.step_dev));
     if (p.rows) rows += int64_t(__ldg(p.rows + sc));
+    int64_t ring_row = rows - 1;
+    if constexpr (kWindow) {
+        // decode window: the prompt's P rows stay, appended row j (= n-1-P) lives at P + j mod R, and P + R rows are
+        // attended once the ring is full (before that the rows are those of the unwindowed launch)
+        if (rows >= 1) {
+            const int64_t P = int64_t(__ldg(p.prompt_rows + sc));
+            if (P < 0) rows = 0;
+            else if (rows > P + p.window) { ring_row = P + (rows - 1 - P) % p.window; rows = P + p.window; }
+        }
+    }
     if (rows < 1 || rows > p.max_rows) rows = 0;
+    const int64_t new_row = kWindow ? ring_row : rows - 1;
     const int64_t ns = min(int64_t(p.nsplit), decode_splits_for(p.Hq, rows, p.num_sms));
     const int64_t chunk = (rows + ns - 1) / ns;
     const int64_t r_begin = int64_t(split) * chunk;
     const int64_t r_end = min(rows, r_begin + chunk);   // may be <= r_begin (empty split): the partial is (-inf, 0, 0)
-    const int64_t new_row = rows - 1;
     const bool own_new = p.k_new != nullptr && new_row >= r_begin && new_row < r_end;   // uniform over the CTA
 
     // fused append: the CTA that owns the last row stores the new token's K/V
@@ -293,21 +308,23 @@ DecodeParams make_params(const DecodeArgs& a) {
     p.ws = a.ws;
     p.step_dev = a.step_dev;
     p.rows = a.rows;
+    p.window = a.window;
+    p.prompt_rows = a.prompt_rows;
     return p;
 }
 
-template <typename T, int D, typename Rows>
+template <typename T, int D, typename Rows, bool kWindow>
 cudaError_t launch_decode_t(const DecodeArgs& a, cudaStream_t st) {
     const DecodeParams p = make_params(a);
     // query heads per CTA: 1 on a cache per query head; on a shared cache the whole group, for E4M3 at most 4 (the registers
     // of eight heads do not fit)
     const int GH = a.heads_per_cache == 1 ? 1 : Rows::kE4M3 ? min(a.G, 4) : a.G;
     const dim3 grid(unsigned(a.nsplit), unsigned(a.Hq / GH), unsigned(a.num_seqs));
-    if (GH == 1) decode_kernel<T, D, Rows, 1><<<grid, kDecodeThreads, 0, st>>>(p);
-    else if (GH == 2) decode_kernel<T, D, Rows, 2><<<grid, kDecodeThreads, 0, st>>>(p);
-    else if (GH == 4) decode_kernel<T, D, Rows, 4><<<grid, kDecodeThreads, 0, st>>>(p);
+    if (GH == 1) decode_kernel<T, D, Rows, 1, kWindow><<<grid, kDecodeThreads, 0, st>>>(p);
+    else if (GH == 2) decode_kernel<T, D, Rows, 2, kWindow><<<grid, kDecodeThreads, 0, st>>>(p);
+    else if (GH == 4) decode_kernel<T, D, Rows, 4, kWindow><<<grid, kDecodeThreads, 0, st>>>(p);
     else if (!Rows::kE4M3 && GH == 8) {
-        if constexpr (!Rows::kE4M3) decode_kernel<T, D, Rows, 8><<<grid, kDecodeThreads, 0, st>>>(p);
+        if constexpr (!Rows::kE4M3) decode_kernel<T, D, Rows, 8, kWindow><<<grid, kDecodeThreads, 0, st>>>(p);
     } else {
         return cudaErrorInvalidValue;   // no instantiation for this group size
     }
@@ -319,9 +336,15 @@ cudaError_t launch_decode_t(const DecodeArgs& a, cudaStream_t st) {
     return cudaGetLastError();
 }
 
-template <typename T, int D>
+template <typename T, int D, bool kWindow>
 cudaError_t launch_decode_rows(const DecodeArgs& a, cudaStream_t st) {
-    return a.k_scale ? launch_decode_t<T, D, RowsE4M3>(a, st) : launch_decode_t<T, D, Rows16<T>>(a, st);
+    return a.k_scale ? launch_decode_t<T, D, RowsE4M3, kWindow>(a, st) : launch_decode_t<T, D, Rows16<T>, kWindow>(a, st);
+}
+
+template <bool kWindow>
+cudaError_t launch_decode_w(const DecodeArgs& a, cudaStream_t st) {
+    if (a.dtype == PKV_BF16) return a.D == 128 ? launch_decode_rows<__nv_bfloat16, 128, kWindow>(a, st) : launch_decode_rows<__nv_bfloat16, 64, kWindow>(a, st);
+    return a.D == 128 ? launch_decode_rows<__half, 128, kWindow>(a, st) : launch_decode_rows<__half, 64, kWindow>(a, st);
 }
 
 }  // namespace
@@ -329,8 +352,7 @@ cudaError_t launch_decode_rows(const DecodeArgs& a, cudaStream_t st) {
 int decode_num_splits(int Hq, int64_t T, int num_sms) { return int(decode_splits_for(Hq, T, num_sms)); }
 
 cudaError_t launch_decode(const DecodeArgs& a, cudaStream_t st) {
-    if (a.dtype == PKV_BF16) return a.D == 128 ? launch_decode_rows<__nv_bfloat16, 128>(a, st) : launch_decode_rows<__nv_bfloat16, 64>(a, st);
-    return a.D == 128 ? launch_decode_rows<__half, 128>(a, st) : launch_decode_rows<__half, 64>(a, st);
+    return a.window > 0 ? launch_decode_w<true>(a, st) : launch_decode_w<false>(a, st);
 }
 
 cudaError_t launch_append(const DecodeArgs& a, cudaStream_t st) {

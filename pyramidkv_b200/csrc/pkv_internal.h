@@ -106,7 +106,8 @@ int fused_tiles_per_cta(const EvictArgs& a);   // largest number of 128-token ti
 cudaError_t launch_evict_fused(const EvictArgs& a, bool pool_only, cudaStream_t st);
 
 // One decode step over a compacted cache of any form. The row count of each (sequence, cache head) is read on the device:
-// T (+ *step_dev) (+ rows[s*(cache heads) + c]); counts outside [1, max_rows] are not attended (NaN output, nothing written).
+// T (+ *step_dev) (+ rows[s*(cache heads) + c]); counts outside [1, max_rows] (with a window: attended counts above
+// max_rows) are not attended (NaN output, nothing written).
 struct DecodeArgs {
     int dtype, Hq, Hkv, G, D;
     int64_t T;  // valid rows after append (at step 0)
@@ -127,6 +128,10 @@ struct DecodeArgs {
     // E4M3 cache when k_scale is set: k_cache / v_cache hold E4M3 bytes, one fp32 scale per (sequence, cache head, row)
     float *k_scale = nullptr, *v_scale = nullptr;
     int64_t scale_sh = 0, scale_sb = 0;   // floats between the scales of consecutive heads / sequences
+    // decode window (pkv_decode_attn_window) when window > 0: the n-th row of (sequence s, cache head c) with n > P + window,
+    // P = prompt_rows[s*(cache heads) + c], is stored at P + (n-1-P) mod window and P + window rows are attended
+    int64_t window = 0;
+    const int32_t* prompt_rows = nullptr;
 };
 // split count for T rows (decode_num_splits); shared by the launch and the decode kernel
 __host__ __device__ inline int64_t decode_splits_for(int64_t Hq, int64_t T, int64_t num_sms) {

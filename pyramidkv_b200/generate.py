@@ -129,6 +129,13 @@ class StaticDecoder:
             l.reserve(int(max_steps))                      # off the per-token path: no reallocation while the graph lives
         self._setup(model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling)
         self.done = None if self.eos is None else (self.ids == self.eos[None, :]).any(dim=1, keepdim=True)   # [B, 1]
+        if layers[0].window is not None and self.done is not None:
+            # decode window: a finished sequence's later rows would overwrite ring rows its cache keeps, so its row counts
+            # leave the range the kernel attends (it reads and writes nothing; its tokens are pad_token_id anyway)
+            self.window_rows = torch.stack([l.rows for l in layers])
+            for i, l in enumerate(layers):
+                l.rows = self.window_rows[i]
+            self._stop_finished()
 
     def _setup(self, model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling) -> None:
         """The state both decoders hold: the step counter and workspace the decode launches read, the per-sequence input
@@ -151,6 +158,7 @@ class StaticDecoder:
         self.pad_token_id = int(pad_token_id)
         self.taken = 0
         self.graph = None
+        self.window_rows = None   # [layers, B * heads] decode-window row counts, when finished sequences must stop writing
         self.use_graph = (dev.type == "cuda") if use_graph is None else bool(use_graph)
         self.sampling = None
         if sampling is not None:
@@ -176,12 +184,20 @@ class StaticDecoder:
             return self.sampled
         return logits.argmax(dim=-1, keepdim=True)                      # [B, 1]
 
+    _STOPPED = -(2 ** 30)   # a row count no step counter brings back into range
+
+    def _stop_finished(self) -> None:
+        B = self.done.shape[0]
+        self.window_rows.view(len(self.layers), B, -1).masked_fill_(self.done.view(1, B, 1), self._STOPPED)
+
     # one greedy step; every tensor it touches is static, every launch argument constant
     def _step(self) -> None:
         nxt = self._greedy_token()
         if self.done is not None:
             nxt = torch.where(self.done, self.pad_token_id, nxt)
             self.done.logical_or_((nxt == self.eos[None, :]).any(dim=1, keepdim=True))
+            if self.window_rows is not None:
+                self._stop_finished()
         self.tokens.index_copy_(1, self.cursor, nxt)
         self.ids.copy_(nxt)
         self.pos.add_(1)
@@ -191,7 +207,8 @@ class StaticDecoder:
     def _counters(self) -> list:
         """The device tensors a step advances (restored after the warm-up step of a capture)."""
         idx = self.sampling.index if self.sampling is not None else None
-        return [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done, idx) if t is not None]
+        return [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done, idx, self.window_rows)
+                if t is not None]
 
     def _capture(self) -> None:
         # warm up on a side stream (lazy initialisation, cuBLAS workspaces), restore the counters, then capture
@@ -282,8 +299,10 @@ def greedy_generate(model, input_ids: torch.Tensor, max_new_tokens: int, use_gra
     first, cache = _prefill(model, input_ids, sampling)
     toks = [first]
     if max_new_tokens > 1 and not (eos and int(first) in eos):
+        # with a decode window the device stops the sequence at its EOS, so that no later row replaces a kept one
+        windowed = eos and getattr(cache.layers[0], "window", None) is not None
         dec = StaticDecoder(model, cache, first, max_new_tokens - 1, use_graph=use_graph,
-                            sampling=None if sampling is None else [sampling])
+                            eos_token_id=sorted(eos) if windowed else None, sampling=None if sampling is None else [sampling])
         if not eos:
             toks.append(dec.run(max_new_tokens - 1).clone())
         else:
@@ -409,7 +428,8 @@ class ContinuousDecoder(StaticDecoder):
         `reserve`). True when a buffer was reallocated (the graph is then captured again on the next chunk)."""
         grew = False
         for l, s in zip(self.layers, src_cache.layers):
-            grew |= l.fit(max(s.rows_host[0]) + int(new_tokens))
+            # with a decode window at most R decoded rows: the capacity depends only on the prompt and R
+            grew |= l.fit(max(s.rows_host[0]) + (int(new_tokens) if l.window is None else min(int(new_tokens), l.window)))
         if grew:
             self.graph = None
         return grew

@@ -90,6 +90,12 @@ class CudaBackend:
         return ops.decode_attn_batch_gqa_fp8(q, k_q, v_q, k_scale, v_scale, length, k_new, v_new, rows, step, max_length, workspace,
                                              out, softmax_scale)
 
+    # -- the decode window (model.config.pkv_decode_window = R): prompt rows plus a ring of the last R appended rows --
+    def decode_attn_window(self, q, k_buf, v_buf, length, k_new, v_new, prompt_rows, window, rows=None, step=None, max_length=0,
+                           workspace=None, out=None, softmax_scale=0.0, scales=None, gqa=False):
+        return ops.decode_attn_window(q, k_buf, v_buf, length, k_new, v_new, prompt_rows, window, rows, step, max_length,
+                                      workspace, out, softmax_scale, scales, gqa)
+
     # -- continuous batching: one prompt's compacted cache into one slot of a batched cache --
     def cache_install(self, layers, slot, step):
         ops.cache_install(layers, slot, step)

@@ -10,7 +10,7 @@ from typing import Dict, Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import METHODS, POOLING, SCORE_KERNELS, DecodeDesc, EvictDesc, RopeDesc, WsLayout
+from ._lib import METHODS, POOLING, SCORE_KERNELS, DecodeDesc, DecodeWindow, EvictDesc, RopeDesc, WsLayout
 
 _DTYPES = {torch.bfloat16: 0, torch.float16: 1}
 
@@ -431,11 +431,11 @@ def decode_attn_batch(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor,
 
 
 def _decode_batch(entry, what, q, k_buf, v_buf, scales, length, k_new, v_new, rows, step, max_length, workspace, out,
-                  softmax_scale, gqa: bool = False) -> torch.Tensor:
-    """The checks and the descriptor of the four batched decode launches, then the launch of the C entry point `entry`.
+                  softmax_scale, gqa: bool = False, window: int = 0, prompt_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The checks and the descriptor of the batched decode launches, then the launch of the C entry point `entry`.
     `scales`: (k_scale, v_scale) of an FP8 cache, or None. `gqa`: a GQA-shared cache (k_buf / v_buf [B, Hkv, capacity, D],
-    q [B, Hq, D])."""
-    _require_cuda(q, k_buf, v_buf, k_new, v_new, rows, step, workspace, out, *(scales or ()))
+    q [B, Hq, D]). `window` > 0: the decode window over `prompt_rows` (`pkv_decode_attn_window`)."""
+    _require_cuda(q, k_buf, v_buf, k_new, v_new, rows, step, workspace, out, prompt_rows, *(scales or ()))
     if scales is not None:
         _check_fp8_buffers(k_buf, v_buf, scales[0], scales[1], what)
     elif k_buf.dim() != 4 or k_buf.shape != v_buf.shape or k_buf.stride() != v_buf.stride() or k_buf.stride(3) != 1 \
@@ -457,10 +457,20 @@ def _decode_batch(entry, what, q, k_buf, v_buf, scales, length, k_new, v_new, ro
         raise ValueError(f"{what}: cache capacity {cap} exceeded or bad row counts (length {length}, max_length {max_length})")
     if step is not None and (step.dtype != torch.int32 or step.numel() != 1):
         raise ValueError("step must be an int32 device tensor with one element")
+    if window:
+        if prompt_rows is None or prompt_rows.dtype != torch.int32 or prompt_rows.numel() != B * H or not prompt_rows.is_contiguous():
+            raise ValueError(f"{what}: prompt_rows must be a contiguous int32 device tensor of B*{heads} = {B * H} elements")
+        if not torch.cuda.is_current_stream_capturing():
+            # the rows attended: min(n, P + R) per (sequence, cache head) (one device read; a captured launch relies on the caller)
+            n = (rows.reshape(-1).long() if rows is not None else 0) + int(length) + (int(step) if step is not None else 0)
+            most = int(torch.minimum(prompt_rows.reshape(-1).long() + int(window),
+                                     n if torch.is_tensor(n) else torch.full_like(prompt_rows.reshape(-1).long(), n)).max())
+            if most > max_length:
+                raise ValueError(f"{what}: cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
     if rows is not None:
         if rows.dtype != torch.int32 or rows.numel() != B * H or not rows.is_contiguous():
             raise ValueError(f"{what}: rows must be a contiguous int32 device tensor of B*{heads} = {B * H} elements")
-        if not torch.cuda.is_current_stream_capturing():
+        if not window and not torch.cuda.is_current_stream_capturing():
             # (one device read; a captured launch relies on the caller, and the kernel reads and writes no row of a
             # (sequence, head) whose count exceeds max_length)
             most = int(rows.max()) + int(length) + (int(step) if step is not None else 0)
@@ -487,6 +497,19 @@ def _decode_batch(entry, what, q, k_buf, v_buf, scales, length, k_new, v_new, ro
     ws = workspace if workspace is not None else _workspace(q.device, nbytes)
     d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel() * ws.element_size()
     d.softmax_scale = float(softmax_scale)
+    if window:
+        w = DecodeWindow()
+        w.struct_bytes = C.sizeof(DecodeWindow)
+        w.num_seqs, w.cache_stride_b, w.gqa_shared, w.window = B, k_buf.stride(0), int(gqa), int(window)
+        w.rows = rows.data_ptr() if rows is not None else None
+        w.prompt_rows = prompt_rows.data_ptr()
+        w.step_dev = step.data_ptr() if step is not None else None
+        w.max_length = max_length
+        if scales is not None:
+            w.k_scale, w.v_scale = scales[0].data_ptr(), scales[1].data_ptr()
+            w.scale_stride_h, w.scale_stride_b = scales[0].stride(1), scales[0].stride(0)
+        _lib.check(_lib.lib().pkv_decode_attn_window(C.byref(d), C.byref(w), torch.cuda.current_stream(q.device).cuda_stream))
+        return out
     args = (C.byref(d), B, k_buf.stride(0), rows.data_ptr() if rows is not None else None,
             step.data_ptr() if step is not None else None, max_length)
     if scales is not None:
@@ -587,6 +610,24 @@ def decode_attn_batch_gqa_fp8(q: torch.Tensor, k_q: torch.Tensor, v_q: torch.Ten
     [B, Hkv, capacity, D], k_scale / v_scale float32 [B, Hkv, capacity]; otherwise as `decode_attn_batch_gqa`."""
     return _decode_batch("pkv_decode_attn_batch_gqa_fp8", "decode_attn_batch_gqa_fp8", q, k_q, v_q, (k_scale, v_scale),
                          length, k_new, v_new, rows, step, max_length, workspace, out, softmax_scale, gqa=True)
+
+
+# ---- the decode window (include/pkv.h: pkv_decode_attn_window) ----
+def decode_attn_window(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor, length: int,
+                       k_new: Optional[torch.Tensor], v_new: Optional[torch.Tensor], prompt_rows: torch.Tensor, window: int,
+                       rows: Optional[torch.Tensor] = None, step: Optional[torch.Tensor] = None, max_length: int = 0,
+                       workspace: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                       softmax_scale: float = 0.0, scales=None, gqa: bool = False) -> torch.Tensor:
+    """The decode step of `decode_attn_batch` / `_gqa` / `_fp8` / `_gqa_fp8` (picked by `scales` = (k_scale, v_scale) of an
+    FP8 cache and `gqa`) with a decode window of `window` = R >= 1 rows (`pkv_decode_attn_window`): (sequence b, cache head c)
+    keeps its P = prompt_rows[b*H + c] prompt rows (int32 device tensor [B*H]) and its last R appended rows, the j-th
+    appended row at P + j mod R. The logical row count n = `length` (+ `*step`) (+ `rows[b*H + c]`) is that of the
+    unwindowed launch; P + min(n - P, R) rows are attended. The launch is sized for `max_length` rows (default: the
+    capacity), which must hold P + R, and is graph-replayable. Returns out [B, Hq, D]."""
+    if int(window) < 1:
+        raise ValueError(f"decode_attn_window: window={window} must be >= 1")
+    return _decode_batch("pkv_decode_attn_window", "decode_attn_window", q, k_buf, v_buf, scales, length, k_new, v_new, rows, step, max_length, workspace, out,
+                         softmax_scale, gqa=gqa, window=int(window), prompt_rows=prompt_rows)
 
 
 # ---- continuous batching: admission into one slot of a batched cache (include/pkv.h: pkv_cache_install) ----

@@ -100,6 +100,9 @@ class PipelineRunner:
         if getattr(stage.config, "pkv_gqa_shared", False):
             raise NotImplementedError("the GQA-shared cache (pkv_gqa_shared) is installed in the batched row-count form that the "
                                       "layer-sliced pipeline does not decode; it keeps the per-query-head cache")
+        if getattr(stage.config, "pkv_decode_window", None) is not None:
+            raise NotImplementedError("the decode window (pkv_decode_window) holds every layer in the batched row-count form "
+                                      "that the layer-sliced pipeline does not decode")
         self.stage, self.group = stage, group
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1

@@ -61,6 +61,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--gqa_shared", action="store_true",
                    help="one selection and one compacted cache per KV head (the score averaged over each GQA group): "
                         "Hq/Hkv times fewer cache bytes; not for fullkv / adakv / headkv")
+    p.add_argument("--decode_window", type=int, default=None,
+                   help="keep each sequence's cache at its compacted prompt plus its last R decoded tokens (fixed memory for "
+                        "any generation length); default: every decoded token stays")
     return p
 
 
@@ -94,7 +97,8 @@ def main(argv=None, backend_factory=None, device=None):
                             backend_factory=backend_factory, out_path=out, decode_loop=args.decode_loop,
                             floor=args.floor, head_beta=args.head_beta, head_path=args.head_path,
                             capacity_ratio=args.max_capacity_prompts_ratio, eval_batch_size=args.eval_batch_size,
-                            kv_cache_dtype=args.kv_cache_dtype, gqa_shared=args.gqa_shared)
+                            kv_cache_dtype=args.kv_cache_dtype, gqa_shared=args.gqa_shared,
+                            decode_window=args.decode_window)
     n = len(recs)
     print(json.dumps({"summary": True, "arch": arch, "method": method, "max_capacity_prompts": capacity, "examples": n,
                       "mean_prefill_ms": sum(r["prefill_ms"] for r in recs) / n,

@@ -44,6 +44,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--gqa_shared", action="store_true",
                    help="one selection and one compacted cache per KV head (the score averaged over each GQA group): "
                         "Hq/Hkv times fewer cache bytes; not for fullkv / adakv / headkv")
+    p.add_argument("--decode_window", type=int, default=None,
+                   help="keep each sequence's cache at its compacted prompt plus its last R decoded tokens (fixed memory for "
+                        "any generation length); default: every decoded token stays")
     return p
 
 
@@ -60,7 +63,8 @@ def main(argv=None, backend_factory=None, device=None):
         out = os.path.join(args.save_dir, f"{args.model_version or arch}_{args.method}_{args.max_capacity_prompt}.jsonl")
     recs = runner.run_suite(arch, args.method, args.max_capacity_prompt, prompts, device=device, dtype=getattr(torch, args.dtype),
                             attn_implementation=args.attn_implementation, backend_factory=backend_factory, out_path=out,
-                            tag={"runner": "needle"}, decode_loop=args.decode_loop, kv_cache_dtype=args.kv_cache_dtype, gqa_shared=args.gqa_shared)
+                            tag={"runner": "needle"}, decode_loop=args.decode_loop, kv_cache_dtype=args.kv_cache_dtype, gqa_shared=args.gqa_shared,
+                            decode_window=args.decode_window)
     print(json.dumps({"summary": True, "arch": arch, "method": runner.canonical_method(args.method),
                       "max_capacity_prompt": args.max_capacity_prompt, "contexts": [r["prompt_tokens"] for r in recs],
                       "prefill_ms": [round(r["prefill_ms"], 3) for r in recs],
