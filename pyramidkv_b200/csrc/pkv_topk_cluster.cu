@@ -18,6 +18,8 @@
 // rows of exactly those winners; larger k falls back to a bitonic sort in the leader CTA. Same tie rule as topk_kernel
 // (pkv_topk.cu): all keys above the k-th value, then the lowest indices among equals; order (value desc, index asc).
 // Deterministic.
+#include <algorithm>
+
 #include "pkv_common.cuh"
 #include "pkv_internal.h"
 
@@ -131,16 +133,22 @@ __device__ __forceinline__ uint32_t sort_key2(uint32_t u) {
 // layout), score rows, index outputs and K / V source and cache pointers. LB = 1 is the per-layer launch.
 template <int LB> struct SelectLayers { SelectParams p[LB]; };
 
-// OCC: CTAs per SM the register allocation aims at (a layer batch trades a few spilled registers for a third resident CTA)
-template <typename T, bool POOL, bool GATHER, int LB, int OCC = 1>
+// OCC: CTAs per SM the register allocation aims at.
+// SOLO (layer batch): one CTA per head, launched without a cluster. Heads outnumber the SMs many times over, so the kernel
+// wants throughput: every exchange becomes CTA-local (__syncthreads, the CTA's own histograms and winner list), the
+// leader-sort path reuses the dead key buffer for its radix buffers (two CTAs per SM at k ~ 4K, 32K tokens), and the gather
+// takes the indices from shared memory.
+template <typename T, bool POOL, bool GATHER, int LB, int OCC = 1, bool SOLO = false>
 __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __grid_constant__ SelectLayers<LB> layers) {
+    static_assert(!(SOLO && POOL), "the one-CTA form reads pooled scores");
     const SelectParams& p = layers.p[LB == 1 ? 0 : blockIdx.z];
     extern __shared__ __align__(16) uint8_t smem_raw[];
     uint64_t* sortbuf = reinterpret_cast<uint64_t*>(smem_raw);                  // [P] (used in the leader CTA only)
     uint4* keys_s = reinterpret_cast<uint4*>(smem_raw + size_t(p.sort_cap) * 8); // [words_per_cta]
     float* sbuf = reinterpret_cast<float*>(keys_s + p.words_per_cta);           // [words_per_cta*8 + 2*pad] window sums (POOL)
-    uint32_t* hist_all = reinterpret_cast<uint32_t*>(smem_raw + p.hist_off);   // [2 passes][C][kBins] every CTA's histograms
-    int2* mine_s = reinterpret_cast<int2*>(hist_all + 2 * kMaxCluster * kBins); // [ceil(k/C) + 1] (output row, token) of my winners
+    uint32_t* hist_all = reinterpret_cast<uint32_t*>(smem_raw + p.hist_off);   // [2 passes][C][kBins] every CTA's histograms (!SOLO)
+    int2* mine_s = SOLO ? reinterpret_cast<int2*>(smem_raw + p.hist_off)       // [ceil(k/C) + 1] (output row, token) of my winners
+                        : reinterpret_cast<int2*>(hist_all + 2 * kMaxCluster * kBins);
     uint64_t* stage_in = reinterpret_cast<uint64_t*>(smem_raw + p.stage_off);  // [C][blk] every CTA's {count, winners...} (rank path)
     uint64_t* flat_s = stage_in + size_t(kMaxCluster) * p.blk;                 // [k] all winners, concatenated in rank order
     __shared__ int gt_cnt_s[kMaxCluster];
@@ -155,15 +163,15 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
     __shared__ __align__(16) StatP stat_p[POOL ? kMaxW / 2 : 1];                // the same as packed row pairs (fp32 pair operands as loaded)
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t rank = cluster_ctarank(), C = cluster_nctarank();
+    const uint32_t rank = SOLO ? 0u : cluster_ctarank(), C = SOLO ? 1u : cluster_nctarank();
     const int h = blockIdx.y;
     const int w_begin = min(int(rank) * p.words_per_cta, p.n8), w_end = min(w_begin + p.words_per_cta, p.n8);
     const int nw = w_end - w_begin;                                             // my key words (possibly 0)
     int xchg = 0;                                                                // mailbox parity
-    unsigned long long* const stamps = (tid == 0 && rank == 0 && blockIdx.y == 0) ? p.stamps : nullptr;
+    unsigned long long* const stamps = (tid == 0 && rank == 0 && blockIdx.y == 0 && blockIdx.z == 0) ? p.stamps : nullptr;
     int stamp_i = 0;
     stamp(stamps, stamp_i++);   // 0: entry
-    if (tid == 0 && rank == C - 1 && blockIdx.y == 0) stamp(p.stamps, 43);
+    if (tid == 0 && rank == C - 1 && blockIdx.y == 0 && blockIdx.z == 0) stamp(p.stamps, 43);
 
     // All-gather of one 64-bit value per CTA through DSMEM mailboxes: thread 0 arms its own mbarrier for C*8 bytes and
     // st.async's its value into slot[rank] of every CTA (each store completes 8 bytes on the RECEIVER's mbarrier); everyone
@@ -183,7 +191,7 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
     };
 
     const bool rank_path = p.rank_path != 0;
-    if (tid == 0) {
+    if (!SOLO && tid == 0) {
         mbar_init(&xbar[0], 1);
         mbar_init(&xbar[1], 1);
         mbar_init(&hbar[0], 1);
@@ -198,7 +206,8 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
     for (int i = tid; i < 2 * kBins; i += kThreads) (&hist_loc[0][0])[i] = 0u;
     if (rank == 0 && !rank_path)
         for (int i = tid; i < p.P; i += kThreads) sortbuf[i] = ~0ull;
-    cluster_sync();   // mbarriers initialised everywhere, sort buffer cleared: remote traffic may start
+    if constexpr (SOLO) __syncthreads();
+    else cluster_sync();   // mbarriers initialised everywhere, sort buffer cleared: remote traffic may start
     stamp(stamps, stamp_i++);   // 1: first cluster barrier
     // everything above overlaps the previous kernel's tail (PDL)
     pdl_wait();      // the previous kernel has finished writing the logits / partials / scores
@@ -232,10 +241,17 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
 
     if constexpr (!POOL) {
         const uint16_t* row = p.scores + int64_t(h) * p.pitch;
-        for (int i = tid; i < nw; i += kThreads) {
-            const uint4 raw = *reinterpret_cast<const uint4*>(row + size_t(w_begin + i) * 8);
-            uint32_t o[4] = {raw.x, raw.y, raw.z, raw.w};
-            take_word(i, o);
+        for (int i0 = tid; i0 < nw; i0 += 4 * kThreads) {   // four loads in flight per thread, then their keys
+            uint4 raw[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+                if (i0 + u * kThreads < nw) raw[u] = *reinterpret_cast<const uint4*>(row + size_t(w_begin + i0 + u * kThreads) * 8);
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+                if (i0 + u * kThreads < nw) {
+                    uint32_t o[4] = {raw[u].x, raw[u].y, raw[u].z, raw[u].w};
+                    take_word(i0 + u * kThreads, o);
+                }
         }
     } else {
         const int g = h / p.G, col0 = (h % p.G) * p.W;
@@ -333,8 +349,10 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
         const uint32_t v = lane < kWarps ? scan_s[lane] : 0x0000ffffu;
         kmin = __reduce_min_sync(0xffffffffu, v & 0xffffu);
         kmax = __reduce_max_sync(0xffffffffu, v >> 16);
-        const uint64_t* box = allgather(uint64_t(kmin) | (uint64_t(kmax) << 32));
-        for (uint32_t r = 0; r < C; ++r) { kmin = min(kmin, uint32_t(box[r] & 0xffffu)); kmax = max(kmax, uint32_t(box[r] >> 32)); }
+        if constexpr (!SOLO) {
+            const uint64_t* box = allgather(uint64_t(kmin) | (uint64_t(kmax) << 32));
+            for (uint32_t r = 0; r < C; ++r) { kmin = min(kmin, uint32_t(box[r] & 0xffffu)); kmax = max(kmax, uint32_t(box[r] >> 32)); }
+        }
     }
 
     stamp(stamps, stamp_i++);   // 4: min/max exchanged
@@ -365,20 +383,21 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
                 if (take) atomicAdd(&hl[bin], 1u);
             }
         }
-        fence_proxy_async();      // the atomics above are read by the async proxy below
+        if constexpr (!SOLO) fence_proxy_async();      // the atomics above are read by the async proxy below
         __syncthreads();
         stamp(stamps, 32 + 2 * pass);
+        if constexpr (SOLO) return;   // pick_bin reads this CTA's histogram in place
         // broadcast my histogram: one 1 KB bulk copy to each of the C CTAs (completes on the receiver's mbarrier)
         if (tid < int(C))
             bulk_copy_to_peer(map_remote(hist_all + (size_t(pass) * kMaxCluster + rank) * kBins, uint32_t(tid)), hl, kBins * 4u,
                               map_remote(&hbar[pass], uint32_t(tid)));
         mbar_wait(&hbar[pass], 0);
         stamp(stamps, 33 + 2 * pass);
-        if (pass == 1 && tid == 0 && rank == C - 1 && blockIdx.y == 0) stamp(p.stamps, 46);
+        if (pass == 1 && tid == 0 && rank == C - 1 && blockIdx.y == 0 && blockIdx.z == 0) stamp(p.stamps, 46);
     };
     // bin B = largest bin whose suffix count reaches `need`; returns B and the number of keys in the bins above it
     auto pick_bin = [&](int pass, int need, int& B, int& above) {
-        const uint32_t* ha = hist_all + size_t(pass) * kMaxCluster * kBins;
+        const uint32_t* ha = SOLO ? hist_loc[pass] : hist_all + size_t(pass) * kMaxCluster * kBins;
         int tot = 0;
         if (tid < kBins)
             for (uint32_t r = 0; r < C; ++r) tot += int(ha[r * kBins + tid]);
@@ -419,7 +438,7 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
         for (uint32_t r = 0; r < rank; ++r) tie_base += int(hl[r * kBins]);
     }
     int gt_base = 0;                             // keys above thr held by the CTAs before me: only the leader-sort path needs it
-    if (!rank_path) {
+    if (!SOLO && !rank_path) {
         if (warp < int(C)) {
             const uint32_t* h1 = hist_all + size_t(warp) * kBins;
             const uint32_t* h2 = hist_all + (size_t(kMaxCluster) + warp) * kBins;
@@ -435,7 +454,7 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
         for (uint32_t r = 0; r < rank; ++r) gt_base += gt_cnt_s[r];
     }
     stamp(stamps, stamp_i++);   // 7: bases
-    if (tid == 0 && rank == C - 1 && blockIdx.y == 0) stamp(p.stamps, 47);
+    if (tid == 0 && rank == C - 1 && blockIdx.y == 0 && blockIdx.z == 0) stamp(p.stamps, 47);
 
     // ---- emit my winners. Thread t owns the contiguous words [t*wpt, (t+1)*wpt) so ONE block scan gives index-order slots:
     //      into my own staging block (k <= 1024: {count, keys above thr..., my ties...}; broadcast below) or straight into
@@ -474,7 +493,7 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
         inc_t += __shfl_sync(0xffffffffu, it - wt, warp);
     }
     const int taken_t = max(0, min(int(cta_t), need - tie_base));       // my ties that make it
-    const uint32_t sort_remote = map_remote(sortbuf, 0);
+    const uint32_t sort_remote = SOLO ? 0u : map_remote(sortbuf, 0);
     if (my_g + my_t) {
         int gt_pos = int(inc_g - my_g);                             // among MY keys above thr, index order
         int tie_pos = int(inc_t - my_t);                            // among MY ties, index order
@@ -493,11 +512,13 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
                     const uint64_t comp = (uint64_t(0xffffu - key) << 32) | uint64_t(uint32_t(i8 * 8 + e));
                     if ((gt >> bit) & 1u) {
                         if (rank_path) sortbuf[1 + gt_pos] = comp;
+                        else if (SOLO) sortbuf[gt_pos] = comp;
                         else st_remote_u64(sort_remote + uint32_t(gt_base + gt_pos) * 8u, comp);
                         ++gt_pos;
                     } else {
                         if (tie_base + tie_pos < need) {
                             if (rank_path) sortbuf[1 + int(cta_g) + tie_pos] = comp;
+                            else if (SOLO) sortbuf[count_gt + tie_pos] = comp;
                             else st_remote_u64(sort_remote + uint32_t(count_gt + tie_base + tie_pos) * 8u, comp);
                         }
                         ++tie_pos;
@@ -509,34 +530,39 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
     if (rank_path) {
         // ================= k <= 1024: distributed rank sort + gather of exactly my winners =================
         if (tid == 0) sortbuf[0] = uint64_t(int(cta_g) + taken_t);      // block header: how many winners follow
-        fence_proxy_async();
+        if constexpr (!SOLO) fence_proxy_async();
         __syncthreads();
         stamp(stamps, 36);
-        if (tid == 0 && rank == C - 1 && blockIdx.y == 0) stamp(p.stamps, 44);
+        if (tid == 0 && rank == C - 1 && blockIdx.y == 0 && blockIdx.z == 0) stamp(p.stamps, 44);
 #ifdef PKV_STAMPS_BUILD
-        if (tid == 0 && blockIdx.y == 0 && p.stamps) { stamp(p.stamps, 48 + int(rank)); p.stamps[56 + rank] = (uint64_t(cta_g) << 32) | cta_t; }
+        if (tid == 0 && blockIdx.y == 0 && blockIdx.z == 0 && p.stamps) { stamp(p.stamps, 48 + int(rank)); p.stamps[56 + rank] = (uint64_t(cta_g) << 32) | cta_t; }
 #endif
-        if (tid < int(C))          // my block -> row `rank` of every CTA's staging area, one transaction each
-            bulk_copy_to_peer(map_remote(stage_in + size_t(rank) * p.blk, uint32_t(tid)), sortbuf, uint32_t(p.blk) * 8u,
-                              map_remote(&wbar, uint32_t(tid)));
-        mbar_wait(&wbar, 0);       // every CTA's block has landed in MY staging area
-        cluster_arrive_relaxed();  // (peers may still be reading my block / histograms: I must not exit before they all got here)
-        if (tid == 0 && rank == C - 1 && blockIdx.y == 0) stamp(p.stamps, 45);
-        stamp(stamps, stamp_i++);   // 8: winners broadcast
-        // flat list of all k winners in CTA order (any order would do: composites are unique, the rank is a count)
-        for (int t = tid; t < p.k; t += kThreads) {
-            uint64_t cand = ~0ull;
-            int rem = t;
-            for (uint32_t r = 0; r < C; ++r) {
-                const int c = int(stage_in[size_t(r) * p.blk]);
-                if (rem >= 0 && rem < c) cand = stage_in[size_t(r) * p.blk + 1 + rem];
-                rem -= c;
+        // SOLO: the CTA holds all k winners already; they are the flat list
+        const uint64_t* flat = SOLO ? sortbuf + 1 : flat_s;
+        if constexpr (!SOLO) {
+            if (tid < int(C))          // my block -> row `rank` of every CTA's staging area, one transaction each
+                bulk_copy_to_peer(map_remote(stage_in + size_t(rank) * p.blk, uint32_t(tid)), sortbuf, uint32_t(p.blk) * 8u,
+                                  map_remote(&wbar, uint32_t(tid)));
+            mbar_wait(&wbar, 0);       // every CTA's block has landed in MY staging area
+            cluster_arrive_relaxed();  // (peers may still be reading my block / histograms: I must not exit before they all got here)
+            if (tid == 0 && rank == C - 1 && blockIdx.y == 0 && blockIdx.z == 0) stamp(p.stamps, 45);
+            stamp(stamps, stamp_i);   // 8: winners broadcast
+            // flat list of all k winners in CTA order (any order would do: composites are unique, the rank is a count)
+            for (int t = tid; t < p.k; t += kThreads) {
+                uint64_t cand = ~0ull;
+                int rem = t;
+                for (uint32_t r = 0; r < C; ++r) {
+                    const int c = int(stage_in[size_t(r) * p.blk]);
+                    if (rem >= 0 && rem < c) cand = stage_in[size_t(r) * p.blk + 1 + rem];
+                    rem -= c;
+                }
+                flat_s[t] = cand;
             }
-            flat_s[t] = cand;
         }
+        ++stamp_i;
         const int s_begin = int((int64_t(rank) * p.k) / int(C)), s_end = int((int64_t(rank + 1) * p.k) / int(C));
         const int n_mine = s_end - s_begin;
-        __syncthreads();
+        if constexpr (!SOLO) __syncthreads();
         stamp(stamps, 37);
         // 8 lanes per winner, 64 winners per step: each lane counts the candidates below its winner in its slice of the
         // flat list (independent loads; composites are unique, so the rank is that count)
@@ -545,11 +571,11 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
             for (int e0 = 0; e0 < n_mine; e0 += kThreads / 8) {
                 const int e = e0 + gi;
                 const bool active = e < n_mine;
-                const uint64_t me = active ? flat_s[s_begin + e] : 0ull;
+                const uint64_t me = active ? flat[s_begin + e] : 0ull;
                 int below = 0;
                 if (active) {
 #pragma unroll 4
-                    for (int j = sub8; j < p.k; j += 8) below += (flat_s[j] < me) ? 1 : 0;
+                    for (int j = sub8; j < p.k; j += 8) below += (flat[j] < me) ? 1 : 0;
                 }
                 below += __shfl_xor_sync(0xffffffffu, below, 1);
                 below += __shfl_xor_sync(0xffffffffu, below, 2);
@@ -602,16 +628,17 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
             }
         }
         stamp(stamps, stamp_i++);   // 10: done
-        cluster_wait();            // everyone has received everything this CTA sent: its shared memory may go away
+        if constexpr (!SOLO) cluster_wait();   // everyone has received everything this CTA sent: its shared memory may go away
         return;
     }
 
     // ================= k > 1024: bitonic sort in the leader, then the whole cluster gathers =================
-    cluster_sync();               // every winner is in the leader's sort buffer
+    if constexpr (SOLO) __syncthreads();
+    else cluster_sync();          // every winner is in the leader's sort buffer
     if (!GATHER && rank != 0) return;
 
+    uint64_t* sorted = sortbuf;
     if (rank == 0) {
-        uint64_t* sorted = sortbuf;
         if (p.radix_off) {
             // ---- leader: stable LSD radix sort on the 16-bit inverted score (4 passes x 4 bits). The winners arrived in index
             //      order (above-threshold block, then the ties, CTA by CTA), so stability alone yields (score desc, index asc).
@@ -620,7 +647,9 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
             //      all, against 78 for the bitonic network at k = 3978. ----
             uint64_t* const buf0 = sortbuf;
             uint64_t* const buf1 = reinterpret_cast<uint64_t*>(smem_raw + p.radix_off);
-            uint16_t* cnt = reinterpret_cast<uint16_t*>(hist_all);                 // [16][kThreads] (the histograms are dead by now)
+            // [16][kThreads]: the histograms are dead by now (SOLO: behind buf1, in the dead key buffer)
+            uint16_t* cnt = SOLO ? reinterpret_cast<uint16_t*>(smem_raw + p.radix_off + ((size_t(p.k) * 8 + 15) & ~size_t(15)))
+                                 : reinterpret_cast<uint16_t*>(hist_all);
             __shared__ uint32_t wsum[kWarps];
             const int E = (p.k + kThreads - 1) / kThreads;                          // <= 16 (k <= 8192)
             const int e0 = min(tid * E, p.k), e1 = min(e0 + E, p.k);
@@ -694,10 +723,44 @@ __global__ void __launch_bounds__(kThreads, OCC) select_cluster_kernel(const __g
             p.idx32[int64_t(h) * p.k + r] = int32_t(idx);
             if (p.idx64) p.idx64[int64_t(h) * p.k + r] = int64_t(idx);
         }
-        if (GATHER) __threadfence();   // idx32 must be visible to the other CTAs of the cluster
+        if (GATHER && !SOLO) __threadfence();   // idx32 must be visible to the other CTAs of the cluster
     }
     stamp(stamps, stamp_i++);   // 19: sorted + indices written
-    if constexpr (GATHER) {
+    if constexpr (GATHER && SOLO) {
+        // ---- stage 4 from the sorted list in shared memory: K and V rows of four slots in flight per lane ----
+        const int lpr = p.D / 8, rpw = 32 / lpr;
+        const int rows = p.k + p.W;
+        const int sub = lane / lpr, piece = lane % lpr;
+        const int kvh = h / p.G;
+        const uint16_t* srcK = p.src[0] + int64_t(kvh) * p.s_sh[0];
+        const uint16_t* srcV = p.src[1] + int64_t(kvh) * p.s_sh[1];
+        uint16_t* dstK = p.dst[0] + int64_t(h) * p.cache_sh;
+        uint16_t* dstV = p.dst[1] + int64_t(h) * p.cache_sh;
+        const int stride = kWarps * rpw;
+        for (int r0 = warp * rpw + sub; r0 < rows; r0 += stride * 4) {
+            uint4 vk[4], vv[4];
+            int64_t tok[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int r = r0 + u * stride;
+                tok[u] = -1;
+                if (r < rows) tok[u] = (r < p.k) ? int64_t(uint32_t(sorted[r] & 0xffffffffull)) : (p.S - p.W + (r - p.k));
+            }
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+                if (tok[u] >= 0) {
+                    vk[u] = ldg_nc_v4(srcK + tok[u] * p.s_ss[0] + piece * 8);
+                    vv[u] = ldg_nc_v4(srcV + tok[u] * p.s_ss[1] + piece * 8);
+                }
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+                if (tok[u] >= 0) {
+                    const int64_t o = int64_t(r0 + u * stride) * p.D + piece * 8;
+                    *reinterpret_cast<uint4*>(dstK + o) = vk[u];
+                    *reinterpret_cast<uint4*>(dstV + o) = vv[u];
+                }
+        }
+    } else if constexpr (GATHER) {
         cluster_sync();
         stamp(stamps, stamp_i++);   // 20
         // ---- stage 4: rows r = rank, rank + C, ... of this head; half-warp (D=128) / quarter-warp (D=64) per 16-byte piece ----
@@ -740,16 +803,9 @@ constexpr size_t kExclusiveSmem = 116 * 1024;   // > 227 KB / 2
 
 int next_pow2(int64_t v) { int p = 2; while (p < v) p <<= 1; return p; }
 
-int pick_cluster(const EvictArgs& a, bool batch = false) {
+int pick_cluster(const EvictArgs& a) {
     int c = kMaxCluster;
     while (c > 1 && a.Hq * c > a.num_sms) c >>= 1;
-    if (batch) {
-        // Layer batch: heads outnumber the SMs many times over, so a head wants FEWER CTAs (fewer, cheaper exchanges), not more:
-        // one CTA for prompts up to 16K tokens and wherever the leader sorts anyway (k > 1024), else two. Experiment knob
-        // PKV_BATCH_CLUSTER (1, 2, 4, 8).
-        static const int env = [] { const char* e = getenv("PKV_BATCH_CLUSTER"); return e ? atoi(e) : 0; }();
-        c = (env == 1 || env == 2 || env == 4 || env == 8) ? env : (a.S <= 16384 || a.k > kRankMaxK) ? 1 : 2;
-    }
     return c;
 }
 
@@ -769,6 +825,20 @@ size_t select_smem(const EvictArgs& a, int c, bool pool, size_t* hist_off = null
                    bool batch = false) {
     const int64_t n8 = (a.n + 7) / 8, words = (n8 + c - 1) / c;
     const bool rank_path = a.k <= rank_limit(batch);
+    if (batch && c == 1) {
+        // one CTA per head (SOLO): sort buffer / winner list, keys, then the (row, token) list of the rank path. The radix
+        // sort's second buffer and digit table reuse the key buffer, dead once the winners are listed.
+        size_t b = size_t(rank_path ? blk_entries(a) : next_pow2(a.k > 0 ? a.k : 1)) * 8;
+        size_t keys = size_t(words) * 16;
+        if (!rank_path && a.k <= kRadixMaxK) {
+            if (radix_off) *radix_off = b;
+            keys = std::max(keys, ((size_t(a.k) * 8 + 15) & ~size_t(15)) + size_t(16) * kThreads * sizeof(uint16_t));
+        }
+        b = (b + keys + 15) & ~size_t(15);
+        if (hist_off) *hist_off = b;
+        if (rank_path) b += (size_t(a.k) + 2) * sizeof(int2);
+        return b;
+    }
     // sort buffer of the leader (bitonic path) / my outgoing block (rank path)
     size_t b = size_t(rank_path ? blk_entries(a) : next_pow2(a.k > 0 ? a.k : 1)) * 8 + size_t(words) * 16;
     if (pool) b += (size_t(words) * 8 + 2 * kMaxPad) * sizeof(float);
@@ -790,16 +860,17 @@ size_t select_smem(const EvictArgs& a, int c, bool pool, size_t* hist_off = null
     return b;
 }
 
-// one layer's parameters; returns the dynamic shared memory it needs
-// CTAs per head of the layer batch: the preferred count (pick_cluster), doubled while the head's keys + buffers do not fit
+// CTAs per head of the layer batch: one (the SOLO form) where the head's keys and buffers fit one CTA's shared memory, else
+// the fewest whose share fits
 int batch_cluster(const EvictArgs& a) {
-    int c = pick_cluster(a, true);
+    int c = 1;
     while (c < kMaxCluster && select_smem(a, c, false, nullptr, nullptr, nullptr, true) > kSmemBudget) c <<= 1;
     return c;
 }
 
+// one layer's parameters; returns the dynamic shared memory it needs
 template <bool POOL, bool GATHER>
-size_t fill_select_params(const EvictArgs& a, int c, SelectParams* out, int layer = 0, int n_layers = 1, int batch_grid = 0) {
+size_t fill_select_params(const EvictArgs& a, int c, SelectParams* out, int layer = 0, int n_layers = 1, int batch_grid = 0, bool batch = false) {
     SelectParams p = {};
     p.scores = reinterpret_cast<const uint16_t*>(a.ws_base + a.ws.pooled_off);
     p.scores_out = reinterpret_cast<uint16_t*>(a.ws_base + a.ws.pooled_off);
@@ -831,33 +902,25 @@ size_t fill_select_params(const EvictArgs& a, int c, SelectParams* out, int laye
     }
     p.stamps = debug_stamps();
     size_t hist_off = 0, stage_off = 0, radix_off = 0;
-    const size_t smem = select_smem(a, c, POOL, &hist_off, &stage_off, &radix_off, n_layers > 1);
+    const size_t smem = select_smem(a, c, POOL, &hist_off, &stage_off, &radix_off, batch);
     p.radix_off = int(radix_off);
     p.hist_off = int(hist_off);
     p.stage_off = int(stage_off);
     p.kcap = int((a.k + 1) & ~int64_t(1));
     p.blk = blk_entries(a);
-    p.rank_path = a.k <= rank_limit(n_layers > 1) ? 1 : 0;
+    p.rank_path = a.k <= rank_limit(batch) ? 1 : 0;
     p.sort_cap = p.rank_path ? p.blk : p.P;
     *out = p;
     return smem;
 }
 
-template <typename T, bool POOL, bool GATHER, int LB, int OCC = 1>
-cudaError_t launch_select_t(const EvictArgs* as, int n, cudaStream_t st, int batch_grid = 0) {
+template <typename T, bool POOL, bool GATHER, int LB, int OCC = 1, bool SOLO = false>
+cudaError_t launch_select_t(const EvictArgs* as, int n, int c, cudaStream_t st, int batch_grid = 0) {
     const EvictArgs& a = as[0];
-    int c = pick_cluster(a);
-    if (LB > 1) {       // one cluster size per launch: what the layer with the largest budget wants, grown until every layer fits
-        int lmax = 0;
-        for (int l = 1; l < n; ++l) if (as[l].k > as[lmax].k) lmax = l;
-        c = batch_cluster(as[lmax]);
-        for (int l = 0; l < n; ++l)
-            while (c < kMaxCluster && select_smem(as[l], c, false, nullptr, nullptr, nullptr, true) > kSmemBudget) c <<= 1;
-    }
     SelectLayers<LB> layers;
     size_t smem = 0;
     for (int l = 0; l < LB; ++l) {
-        const size_t b = fill_select_params<POOL, GATHER>(as[l < n ? l : 0], c, &layers.p[l], l < n ? l : 0, n, batch_grid);
+        const size_t b = fill_select_params<POOL, GATHER>(as[l < n ? l : 0], c, &layers.p[l], l < n ? l : 0, n, batch_grid, LB > 1);
         if (b > smem) smem = b;
     }
     // Per-layer launch, one CTA per SM: the kernel is a chain of short latency-bound phases, two CTAs sharing an SM's
@@ -866,7 +929,7 @@ cudaError_t launch_select_t(const EvictArgs* as, int n, cudaStream_t st, int bat
     // clusters than SMs and wants throughput, not latency: there the CTAs share SMs as far as their shared memory allows.
     static const bool exclusive = [] { const char* e = getenv("PKV_SELECT_EXCLUSIVE"); return e ? atoi(e) != 0 : true; }();
     const size_t smem_req = (exclusive && LB == 1) ? (smem > kExclusiveSmem ? smem : kExclusiveSmem) : smem;
-    auto kern = select_cluster_kernel<T, POOL, GATHER, LB, OCC>;
+    auto kern = select_cluster_kernel<T, POOL, GATHER, LB, OCC, SOLO>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kSmemBudget));
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};
@@ -875,14 +938,21 @@ cudaError_t launch_select_t(const EvictArgs* as, int n, cudaStream_t st, int bat
     cfg.dynamicSmemBytes = smem_req;
     cfg.stream = st;
     cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = unsigned(c);
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
+    int na = 0;
+    if (!SOLO) {
+        attr[na].id = cudaLaunchAttributeClusterDimension;
+        attr[na].val.clusterDim.x = unsigned(c);
+        attr[na].val.clusterDim.y = 1;
+        attr[na].val.clusterDim.z = 1;
+        ++na;
+    }
+    if (pdl_mask() & 4) {
+        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[na].val.programmaticStreamSerializationAllowed = 1;
+        ++na;
+    }
     cfg.attrs = attr;
-    cfg.numAttrs = (pdl_mask() & 4) ? 2 : 1;
+    cfg.numAttrs = unsigned(na);
     e = cudaLaunchKernelEx(&cfg, kern, layers);
     count_launch();
     return e != cudaSuccess ? e : cudaGetLastError();
@@ -890,7 +960,14 @@ cudaError_t launch_select_t(const EvictArgs* as, int n, cudaStream_t st, int bat
 
 template <bool POOL, bool GATHER>
 cudaError_t launch_select(const EvictArgs& a, cudaStream_t st) {
-    return a.dtype == PKV_BF16 ? launch_select_t<__nv_bfloat16, POOL, GATHER, 1>(&a, 1, st) : launch_select_t<__half, POOL, GATHER, 1>(&a, 1, st);
+    const int c = pick_cluster(a);
+    return a.dtype == PKV_BF16 ? launch_select_t<__nv_bfloat16, POOL, GATHER, 1>(&a, 1, c, st) : launch_select_t<__half, POOL, GATHER, 1>(&a, 1, c, st);
+}
+
+template <int OCC, bool SOLO>
+cudaError_t launch_select_batch(const EvictArgs* as, int n, int c, cudaStream_t st) {
+    return as[0].dtype == PKV_BF16 ? launch_select_t<__nv_bfloat16, false, true, kMaxLayerBatch, OCC, SOLO>(as, n, c, st)
+                                   : launch_select_t<__half, false, true, kMaxLayerBatch, OCC, SOLO>(as, n, c, st);
 }
 
 }  // namespace
@@ -927,22 +1004,13 @@ cudaError_t launch_select_fused(const EvictArgs& a, bool pool, cudaStream_t st) 
 // stages 3+4 of n layers of identical geometry (budgets may differ) in one launch: blockIdx.z = layer
 cudaError_t launch_select_layers(const EvictArgs* as, int n, cudaStream_t st) {
     if (n < 1 || n > kMaxLayerBatch) return cudaErrorInvalidValue;
-    // Register builds for 2 / 3 / 4 resident CTAs per SM (56 / 40 / 32 registers; the kernel is a chain of latency-bound phases, so
-    // residency beats spills). PKV_BATCH_SELECT_OCC picks another build for A/B runs.
-    static const int occ_env = [] { const char* e = getenv("PKV_BATCH_SELECT_OCC"); return e ? atoi(e) : 0; }();
-    int lmax = 0;
-    for (int l = 1; l < n; ++l) if (as[l].k > as[lmax].k) lmax = l;
-    // 40 registers (three CTAs per SM) for the rank-sort path; where the leader sorts (k > 1024) the 56-register build, which
-    // holds the sort without spills
-    const int occ = occ_env ? occ_env : as[lmax].k > kRankMaxK ? 2 : 3;
-    if (occ == 2)
-        return as[0].dtype == PKV_BF16 ? launch_select_t<__nv_bfloat16, false, true, kMaxLayerBatch, 1>(as, n, st)
-                                       : launch_select_t<__half, false, true, kMaxLayerBatch, 1>(as, n, st);
-    if (occ == 4)
-        return as[0].dtype == PKV_BF16 ? launch_select_t<__nv_bfloat16, false, true, kMaxLayerBatch, 4>(as, n, st)
-                                       : launch_select_t<__half, false, true, kMaxLayerBatch, 4>(as, n, st);
-    return as[0].dtype == PKV_BF16 ? launch_select_t<__nv_bfloat16, false, true, kMaxLayerBatch, 3>(as, n, st)
-                                   : launch_select_t<__half, false, true, kMaxLayerBatch, 3>(as, n, st);
+    // one CTA count per launch: the largest any layer needs
+    int c = 1, kmax = 0;
+    for (int l = 0; l < n; ++l) { c = std::max(c, batch_cluster(as[l])); kmax = std::max(kmax, int(as[l].k)); }
+    // Register builds: 40 registers (three 512-thread CTAs per SM) for the rank sort; where the leader sorts, 64 registers for the
+    // one-CTA form (two CTAs per SM, which its shared memory allows up to k = 8192 at 32K tokens) and 56 for the cluster form
+    if (c == 1) return kmax > rank_limit(true) ? launch_select_batch<2, true>(as, n, c, st) : launch_select_batch<3, true>(as, n, c, st);
+    return kmax > kRankMaxK ? launch_select_batch<1, false>(as, n, c, st) : launch_select_batch<3, false>(as, n, c, st);
 }
 
 }  // namespace pkv
