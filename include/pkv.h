@@ -469,6 +469,39 @@ typedef struct pkv_sample_desc {
 } pkv_sample_desc;
 int pkv_sample_tokens(const pkv_sample_desc* d, void* stream);
 
+/* ---- token log-probabilities: the log-softmax of each row of logits at a token and at its top N (DESIGN.md §4.8) ----
+ * Row b (logits[b*logits_stride .. + vocab), bf16 / fp16) is read as the model's raw distribution: x_i = f32(logit_i),
+ * temperature 1, no filters (whatever a sampler does with the row). With m = max_i x_i and Z = sum_i expf(x_i - m), summed
+ * exactly in 64-bit fixed point (2^-40 units, as pkv_sample_tokens sums its masses, so the result does not depend on the
+ * thread schedule):  lp_i = (x_i - m) - logf(Z).  Written, at column c = column (+ *cursor when cursor is not NULL):
+ *  - logprob[b*logprob_stride + c] (fp32) = lp_t of the token t = tokens[b*tokens_stride + tokens_column];
+ *  - for n < top_n: top_ids[b*top_stride + c*top_n + n] (int64) and top_logprobs[same] (fp32), the row's top_n tokens in
+ *    (logit descending, index ascending) order with their lp, so entry 0 is torch.argmax's token of a finite row.
+ * A row with a NaN or +-inf logit gets NaN log-probabilities and top ids -1; so do top entries n >= vocab. A token outside
+ * [0, vocab) gets NaN (device data: not an error). The error of lp against the exact log-softmax of the row is bounded in
+ * DESIGN.md §4.8 (below 1e-5 absolute plus half an fp32 ulp of lp). No allocation, no synchronisation, fixed launch
+ * arguments: the launch replays in a CUDA graph. PKV_ERR_INVALID_ARG: batch outside [1, 2^20], vocab outside [1, 2^24],
+ * logits_stride < vocab, top_n outside [0, 20], tokens_column outside [0, tokens_stride), column < 0, logprob_stride <=
+ * column, top_stride < (column + 1) * top_n, null or misaligned pointers (2 bytes for the logits, 4 for logprob /
+ * top_logprobs, 8 for tokens / top_ids / cursor; top_ids and top_logprobs may be NULL when top_n = 0), unknown flags.
+ * With a cursor the strides cannot bound the column it adds: the caller keeps column + *cursor inside its buffers. */
+typedef struct pkv_logprobs_desc {
+    uint32_t struct_bytes;  /* = sizeof(pkv_logprobs_desc) */
+    int32_t dtype;          /* pkv_dtype of the logits */
+    int32_t device;
+    int32_t batch;          /* rows */
+    int64_t vocab;          /* logits per row */
+    const void* logits; int64_t logits_stride;   /* elements between rows */
+    const int64_t* tokens; int64_t tokens_stride; int64_t tokens_column;   /* int64 [batch, tokens_stride] */
+    int32_t top_n;          /* 0 .. 20 */
+    uint32_t flags;         /* none defined: 0 */
+    const int64_t* cursor;  /* optional device int64 added to column */
+    int64_t column;
+    float* logprob; int64_t logprob_stride;           /* fp32 [batch, logprob_stride] */
+    int64_t* top_ids; float* top_logprobs; int64_t top_stride;   /* [batch, top_stride], top_n entries per column */
+} pkv_logprobs_desc;
+int pkv_token_logprobs(const pkv_logprobs_desc* d, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

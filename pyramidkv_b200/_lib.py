@@ -23,6 +23,7 @@ EXPORTS = [
     "pkv_evict_prefill_batch", "pkv_evict_batch_supported", "pkv_stage_batch", "pkv_decode_attn_batch",
     "pkv_decode_attn_batch_fp8", "pkv_cache_quantize_fp8", "pkv_decode_attn_batch_gqa", "pkv_decode_attn_batch_gqa_fp8",
     "pkv_evict_pooled_kv_offset", "pkv_cache_install", "pkv_sample_tokens", "pkv_decode_attn_window",
+    "pkv_token_logprobs",
 ]
 FLAG_GQA_SHARED = 128          # pkv_evict_desc.flags: one compacted cache per KV head
 
@@ -92,6 +93,20 @@ class SampleDesc(C.Structure):
         ("token_index", C.c_void_p), ("tokens", C.c_void_p), ("tokens_stride", C.c_int64), ("column", C.c_int64),
         ("flags", C.c_uint32), ("reserved", C.c_uint32),
     ]
+
+
+class LogprobsDesc(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("dtype", C.c_int32), ("device", C.c_int32), ("batch", C.c_int32),
+        ("vocab", C.c_int64), ("logits", C.c_void_p), ("logits_stride", C.c_int64),
+        ("tokens", C.c_void_p), ("tokens_stride", C.c_int64), ("tokens_column", C.c_int64),
+        ("top_n", C.c_int32), ("flags", C.c_uint32), ("cursor", C.c_void_p), ("column", C.c_int64),
+        ("logprob", C.c_void_p), ("logprob_stride", C.c_int64),
+        ("top_ids", C.c_void_p), ("top_logprobs", C.c_void_p), ("top_stride", C.c_int64),
+    ]
+
+
+MAX_TOP_LOGPROBS = 20         # pkv_logprobs_desc.top_n
 
 
 class PkvError(RuntimeError):
@@ -180,6 +195,8 @@ def lib() -> C.CDLL:
     L.pkv_cache_install.restype = i32
     L.pkv_sample_tokens.argtypes = [C.POINTER(SampleDesc), p]
     L.pkv_sample_tokens.restype = i32
+    L.pkv_token_logprobs.argtypes = [C.POINTER(LogprobsDesc), p]
+    L.pkv_token_logprobs.restype = i32
     if L.pkv_version() != 3:
         raise RuntimeError(f"libpkv ABI version {L.pkv_version()} != 3; rebuild with `python -m pyramidkv_b200.build --force`")
     _lib = L

@@ -891,6 +891,45 @@ int pkv_sample_tokens(const pkv_sample_desc* d, void* stream) {
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "sample launch");
 }
 
+int pkv_token_logprobs(const pkv_logprobs_desc* d, void* stream) {
+    const char* fn = "pkv_token_logprobs";
+    if (!d) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
+    if (d->struct_bytes != sizeof(pkv_logprobs_desc))
+        return fail(PKV_ERR_INVALID_ARG, "pkv_logprobs_desc.struct_bytes=%u, library expects %zu (ABI mismatch)", d->struct_bytes, sizeof(pkv_logprobs_desc));
+    if (d->dtype != PKV_BF16 && d->dtype != PKV_FP16) return fail(PKV_ERR_UNSUPPORTED_DTYPE, "%s: dtype %d: only bf16 (0) and fp16 (1) logits", fn, d->dtype);
+    if (d->batch < 1 || d->batch > (1 << 20)) return fail(PKV_ERR_INVALID_ARG, "%s: batch=%d outside [1, 2^20]", fn, d->batch);
+    if (d->vocab < 1 || d->vocab > (int64_t(1) << 24)) return fail(PKV_ERR_INVALID_ARG, "%s: vocab=%lld outside [1, 2^24]", fn, (long long)d->vocab);
+    if (d->logits_stride < d->vocab) return fail(PKV_ERR_INVALID_ARG, "%s: logits_stride=%lld < vocab=%lld", fn, (long long)d->logits_stride, (long long)d->vocab);
+    if (d->top_n < 0 || d->top_n > kMaxTopLogprobs) return fail(PKV_ERR_INVALID_ARG, "%s: top_n=%d outside [0, %d]", fn, d->top_n, kMaxTopLogprobs);
+    if (d->tokens_column < 0 || d->tokens_column >= d->tokens_stride)
+        return fail(PKV_ERR_INVALID_ARG, "%s: tokens_column=%lld outside [0, tokens_stride=%lld)", fn, (long long)d->tokens_column, (long long)d->tokens_stride);
+    if (d->column < 0 || d->logprob_stride <= d->column)
+        return fail(PKV_ERR_INVALID_ARG, "%s: column=%lld outside [0, logprob_stride=%lld)", fn, (long long)d->column, (long long)d->logprob_stride);
+    if (d->top_n > 0 && d->top_stride < (d->column + 1) * d->top_n)
+        return fail(PKV_ERR_INVALID_ARG, "%s: top_stride=%lld < (column + 1) * top_n = %lld", fn, (long long)d->top_stride, (long long)((d->column + 1) * d->top_n));
+    if (d->flags) return fail(PKV_ERR_INVALID_ARG, "%s: unknown flags 0x%x", fn, d->flags);
+    auto bad = [](const void* p, uintptr_t align) { return !p || (reinterpret_cast<uintptr_t>(p) & (align - 1)); };
+    if (bad(d->logits, 2)) return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned logits (2 bytes)", fn);
+    if (bad(d->tokens, 8)) return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned tokens (8 bytes)", fn);
+    if (bad(d->logprob, 4)) return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned logprob (4 bytes)", fn);
+    if (d->cursor && (reinterpret_cast<uintptr_t>(d->cursor) & 7u)) return fail(PKV_ERR_INVALID_ARG, "%s: misaligned cursor (8 bytes)", fn);
+    if (d->top_n > 0 && (bad(d->top_ids, 8) || bad(d->top_logprobs, 4)))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned top_ids (8 bytes) / top_logprobs (4 bytes)", fn);
+    const DevInfo* di = nullptr;
+    int rc = device_info(d->device, &di);
+    if (rc) return rc;
+    LogprobsArgs a;
+    a.dtype = d->dtype; a.B = d->batch; a.V = int(d->vocab); a.N = d->top_n;
+    a.logits = static_cast<const uint16_t*>(d->logits); a.ld = d->logits_stride;
+    a.tokens = d->tokens; a.tokens_ld = d->tokens_stride; a.tokens_col = d->tokens_column;
+    a.cursor = d->cursor; a.col = d->column;
+    a.lp = d->logprob; a.lp_ld = d->logprob_stride;
+    a.top_ids = d->top_ids; a.top_lp = d->top_logprobs; a.top_ld = d->top_stride;
+    DeviceGuard guard(d->device);
+    const cudaError_t e = launch_logprobs(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "logprobs launch");
+}
+
 int pkv_cache_append(const pkv_decode_desc* d, void* stream) {
     DecodeArgs a;
     int rc = resolve_decode(d, &a, false);

@@ -196,6 +196,24 @@ struct SampleArgs {
 };
 cudaError_t launch_sample(const SampleArgs& a, cudaStream_t st);
 
+// log-probabilities of one row of logits at a token and at its top N (pkv_logprobs.cu): one CTA per row
+constexpr int kMaxTopLogprobs = 20;
+struct LogprobsArgs {
+    int dtype, B, V, N;         // N: top entries per row, <= kMaxTopLogprobs
+    const uint16_t* logits;
+    int64_t ld;                 // elements between rows
+    const int64_t* tokens;      // token of row b at tokens[b * tokens_ld + tokens_col]
+    int64_t tokens_ld, tokens_col;
+    const int64_t* cursor;      // optional device column added to col
+    int64_t col;
+    float* lp;                  // lp[b * lp_ld + c], c = col (+ *cursor)
+    int64_t lp_ld;
+    int64_t* top_ids;           // top_ids / top_lp[b * top_ld + c * N + n]
+    float* top_lp;
+    int64_t top_ld;
+};
+cudaError_t launch_logprobs(const LogprobsArgs& a, cudaStream_t st);
+
 // RoPE in place on Q and K (pkv_rope.cu)
 struct RopeArgs {
     int dtype, Hq, Hkv, D;

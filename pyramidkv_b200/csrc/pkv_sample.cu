@@ -13,24 +13,13 @@
 // rounds distinct logits together): the k-th largest x is f32(l_k) / T, and both selections can walk histograms of the
 // 16-bit logit keys. Every sum is an integer sum and every tie is broken by index, so the token does not depend on the
 // thread schedule: a graph replay and a host launch give the same token.
-#include <cmath>
-
-#include "pkv_common.cuh"
 #include "pkv_internal.h"
+#include "pkv_rowsel.cuh"
 
 namespace pkv {
 namespace {
 
-constexpr int kThreads = 1024;
-constexpr int kWarps = kThreads / 32;
-constexpr float kFixScale = 1099511627776.0f;   // 2^40: e_i in (0, 1] -> at most 2^40 units, V <= 2^24 rows sum below 2^64
-
-// bf16 / fp16 bits -> a 16-bit key whose unsigned order is the numeric order (-0 is folded onto +0; NaN never gets here)
-__device__ __forceinline__ uint32_t okey(uint32_t b) {
-    if ((b & 0x7fffu) == 0) b = 0;
-    return (b & 0x8000u) ? (~b & 0xffffu) : (b | 0x8000u);
-}
-__device__ __forceinline__ uint16_t key_bits(uint32_t k) { return uint16_t((k & 0x8000u) ? (k & 0x7fffu) : (~k & 0xffffu)); }
+using namespace rowsel;
 
 // Philox4x32-10 (Salmon et al., SC'11; the Random123 reference constants)
 __device__ __forceinline__ uint4 philox(uint4 c, uint32_t k0, uint32_t k1) {
@@ -50,126 +39,12 @@ __device__ __forceinline__ float gumbel(uint32_t r) {
     return -logf(-logf(u));
 }
 
-__device__ __forceinline__ unsigned long long fixed_mass(float x, float m) {
-    return __float2ull_rn(expf(x - m) * kFixScale);
-}
-
-// (value, index) is better: larger value, NaN above everything, then the lower index
-__device__ __forceinline__ bool better_nan(float v, int i, float bv, int bi) {
-    const bool n = v != v, bn = bv != bv;
-    if (n != bn) return n;
-    if (!n && v != bv) return v > bv;
-    return i < bi;
-}
-__device__ __forceinline__ bool better(float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); }
-
-// Histograms are replicated per lane (bin * 32 + lane): lanes of a warp never add to the same word, whatever the logits
-// (a row's 16-bit keys crowd into a few high-byte bins). reduce_hist folds the replicas into one table before a walk.
+// the per-lane replicated count and mass histograms (rowsel::reduce_hist)
 struct Hist {
     uint32_t cnt[256 * 32];
     unsigned long long mass[256 * 32];
 };
 constexpr size_t kHistBytes = sizeof(Hist);
-
-struct Shared {
-    uint32_t cnt[256];
-    unsigned long long mass[256];
-    float rf[kWarps];
-    int ri[kWarps];
-    unsigned long long ru[kWarps];
-    int wc[kWarps];
-    int bin;
-    unsigned long long above;
-    int cut;
-};
-
-// elements 4g .. 4g+3 of the row (0 past its end): one 8-byte load where the row allows it
-__device__ __forceinline__ void load4(const uint16_t* lg, int g, int V, bool vec, uint32_t (&b)[4]) {
-    const int i = 4 * g;
-    if (vec && i + 3 < V) {
-        const uint2 u = __ldg(reinterpret_cast<const uint2*>(lg) + g);
-        b[0] = u.x & 0xffffu; b[1] = u.x >> 16; b[2] = u.y & 0xffffu; b[3] = u.y >> 16;
-    } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) b[j] = i + j < V ? __ldg(lg + i + j) : 0u;
-    }
-}
-
-template <bool NaN>
-__device__ __forceinline__ void block_best(Shared& S, float& v, int& i) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, v, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, i, o);
-        if (NaN ? better_nan(ov, oi, v, i) : better(ov, oi, v, i)) { v = ov; i = oi; }
-    }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (lane == 0) { S.rf[warp] = v; S.ri[warp] = i; }
-    __syncthreads();
-    v = S.rf[0]; i = S.ri[0];
-    for (int w = 1; w < kWarps; ++w)
-        if (NaN ? better_nan(S.rf[w], S.ri[w], v, i) : better(S.rf[w], S.ri[w], v, i)) { v = S.rf[w]; i = S.ri[w]; }
-    __syncthreads();
-}
-
-__device__ __forceinline__ unsigned long long block_sum(Shared& S, unsigned long long s) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if ((threadIdx.x & 31) == 0) S.ru[threadIdx.x >> 5] = s;
-    __syncthreads();
-    s = 0;
-    for (int w = 0; w < kWarps; ++w) s += S.ru[w];
-    __syncthreads();
-    return s;
-}
-
-// The replicas of each bin summed into red[bin] (warp w: bins 8w .. 8w+7) and cleared. Caller synchronises before and after.
-template <typename T>
-__device__ __forceinline__ void reduce_hist(T* rep, T* red) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int j = 0; j < 256 / kWarps; ++j) {
-        const int bin = warp * (256 / kWarps) + j;
-        T v = rep[bin * 32 + lane];
-        rep[bin * 32 + lane] = 0;
-#pragma unroll
-        for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) red[bin] = v;
-    }
-}
-
-// Warp 0 walks hist[255..0] from the top: the bin b with above(b) < target <= above(b) + hist[b] -> S.bin, S.above.
-// Bins are cleared for the next pass. Caller synchronises before and after.
-template <typename T>
-__device__ void walk_top(Shared& S, T* hist, unsigned long long target) {
-    if (threadIdx.x >= 32) return;
-    const int lane = threadIdx.x;
-    T v[8];
-    unsigned long long own = 0;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { v[j] = hist[255 - 8 * lane - j]; own += v[j]; }
-    unsigned long long incl = own;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-    }
-    const unsigned hit = __ballot_sync(0xffffffffu, incl >= target);
-    const int first = hit ? __ffs(hit) - 1 : 31;
-    if (lane == first) {
-        unsigned long long above = incl - own;
-        int b = 255 - 8 * lane - 7;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            if (above + v[j] >= target) { b = 255 - 8 * lane - j; break; }
-            above += v[j];
-        }
-        S.bin = b;
-        S.above = above;
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) hist[8 * lane + j] = 0;
-}
 
 template <typename E>   // element type of the logits
 __global__ void __launch_bounds__(kThreads, 1) sample_kernel(const __grid_constant__ SampleArgs a) {
@@ -319,23 +194,8 @@ __global__ void __launch_bounds__(kThreads, 1) sample_kernel(const __grid_consta
             const unsigned long long need = (e_tau && above < target) ? (target - above + e_tau - 1) / e_tau : 1;
             if (need < ties) {
                 // pass 6: the index of the need-th tie
-                long long left = (long long)need;
-                const int warp = tid >> 5;
-                if (tid == 0) S.cut = V - 1;
-                for (int base = 0; base < V; base += kThreads) {
-                    const int i = base + tid;
-                    const bool f = i < V && __fdiv_rn(DT<E>::to_f32(__ldg(lg + i)), T) == tau;
-                    const unsigned bal = __ballot_sync(0xffffffffu, f);
-                    if (lane == 0) S.wc[warp] = __popc(bal);
-                    __syncthreads();
-                    int before = 0, total = 0;
-                    for (int w = 0; w < kWarps; ++w) { const int c = S.wc[w]; before += w < warp ? c : 0; total += c; }
-                    if (f && before + __popc(bal & ((1u << lane) - 1u)) + 1 == left) S.cut = i;
-                    __syncthreads();
-                    if (left <= total) break;
-                    left -= total;
-                }
-                cut = S.cut;
+                cut = nth_index(S, V, (long long)need,
+                                [&](int i) { return __fdiv_rn(DT<E>::to_f32(__ldg(lg + i)), T) == tau; });
             }
         }
         // pass 7: Gumbel-max over the kept set {x > tau} + {x == tau, index <= cut}

@@ -30,6 +30,12 @@ All three loops are greedy by default. `sampling=SamplingParams(...)` (or one pe
 prefill's with token index t = 0, decode step n's with t = n - with temperature, top-k, top-p and a per-request seed, one
 `pkv_sample_tokens` launch per step for the whole batch in place of the argmax (DESIGN.md §4.6). A request's tokens depend
 only on its logits, its parameters and its seed, not on its batch position, slot or the graph.
+
+`logprobs=N` (0 to 20) in any of the three loops also returns one `TokenLogprobs` per prompt: the log-probability of every
+generated token and the N most likely tokens at each position, under the model's raw distribution (log_softmax of the
+logits, whatever the sampling parameters), from one `pkv_token_logprobs` launch per step after the argmax or the draw
+(DESIGN.md §4.8). `score_continuations` forces given continuations through the same step and returns their
+log-probabilities over the compacted cache: the likelihood a cache form gives a fixed text.
 """
 from __future__ import annotations
 
@@ -99,6 +105,51 @@ def _sampling_list(sampling, n: int, what: str):
     return out
 
 
+@dataclass
+class TokenLogprobs:
+    """Log-probabilities of one sequence's tokens (host tensors, n tokens, N = the `logprobs` / `top_n` asked for), under
+    the model's raw distribution log_softmax(f32(logits)): temperature 1, no filters. token_ids [n] int64 (the generated or
+    scored tokens), logprobs [n] float32, top_ids [n, N] int64 (logit descending, index ascending) and top_logprobs [n, N]
+    float32. A position whose logits hold a NaN or +-inf has NaN log-probabilities and top ids -1."""
+    token_ids: torch.Tensor
+    logprobs: torch.Tensor
+    top_ids: torch.Tensor
+    top_logprobs: torch.Tensor
+
+
+MAX_LOGPROBS = 20
+
+
+def _check_logprobs(n, what: str) -> Optional[int]:
+    if n is None:
+        return None
+    if isinstance(n, bool) or int(n) != n or not 0 <= int(n) <= MAX_LOGPROBS:
+        raise ValueError(f"{what}: logprobs must be None or an integer in [0, {MAX_LOGPROBS}], got {n!r}")
+    return int(n)
+
+
+class _LogprobBuffers:
+    """Static [B, n] / [B, n, N] buffers `token_logprobs` writes at a column (a device cursor in the decode step)."""
+
+    def __init__(self, B: int, n: int, N: int, device):
+        self.lp = torch.zeros(B, n, dtype=torch.float32, device=device)
+        self.ids = torch.zeros(B, n, N, dtype=torch.long, device=device)
+        self.top = torch.zeros(B, n, N, dtype=torch.float32, device=device)
+
+    def write(self, backend, logits, tokens, cursor=None) -> None:
+        backend.token_logprobs(logits, tokens, self.lp, self.ids, self.top, 0, 0, cursor)
+
+    def host(self, steps: int):
+        """Copies of the first `steps` columns on the host (the buffers are rewritten by the next chunk)."""
+        return tuple(t[:, :steps].to("cpu", copy=True) for t in (self.lp, self.ids, self.top))
+
+
+def _join_entries(tokens, parts) -> TokenLogprobs:
+    """tokens: ids [n]; parts: (lp [k], ids [k, N], top [k, N]) host pieces in order, k summing to n."""
+    return TokenLogprobs(torch.as_tensor(tokens, dtype=torch.long).reshape(-1), torch.cat([p[0] for p in parts]),
+                         torch.cat([p[1] for p in parts]), torch.cat([p[2] for p in parts]))
+
+
 def _backend(model):
     return model.model.layers[0].self_attn.kv_cluster.backend
 
@@ -117,17 +168,27 @@ class StaticDecoder:
     `cache.join_caches`; first_token: the token the prefill produced per sequence ([B] or [B, 1] int64).
     eos_token_id (int or list): a sequence that produced one is done - it keeps decoding in lock-step, but its tokens are
     `pad_token_id` from then on (on the device: `done` [B]); None masks nothing. sampling: None (greedy: the argmax) or one
-    SamplingParams per sequence, whose first decode step draws with token index 1 (the prefill's token is t = 0)."""
+    SamplingParams per sequence, whose first decode step draws with token index 1 (the prefill's token is t = 0).
+    logprobs: None, or N: each step also writes the log-probability of its token and the top N into `self.logprobs`
+    (`_LogprobBuffers`, column = the step). forced: None, or int64 [B, max_steps]: step n takes forced[:, n] as its token
+    instead of the argmax (teacher forcing; it is then the next step's input, and with `logprobs` the token scored)."""
 
     def __init__(self, model, cache, first_token: torch.Tensor, max_steps: int, use_graph: Optional[bool] = None,
-                 eos_token_id=None, pad_token_id: int = 0, sampling: Optional[List[SamplingParams]] = None):
+                 eos_token_id=None, pad_token_id: int = 0, sampling: Optional[List[SamplingParams]] = None,
+                 logprobs: Optional[int] = None, forced: Optional[torch.Tensor] = None):
         layers = [l for l in cache.layers if isinstance(l, PkvCacheLayer)]
         if len(layers) != model.config.num_hidden_layers:
             raise RuntimeError("StaticDecoder needs a cache prefilled by the patched forward on every layer "
                                "(method 'fullkv' and stock caches go through model.generate)")
         for l in layers:
             l.reserve(int(max_steps))                      # off the per-token path: no reallocation while the graph lives
-        self._setup(model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling)
+        self._setup(model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling, logprobs)
+        if forced is not None:
+            if sampling is not None:
+                raise ValueError("StaticDecoder: forced tokens and sampling exclude each other")
+            if tuple(forced.shape) != (self.ids.shape[0], self.max_steps):
+                raise ValueError(f"StaticDecoder: forced must be [B={self.ids.shape[0]}, {self.max_steps}], got {tuple(forced.shape)}")
+            self.forced = forced.to(device=self.ids.device, dtype=torch.long).contiguous()
         self.done = None if self.eos is None else (self.ids == self.eos[None, :]).any(dim=1, keepdim=True)   # [B, 1]
         if layers[0].window is not None and self.done is not None:
             # decode window: a finished sequence's later rows would overwrite ring rows its cache keeps, so its row counts
@@ -137,10 +198,11 @@ class StaticDecoder:
                 l.rows = self.window_rows[i]
             self._stop_finished()
 
-    def _setup(self, model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling) -> None:
+    def _setup(self, model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling,
+               logprobs=None) -> None:
         """The state both decoders hold: the step counter and workspace the decode launches read, the per-sequence input
-        ids and positions, the token buffer [B, max_steps] and its cursor, the EOS ids and, when sampling, the per-sequence
-        sampling state with the buffer the sampled tokens land in."""
+        ids and positions, the token buffer [B, max_steps] and its cursor, the EOS ids, when sampling, the per-sequence
+        sampling state with the buffer the sampled tokens land in, and with `logprobs` the buffers of the log-probabilities."""
         self.model, self.cache, self.layers, self.max_steps = model, cache, layers, int(max_steps)
         dev = layers[0].device
         bsz = layers[0].k_buf.shape[0]
@@ -166,11 +228,14 @@ class StaticDecoder:
                 raise ValueError(f"{len(sampling)} SamplingParams for {bsz} sequences")
             self.sampling = SamplingState(sampling, dev, index=1)
             self.sampled = torch.zeros(bsz, 1, dtype=torch.long, device=dev)
+        self.forced = None
+        self.logprobs = None if logprobs is None else _LogprobBuffers(bsz, self.max_steps, int(logprobs), dev)
         cache._pkv_static = self.state
 
     def _greedy_token(self) -> torch.Tensor:
-        """The forward of one token per sequence through every layer (appending to the cache); the argmax [B, 1], or with
-        sampling the drawn tokens (one `sample_tokens` launch for every sequence; each token index advances by one)."""
+        """The forward of one token per sequence through every layer (appending to the cache); the argmax [B, 1], with
+        sampling the drawn tokens (one `sample_tokens` launch for every sequence; each token index advances by one), or the
+        forced tokens at the cursor. With `logprobs`, one `token_logprobs` launch then scores the token at the cursor."""
         m = self.model.model
         h = m.embed_tokens(self.ids)
         pos_emb = m.rotary_emb(h, position_ids=self.pos)
@@ -179,10 +244,16 @@ class StaticDecoder:
                       past_key_values=self.cache, use_cache=True)
         h = m.norm(h)
         logits = self.model.lm_head(h[:, -1, :])
-        if self.sampling is not None:
+        if self.forced is not None:
+            tok = self.forced.index_select(1, self.cursor)                # [B, 1]
+        elif self.sampling is not None:
             self.backend.sample_tokens(logits, self.sampling, self.sampled, 0)
-            return self.sampled
-        return logits.argmax(dim=-1, keepdim=True)                      # [B, 1]
+            tok = self.sampled
+        else:
+            tok = logits.argmax(dim=-1, keepdim=True)                     # [B, 1]
+        if self.logprobs is not None:
+            self.logprobs.write(self.backend, logits, tok, self.cursor)
+        return tok
 
     _STOPPED = -(2 ** 30)   # a row count no step counter brings back into range
 
@@ -258,21 +329,37 @@ class StaticDecoder:
         self.taken = 0
 
 
-def _prefill(model, input_ids: torch.Tensor, sampling: Optional[SamplingParams] = None):
-    """Prefill (+ eviction in every patched layer) of one prompt: (first token [1, 1], cache). The token is the argmax, or
-    with `sampling` drawn with token index 0."""
+def _prefill_logits(model, input_ids: torch.Tensor):
+    """Prefill (+ eviction in every patched layer) of one prompt: (logits of its last position [1, V], cache)."""
     from transformers import DynamicCache
     if hasattr(model, "prepare_inputs_for_generation"):
         for layer in model.model.layers:                 # what the patched prepare_inputs does on an empty cache (llama_model.py:2609-2612)
             layer.self_attn.kv_seq_len = 0
     cache = DynamicCache(config=model.config)
     out = model(input_ids=input_ids, past_key_values=cache, use_cache=True, logits_to_keep=1)
+    return out.logits[:, -1, :], cache
+
+
+def _score(model, logits: torch.Tensor, token: torch.Tensor, top_n: int):
+    """The log-probability entry of `token` [1, 1] under `logits` [1, V]: host (lp [1], ids [1, N], top [1, N])."""
+    buf = _LogprobBuffers(1, 1, top_n, logits.device)
+    buf.write(_backend(model), logits, token)
+    lp, ids, top = buf.host(1)
+    return lp[0], ids[0], top[0]
+
+
+def _prefill(model, input_ids: torch.Tensor, sampling: Optional[SamplingParams] = None, logprobs: Optional[int] = None):
+    """Prefill (+ eviction in every patched layer) of one prompt: (first token [1, 1], cache), and with `logprobs` the
+    first token's log-probability entry (`_score`). The token is the argmax, or with `sampling` drawn with token index 0."""
+    logits, cache = _prefill_logits(model, input_ids)
     if sampling is None:
-        return out.logits[:, -1, :].argmax(dim=-1, keepdim=True), cache
-    logits = out.logits[:, -1, :]
-    first = torch.zeros(1, 1, dtype=torch.long, device=logits.device)
-    _backend(model).sample_tokens(logits, SamplingState([sampling], logits.device, index=0), first, 0, advance=False)
-    return first, cache
+        first = logits.argmax(dim=-1, keepdim=True)
+    else:
+        first = torch.zeros(1, 1, dtype=torch.long, device=logits.device)
+        _backend(model).sample_tokens(logits, SamplingState([sampling], logits.device, index=0), first, 0, advance=False)
+    if logprobs is None:
+        return first, cache
+    return first, cache, _score(model, logits, first, logprobs)
 
 
 def _eos_set(eos_token_id) -> set:
@@ -284,25 +371,29 @@ def _eos_set(eos_token_id) -> set:
 @torch.no_grad()
 def greedy_generate(model, input_ids: torch.Tensor, max_new_tokens: int, use_graph: Optional[bool] = None,
                     return_cache: bool = False, eos_token_id=None, check_every: int = 16,
-                    sampling: Optional[SamplingParams] = None):
+                    sampling: Optional[SamplingParams] = None, logprobs: Optional[int] = None):
     """Prefill (+ eviction in every patched layer) then up to `max_new_tokens - 1` static decode steps. Greedy unless
     `sampling` (a SamplingParams) is given: every token is then drawn with it (DESIGN.md §4.6).
     Returns sequences [1, prompt + generated] like `generate(...).sequences` (and the cache on request).
     `eos_token_id` (int or list, as the reference runner passes it: run_longbench.py:270-272) ends the generation with the first
     such token (kept, like HF); the device never waits for the host, so the tokens are inspected every `check_every` steps
-    and the surplus steps are dropped."""
+    and the surplus steps are dropped. With `logprobs` = N (0 to 20) the return value gains, as its last element, a list of
+    one `TokenLogprobs` for the generated tokens (DESIGN.md §4.8)."""
     if input_ids.dim() != 2 or input_ids.shape[0] != 1:
         raise NotImplementedError("batch size 1 (as in the reference: README.md:47); greedy_generate_batch decodes several prompts together")
     eos = _eos_set(eos_token_id)
     if sampling is not None and not isinstance(sampling, SamplingParams):
         raise ValueError("greedy_generate: sampling must be a SamplingParams")
-    first, cache = _prefill(model, input_ids, sampling)
-    toks = [first]
+    logprobs = _check_logprobs(logprobs, "greedy_generate")
+    first, cache, *entry = _prefill(model, input_ids, sampling, logprobs)
+    toks, parts = [first], entry
     if max_new_tokens > 1 and not (eos and int(first) in eos):
         # with a decode window the device stops the sequence at its EOS, so that no later row replaces a kept one
         windowed = eos and getattr(cache.layers[0], "window", None) is not None
         dec = StaticDecoder(model, cache, first, max_new_tokens - 1, use_graph=use_graph,
-                            eos_token_id=sorted(eos) if windowed else None, sampling=None if sampling is None else [sampling])
+                            eos_token_id=sorted(eos) if windowed else None, sampling=None if sampling is None else [sampling],
+                            logprobs=logprobs)
+        keep = max_new_tokens - 1
         if not eos:
             toks.append(dec.run(max_new_tokens - 1).clone())
         else:
@@ -318,30 +409,40 @@ def greedy_generate(model, input_ids: torch.Tensor, max_new_tokens: int, use_gra
             toks.append(dec.tokens[:, :keep].clone())
             # rows appended after the EOS stay in the buffers but are not counted: the cache ends with the EOS token
             dec.taken = keep
+        if logprobs is not None:
+            parts.append(tuple(t[0] for t in dec.logprobs.host(keep)))
         dec.finish()
     seq = torch.cat([input_ids, *toks], dim=1)
-    return (seq, cache) if return_cache else seq
+    out = (seq, cache) if return_cache else (seq,)
+    if logprobs is not None:
+        out += ([_join_entries(seq[0, input_ids.shape[1]:].cpu(), parts)],)
+    return out if len(out) > 1 else seq
 
 
 @torch.no_grad()
 def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None, pad_token_id: int = 0,
-                          use_graph: Optional[bool] = None, check_every: int = 16, return_cache: bool = False, sampling=None):
+                          use_graph: Optional[bool] = None, check_every: int = 16, return_cache: bool = False, sampling=None,
+                          logprobs: Optional[int] = None):
     """Greedy generation for several prompts of any lengths (1-D or [1, S] id tensors): each prompt is prefilled alone
     exactly as `greedy_generate` does, the compacted caches are joined, and up to `max_new_tokens - 1` steps decode all of
     them together (`StaticDecoder` over the joined cache). Each sequence stops at its first `eos_token_id` (kept, like HF);
     the loop ends once all are done, which the host checks every `check_every` steps. Returns one 1-D tensor per prompt,
     prompt + generated (and the joined cache on request, its per-sequence rows ending at each EOS). Greedy unless `sampling`
-    (one SamplingParams for all prompts, or one per prompt) is given: each prompt's tokens are then drawn with its own."""
+    (one SamplingParams for all prompts, or one per prompt) is given: each prompt's tokens are then drawn with its own.
+    With `logprobs` = N (0 to 20) the return value gains, as its last element, one `TokenLogprobs` per prompt for its
+    generated tokens (DESIGN.md §4.8)."""
     ids = [p.reshape(1, -1) for p in prompts]
     if not ids:
         raise ValueError("greedy_generate_batch: no prompts")
     eos = _eos_set(eos_token_id)
     samp = _sampling_list(sampling, len(ids), "greedy_generate_batch")
-    firsts, caches = [], []
+    logprobs = _check_logprobs(logprobs, "greedy_generate_batch")
+    firsts, caches, entries = [], [], []
     for i, p in enumerate(ids):
-        f, c = _prefill(model, p, None if samp is None else samp[i])
+        f, c, *e = _prefill(model, p, None if samp is None else samp[i], logprobs)
         firsts.append(f)
         caches.append(c)
+        entries.append(e)
     first = torch.cat(firsts)                                            # [B, 1]
     steps = max(0, max_new_tokens - 1)
     cache = join_caches(caches, reserve=steps)
@@ -351,7 +452,7 @@ def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None
     gen = torch.empty(len(ids), 0, dtype=torch.long)
     if steps and not all(t in eos for t in first_host):
         dec = StaticDecoder(model, cache, first, steps, use_graph=use_graph, eos_token_id=sorted(eos) if eos else None,
-                            pad_token_id=pad_token_id, sampling=samp)
+                            pad_token_id=pad_token_id, sampling=samp, logprobs=logprobs)
         while dec.taken < steps:
             dec.run(min(max(1, check_every) if eos else steps, steps - dec.taken))
             if eos and bool(dec.done.all()):                            # one device-to-host read per chunk
@@ -363,9 +464,16 @@ def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None
             row = gen[b].tolist()
             hit = next((i for i, t in enumerate(row) if t in eos), None)
             kept[b] = len(row) if hit is None else hit + 1
+        if logprobs is not None:
+            lp, lp_ids, lp_top = dec.logprobs.host(dec.taken)
+            for b in range(len(ids)):
+                entries[b].append((lp[b, : kept[b]], lp_ids[b, : kept[b]], lp_top[b, : kept[b]]))
         dec.finish(kept)
     seqs = [torch.cat([p[0].cpu(), first[b].cpu(), gen[b, : kept[b]]]).to(p.device) for b, p in enumerate(ids)]
-    return (seqs, cache) if return_cache else seqs
+    out = (seqs, cache) if return_cache else (seqs,)
+    if logprobs is not None:
+        out += ([_join_entries(s[p.shape[1]:].cpu(), e) for s, p, e in zip(seqs, ids, entries)],)
+    return out if len(out) > 1 else seqs
 
 
 class ContinuousDecoder(StaticDecoder):
@@ -380,11 +488,13 @@ class ContinuousDecoder(StaticDecoder):
     when an admission needs more rows; the graph is then captured again."""
 
     def __init__(self, model, cache, first_token: torch.Tensor, left, chunk: int, use_graph: Optional[bool] = None,
-                 eos_token_id=None, pad_token_id: int = 0, sampling: Optional[List[SamplingParams]] = None):
+                 eos_token_id=None, pad_token_id: int = 0, sampling: Optional[List[SamplingParams]] = None,
+                 logprobs: Optional[int] = None):
         layers = [l for l in cache.layers if isinstance(l, PkvBatchCacheLayer)]
         if len(layers) != model.config.num_hidden_layers or len(layers) != len(cache.layers):
             raise RuntimeError("ContinuousDecoder needs a batched cache (cache.join_caches) on every layer")
-        self._setup(model, cache, layers, first_token, max(1, int(chunk)), use_graph, eos_token_id, pad_token_id, sampling)
+        self._setup(model, cache, layers, first_token, max(1, int(chunk)), use_graph, eos_token_id, pad_token_id, sampling,
+                    logprobs)
         # every layer's row counts are rows of one tensor, so one op per step stops them growing for the done slots
         self.rows_all = torch.stack([l.rows for l in layers])
         for i, l in enumerate(layers):
@@ -416,9 +526,12 @@ class ContinuousDecoder(StaticDecoder):
         self.captures += 1
 
     def run_chunk(self, steps: int) -> torch.Tensor:
-        """Take `steps` (<= chunk) steps; their tokens [B, steps] on the host."""
+        """Take `steps` (<= chunk) steps; their tokens [B, steps] on the host (with `logprobs`, their log-probabilities in
+        `chunk_logprobs`: host [B, steps], [B, steps, N], [B, steps, N])."""
         self.run(steps)
         toks = self.tokens[:, :steps].cpu()
+        if self.logprobs is not None:
+            self.chunk_logprobs = self.logprobs.host(steps)
         self.cursor.zero_()
         self.taken = 0
         return toks
@@ -472,7 +585,7 @@ def _sync(device: torch.device) -> None:
 @torch.no_grad()
 def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, eos_token_id=None, pad_token_id: int = 0,
                                use_graph: Optional[bool] = None, check_every: int = 16, return_stats: bool = False,
-                               sampling=None):
+                               sampling=None, logprobs: Optional[int] = None):
     """Greedy generation for any number of prompts (1-D or [1, S] id tensors) through `num_slots` sequences decoded together
     (continuous batching). `max_new_tokens`: an int, or one per prompt. The first `num_slots` prompts are prefilled one at a
     time and joined exactly as in `greedy_generate_batch`; decoding then runs in chunks of `check_every` steps. After each
@@ -484,7 +597,9 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     prefill_s / decode_s (host wall time of the prefills and of the rest of the loop) and per prompt `prefill_ms` and
     `cache_rows_first_last` (rows of its first and last layer after the prefill). Greedy unless `sampling` (one
     SamplingParams for all prompts, or one per prompt) is given: each request's tokens are then drawn with its own, and
-    equal those it gets from `greedy_generate_batch` with the same parameters wherever its logits are equal there."""
+    equal those it gets from `greedy_generate_batch` with the same parameters wherever its logits are equal there. With
+    `logprobs` = N (0 to 20) the return value gains, as its last element, one `TokenLogprobs` per prompt for its generated
+    tokens, read with the tokens once per chunk (DESIGN.md §4.8)."""
     ids = [p.reshape(1, -1) for p in prompts]
     if not ids:
         raise ValueError("greedy_generate_continuous: no prompts")
@@ -495,9 +610,11 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
         raise ValueError(f"greedy_generate_continuous: num_slots must be >= 1, got {num_slots}")
     eos = _eos_set(eos_token_id)
     samp = _sampling_list(sampling, len(ids), "greedy_generate_continuous")
+    logprobs = _check_logprobs(logprobs, "greedy_generate_continuous")
     chunk = max(1, int(check_every))
     dev = ids[0].device
     gen = [[] for _ in ids]                        # generated tokens per prompt, the prefill's first token included
+    lps = [[] for _ in ids]                        # with logprobs: their entries, host (lp [k], ids [k, N], top [k, N])
     stats = dict(decode_steps=0, live_slot_steps=0, admissions=0, regrowths=0, graph_captures=0, prefill_s=0.0, decode_s=0.0,
                  prefill_ms=[0.0] * len(ids), cache_rows_first_last=[[] for _ in ids])
     t_start = time.perf_counter()
@@ -508,8 +625,9 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     def prefill(i):
         _sync(dev)
         t0 = time.perf_counter()
-        first, cache = _prefill(model, ids[i], None if samp is None else samp[i])
+        first, cache, *entry = _prefill(model, ids[i], None if samp is None else samp[i], logprobs)
         gen[i].append(int(first))                  # waits for the prefill
+        lps[i].extend(entry)
         ms = (time.perf_counter() - t0) * 1e3
         stats["prefill_ms"][i] = ms
         stats["prefill_s"] += ms / 1e3
@@ -523,7 +641,7 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     slot_req = list(range(B))
     dec = ContinuousDecoder(model, cache, torch.cat(firsts), [0 if finished(b) else caps[b] - 1 for b in range(B)], chunk,
                             use_graph=use_graph, eos_token_id=sorted(eos) if eos else None, pad_token_id=pad_token_id,
-                            sampling=None if samp is None else samp[:B])
+                            sampling=None if samp is None else samp[:B], logprobs=logprobs)
     waiting = B
     while True:
         for s in range(B):
@@ -550,13 +668,64 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
         stats["decode_steps"] += n
         for s in live:
             r = slot_req[s]
-            for t in toks[s].tolist():
+            for j, t in enumerate(toks[s].tolist()):
                 gen[r].append(t)
                 stats["live_slot_steps"] += 1
                 if finished(r):
                     break
+            if logprobs is not None:
+                lps[r].append(tuple(x[s, : j + 1] for x in dec.chunk_logprobs))
     dec.finish()
     stats["graph_captures"] = dec.captures
     stats["decode_s"] = time.perf_counter() - t_start - stats["prefill_s"]
     seqs = [torch.cat([p[0].cpu(), torch.tensor(g, dtype=torch.long)]).to(p.device) for p, g in zip(ids, gen)]
-    return (seqs, stats) if return_stats else seqs
+    out = (seqs, stats) if return_stats else (seqs,)
+    if logprobs is not None:
+        out += ([_join_entries(g, e) for g, e in zip(gen, lps)],)
+    return out if len(out) > 1 else seqs
+
+
+@torch.no_grad()
+def score_continuations(model, prompts, continuations, top_n: int = 0, use_graph: Optional[bool] = None) -> List[TokenLogprobs]:
+    """Teacher-forced log-probabilities of given continuations over the compacted cache: one `TokenLogprobs` per (prompt,
+    continuation) pair (1-D or [1, S] id tensors, or lists of ids; every continuation holds at least one token), for the
+    continuation's tokens, with the top `top_n` (0 to 20) at each position. Each prompt is prefilled alone with its
+    eviction, exactly as in `greedy_generate_batch`, whose logits score continuation[0]; the caches are joined and a
+    `StaticDecoder` in forced mode takes max(len) - 1 steps, step n feeding continuation[n] through the one-token decode step
+    (every cache form, the decode window included) and scoring continuation[n + 1]. Shorter continuations are padded on the
+    device and trimmed here. On the greedy continuations of `greedy_generate_batch` it returns the log-probabilities that
+    `greedy_generate_batch(logprobs=...)` reports: both join the caches and run the same step."""
+    ids = [p.reshape(1, -1) for p in prompts]
+    conts = [torch.as_tensor(c, dtype=torch.long).reshape(-1).cpu() for c in continuations]
+    if not ids or len(conts) != len(ids):
+        raise ValueError(f"score_continuations: {len(ids)} prompts and {len(conts)} continuations; one per prompt, at least one")
+    if any(c.numel() == 0 for c in conts):
+        raise ValueError("score_continuations: every continuation needs at least one token")
+    top_n = _check_logprobs(top_n, "score_continuations")
+    if top_n is None:
+        raise ValueError("score_continuations: top_n must be an integer in [0, 20]")
+    firsts, caches, entries = [], [], []
+    for p, c in zip(ids, conts):
+        logits, cache = _prefill_logits(model, p)
+        if not all(isinstance(l, PkvCacheLayer) for l in cache.layers):
+            raise RuntimeError("score_continuations needs a cache prefilled by the patched forward on every layer "
+                               "(method 'fullkv' and stock caches go through model.generate)")
+        first = c[:1].reshape(1, 1).to(logits.device)
+        firsts.append(first)
+        caches.append(cache)
+        entries.append([_score(model, logits, first, top_n)])
+    steps = max(c.numel() for c in conts) - 1
+    cache = join_caches(caches, reserve=steps)
+    del caches
+    if steps:
+        forced = torch.zeros(len(ids), steps, dtype=torch.long)
+        for b, c in enumerate(conts):
+            forced[b, : c.numel() - 1] = c[1:]
+        dec = StaticDecoder(model, cache, torch.cat(firsts), steps, use_graph=use_graph, logprobs=top_n, forced=forced)
+        dec.run(steps)
+        lp, lp_ids, lp_top = dec.logprobs.host(steps)
+        kept = [c.numel() - 1 for c in conts]
+        for b, k in enumerate(kept):
+            entries[b].append((lp[b, :k], lp_ids[b, :k], lp_top[b, :k]))
+        dec.finish(kept)
+    return [_join_entries(c, e) for c, e in zip(conts, entries)]

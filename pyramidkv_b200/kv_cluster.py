@@ -107,6 +107,10 @@ class CudaBackend:
     def sample_tokens(self, logits, params, out, col, advance=True):
         ops.sample_tokens(logits, params, out, col, advance)
 
+    # -- token log-probabilities: the raw log-softmax at a token and at the row's top N --
+    def token_logprobs(self, logits, tokens, out_lp, out_ids, out_top, col=0, tokens_col=0, cursor=None):
+        ops.token_logprobs(logits, tokens, out_lp, out_ids, out_top, col, tokens_col, cursor)
+
     # -- ragged per-head budgets (AdaKV / HeadKV): scores first, budgets from the host, then select + gather --
     def ragged_begin(self, q, k, v, window_size, kernel_size, pooling):
         """Stages 1-2 (window logits, softmax + pool) into a workspace that stays alive until ragged_finish."""

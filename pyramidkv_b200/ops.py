@@ -755,3 +755,41 @@ def sample_tokens(logits: torch.Tensor, params, out: torch.Tensor, col: int, adv
     d.tokens, d.tokens_stride, d.column = out.data_ptr(), out.stride(0) if B > 1 else out.shape[1], int(col)
     d.flags = _lib.SAMPLE_ADVANCE if advance else 0
     _lib.check(_lib.lib().pkv_sample_tokens(C.byref(d), torch.cuda.current_stream(logits.device).cuda_stream))
+
+
+# ---- token log-probabilities (include/pkv.h: pkv_token_logprobs, DESIGN.md §4.8) ----
+def token_logprobs(logits: torch.Tensor, tokens: torch.Tensor, out_lp: torch.Tensor, out_ids: torch.Tensor,
+                   out_top: torch.Tensor, col: int = 0, tokens_col: int = 0, cursor: Optional[torch.Tensor] = None) -> None:
+    """log_softmax(f32(logits)) of each row of `logits` [B, V] (bf16 / fp16, rows may be strided), the model's raw
+    distribution, in ONE launch: out_lp[b, c] (float32 [B, n]) at the token tokens[b, tokens_col] (int64 [B, *]), and the
+    row's top N = out_ids.shape[2] tokens (logit descending, index ascending) with their log-probabilities into
+    out_ids[b, c] (int64 [B, n, N]) and out_top[b, c] (float32 [B, n, N]). c = col, plus the DEVICE int64 `cursor` [1]
+    when given (not bounds-checked: the caller keeps it inside n). Nothing is read back: the launch replays in a CUDA graph."""
+    _require_cuda(logits, tokens, out_lp, out_ids, out_top, *(() if cursor is None else (cursor,)))
+    if logits.dim() != 2 or logits.stride(1) != 1:
+        raise ValueError(f"token_logprobs: logits must be [B, V] with contiguous rows, got {tuple(logits.shape)}")
+    B, V = logits.shape
+    if tokens.dim() != 2 or tokens.dtype != torch.long or tokens.shape[0] != B or tokens.stride(1) != 1:
+        raise ValueError(f"token_logprobs: tokens must be an int64 [B={B}, n] tensor with contiguous rows")
+    if out_lp.dim() != 2 or out_lp.dtype != torch.float32 or out_lp.shape[0] != B or not out_lp.is_contiguous():
+        raise ValueError(f"token_logprobs: out_lp must be a contiguous float32 [B={B}, n] tensor")
+    n = out_lp.shape[1]
+    if (out_ids.dim() != 3 or out_ids.dtype != torch.long or tuple(out_ids.shape[:2]) != (B, n) or not out_ids.is_contiguous()
+            or out_top.dtype != torch.float32 or out_top.shape != out_ids.shape or not out_top.is_contiguous()):
+        raise ValueError(f"token_logprobs: out_ids / out_top must be contiguous int64 / float32 [B={B}, n={n}, N] tensors")
+    if cursor is not None and (cursor.dtype != torch.long or cursor.numel() != 1):
+        raise ValueError("token_logprobs: cursor must be a one-element int64 tensor")
+    N = out_ids.shape[2]
+    d = _lib.LogprobsDesc()
+    d.struct_bytes = C.sizeof(_lib.LogprobsDesc)
+    d.dtype = _dtype_code(logits)
+    d.device = logits.device.index if logits.device.index is not None else torch.cuda.current_device()
+    d.batch, d.vocab, d.top_n = B, V, N
+    d.logits, d.logits_stride = logits.data_ptr(), logits.stride(0) if B > 1 else V
+    d.tokens, d.tokens_stride, d.tokens_column = tokens.data_ptr(), tokens.stride(0) if B > 1 else tokens.shape[1], int(tokens_col)
+    d.cursor = None if cursor is None else cursor.data_ptr()
+    d.column = int(col)
+    d.logprob, d.logprob_stride = out_lp.data_ptr(), n
+    if N > 0:
+        d.top_ids, d.top_logprobs, d.top_stride = out_ids.data_ptr(), out_top.data_ptr(), n * N
+    _lib.check(_lib.lib().pkv_token_logprobs(C.byref(d), torch.cuda.current_stream(logits.device).cuda_stream))
