@@ -344,6 +344,52 @@ typedef struct pkv_decode_window {
     int64_t window;             /* R >= 1 */
 } pkv_decode_window;
 int pkv_decode_attn_window(const pkv_decode_desc* d, const pkv_decode_window* w, void* stream);
+/* The decode window with heavy hitters (H2O's decode-time rule): the victim is the generated row with the least
+ * accumulated attention, while the R - H most recent rows always stay. `w` is the window of pkv_decode_attn_window (same
+ * forms, layouts, row counts, checks and out-of-range rule); `h` adds H = h->heavy in [0, R - 1] and the state of one layer,
+ * DEVICE memory the caller owns, with H = num_q_heads (or num_kv_heads when gqa_shared) cache heads per sequence:
+ *   scores fp32  [num_seqs*H][R]  A, the accumulated attention of the generated row held in each slot (slot k = row P + k);
+ *   gen    int32 [num_seqs*H][R]  the generation index of that row;
+ *   victim int32 [num_seqs*H]     the row the next appended row replaces once the window is full.
+ * Semantics, per (sequence, cache head) with P prompt rows. The j-th generated row (j = 0 is the prefill's token, appended at
+ * logical count n = P + j + 1) has a score A_j that starts from 0 at the step that appends it. At every step, query head h
+ * gives each row r it attends the probability p = expf(s_r - m_h) / l_h (an IEEE fp32 division), where s_r is the softmax
+ * input of the row as the kernel computes it (for E4M3 rows with the row's K scale) and m_h, l_h are the fp32 maximum and
+ * sum the output of head h is normalised by at this step. Every held generated row, the new one included, then adds
+ * (sum over the query heads reading this cache head, in ascending head order, of p), in fp32: one head for a cache per query
+ * head, the G heads of the group for a GQA-shared one. Prompt rows are never scored or evicted.
+ *   While n <= P + R the step is the ring's (and the unwindowed one's): the row goes to n - 1.
+ *   Once n > P + R the new row j takes the slot of the victim: among the held generated rows of generation index
+ *   <= j - (R - H) (every held row but the R - H - 1 most recent), the one with the smallest A after step n - 1, ties to the
+ *   smallest generation index. So H + 1 rows compete at each step, and the R - H most recent rows always stay.
+ *   When no row qualifies (a count that repeats appends generation j again, as a finished slot of continuous batching
+ *   does, until every held row is that recent), victim = -1 and the following full-window steps are out of range.
+ *   H = 0 is the ring: the only candidate is the oldest row, at P + j mod R, so the cache is bit-identical to
+ *   pkv_decode_attn_window's.
+ * A step's output and appended row are bit-identical to pkv_decode_attn_batch / _gqa / _fp8 / _gqa_fp8 run without k_new
+ * over the same buffer with the new row already at its slot. A count n < 1, P < 0, an attended count above max_length, or a
+ * victim outside [P, P + R) reads and writes nothing (no cache row, no score, no victim) and gives a NaN output; a count
+ * n <= P appends inside the prompt as the unwindowed step does and scores nothing. Every write stays inside rows
+ * [0, P + R). The arithmetic is fixed-order fp32 without atomics: state and outputs do not depend on the thread schedule,
+ * and a graph replay writes the bits of a host launch. A new (sequence, cache head) needs no reset: the rows it appends
+ * overwrite the slots it reads. Launches: the decode (and its combine) and one small bookkeeping kernel.
+ * `scratch` holds the per-step logits and (m, l): pkv_decode_heavy_workspace_bytes(num_seqs, num_q_heads, R) bytes, one
+ * buffer for every layer (the launches are stream-ordered). PKV_ERR_INVALID_ARG, in addition to pkv_decode_attn_window's
+ * errors: h NULL or h->struct_bytes != sizeof(pkv_decode_heavy), heavy outside [0, R - 1], k_new or v_new NULL, a NULL or
+ * not 4-byte aligned scores / gen / victim / scratch. PKV_ERR_WORKSPACE: scratch_bytes too small. */
+typedef struct pkv_decode_heavy {
+    uint32_t struct_bytes;
+    int32_t reserved;
+    int64_t heavy;              /* H in [0, window - 1] */
+    float* scores;              /* DEVICE fp32 [num_seqs*H][window] */
+    int32_t* gen;               /* DEVICE int32 [num_seqs*H][window] */
+    int32_t* victim;            /* DEVICE int32 [num_seqs*H] */
+    void* scratch;              /* DEVICE, pkv_decode_heavy_workspace_bytes */
+    uint64_t scratch_bytes;
+} pkv_decode_heavy;
+int pkv_decode_attn_heavy(const pkv_decode_desc* d, const pkv_decode_window* w, const pkv_decode_heavy* h, void* stream);
+/* Bytes of the per-step scratch of pkv_decode_attn_heavy: num_seqs*num_q_heads*(window + 2) floats; 0 for a count below 1. */
+uint64_t pkv_decode_heavy_workspace_bytes(int32_t num_seqs, int32_t num_q_heads, int64_t window);
 /* Conversion of the compacted 16-bit caches of num_layers layers (one prompt, or one equal-length batch of num_seqs
  * sequences) to the FP8 format above, in one launch per 32 layers; the per-layer tables travel as kernel parameters.
  * Layer l: src[2l] / src[2l+1] = K / V, 16-bit contiguous [num_seqs, num_heads, src_capacity[l], head_dim]; dst[2l] /

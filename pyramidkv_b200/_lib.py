@@ -23,6 +23,7 @@ EXPORTS = [
     "pkv_evict_prefill_batch", "pkv_evict_batch_supported", "pkv_stage_batch", "pkv_decode_attn_batch",
     "pkv_decode_attn_batch_fp8", "pkv_cache_quantize_fp8", "pkv_decode_attn_batch_gqa", "pkv_decode_attn_batch_gqa_fp8",
     "pkv_evict_pooled_kv_offset", "pkv_cache_install", "pkv_sample_tokens", "pkv_decode_attn_window",
+    "pkv_decode_attn_heavy", "pkv_decode_heavy_workspace_bytes",
     "pkv_token_logprobs",
 ]
 FLAG_GQA_SHARED = 128          # pkv_evict_desc.flags: one compacted cache per KV head
@@ -69,6 +70,13 @@ class DecodeWindow(C.Structure):
         ("rows", C.c_void_p), ("prompt_rows", C.c_void_p), ("step_dev", C.c_void_p), ("max_length", C.c_int64),
         ("k_scale", C.c_void_p), ("v_scale", C.c_void_p), ("scale_stride_h", C.c_int64), ("scale_stride_b", C.c_int64),
         ("window", C.c_int64),
+    ]
+
+
+class DecodeHeavy(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("reserved", C.c_int32), ("heavy", C.c_int64),
+        ("scores", C.c_void_p), ("gen", C.c_void_p), ("victim", C.c_void_p), ("scratch", C.c_void_p), ("scratch_bytes", C.c_uint64),
     ]
 
 
@@ -186,6 +194,10 @@ def lib() -> C.CDLL:
     L.pkv_decode_attn_batch_gqa_fp8.restype = i32
     L.pkv_decode_attn_window.argtypes = [C.POINTER(DecodeDesc), C.POINTER(DecodeWindow), p]
     L.pkv_decode_attn_window.restype = i32
+    L.pkv_decode_attn_heavy.argtypes = [C.POINTER(DecodeDesc), C.POINTER(DecodeWindow), C.POINTER(DecodeHeavy), p]
+    L.pkv_decode_attn_heavy.restype = i32
+    L.pkv_decode_heavy_workspace_bytes.argtypes = [C.c_int32, C.c_int32, i64]
+    L.pkv_decode_heavy_workspace_bytes.restype = u64
     # tables: src / dst / scales [2*layers] pointers, capacities and rows [layers] int64, rows_dev [layers] pointers or NULL
     L.pkv_cache_quantize_fp8.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p, p, p, p, p, p, p, p]
     L.pkv_cache_quantize_fp8.restype = i32

@@ -22,8 +22,8 @@ from typing import Callable, Optional
 import torch
 from transformers.modeling_utils import ALL_ATTENTION_FUNCTIONS
 
-from .cache import (PkvBatchCacheLayer, PkvCacheLayer, PkvRaggedCacheLayer, decode_window, gqa_shared, install_layer,
-                    kv_cache_dtype, layer_is_empty, quantize_caches_fp8)
+from .cache import (PkvBatchCacheLayer, PkvCacheLayer, PkvRaggedCacheLayer, decode_heavy, decode_window, gqa_shared,
+                    install_layer, kv_cache_dtype, layer_is_empty, quantize_caches_fp8)
 from .kv_cluster import INIT_BY_METHOD, flush_pending
 
 DEFAULT_DECODE_RESERVE = 256   # rows of head-room behind the compacted prompt (grows by doubling)
@@ -112,6 +112,7 @@ def make_forward(method: str, modeling, original_forward):
             cluster.inputs_ready = True      # the launch in front of the eviction is the dense attention: it only reads q / k / v
             reserve = int(getattr(self.config, "pkv_decode_reserve", DEFAULT_DECODE_RESERVE))
             window = decode_window(self.config)
+            heavy = decode_heavy(self.config)   # knob pkv_decode_heavy: heavy hitters in that window
             if window is not None:       # knob pkv_decode_window: at most R decoded rows behind the prompt
                 reserve = min(reserve, window)
             group = num_q_heads // key_states.shape[1] if gqa_shared(self.config) else 1
@@ -124,7 +125,8 @@ def make_forward(method: str, modeling, original_forward):
                     raise NotImplementedError("AdaKV / HeadKV are batch size 1 (pyramidkv_utils.py:723)")
                 k_buf, v_buf, head_rows = cluster.evict_ragged(query_states[0], key_states[0], value_states[0], reserve=reserve)
                 if window is not None:   # the per-(sequence, head) row-count form carries the window
-                    layer = PkvBatchCacheLayer(k_buf[None], v_buf[None], [[int(r) for r in head_rows]], [q_len], window=window)
+                    layer = PkvBatchCacheLayer(k_buf[None], v_buf[None], [[int(r) for r in head_rows]], [q_len], window=window,
+                                               heavy=heavy)
                 else:
                     layer = PkvRaggedCacheLayer(k_buf[None], v_buf[None], head_rows, seen_tokens=q_len)
                 install_layer(past_key_values, self.layer_idx, layer)
@@ -152,7 +154,8 @@ def make_forward(method: str, modeling, original_forward):
             if group > 1 or window is not None:
                 # knob pkv_gqa_shared: one cache per KV head; knob pkv_decode_window: a ring of decoded rows. Both are held in
                 # the per-(sequence, head) row-count form
-                layer = PkvBatchCacheLayer(k_buf, v_buf, [[rows] * k_buf.shape[1]] * bsz, [q_len] * bsz, group=group, window=window)
+                layer = PkvBatchCacheLayer(k_buf, v_buf, [[rows] * k_buf.shape[1]] * bsz, [q_len] * bsz, group=group, window=window,
+                                           heavy=heavy)
             else:
                 layer = PkvCacheLayer(k_buf, v_buf, rows, seen_tokens=q_len)
             install_layer(past_key_values, self.layer_idx, layer)

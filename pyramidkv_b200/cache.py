@@ -28,6 +28,7 @@ class PkvCacheLayer(DynamicLayer):
     is_sliding = False
     group = 1                        # query heads per cache head (> 1: a GQA-shared cache, `PkvBatchCacheLayer`)
     window = None                    # decode window R (knob `pkv_decode_window`; `PkvBatchCacheLayer` only)
+    heavy = None                     # heavy hitters H in the decode window (knob `pkv_decode_heavy`; `PkvBatchCacheLayer` only)
     _BUFFERS = ("k_buf", "v_buf")    # the [B, H, capacity, ...] tensors a resize or a join copies
 
     def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, length: int, seen_tokens: int):
@@ -225,12 +226,18 @@ class PkvBatchCacheLayer(PkvCacheLayer):
     of its last R appended rows, the j-th at row P + j mod R (`pkv_decode_attn_window`). `generated[b]` counts the rows
     sequence b appended; `rows_host[b][h]` = P + min(generated[b], R) are the rows the buffers hold, in ring order (not
     token order) past P, while the device `rows` hold the logical counts P + generated[b] the kernel derives the ring slot
-    from. `prompt_rows` is the device copy of P (int32 [B*H]). None: no window."""
+    from. `prompt_rows` is the device copy of P (int32 [B*H]). None: no window.
+
+    `heavy` H (knob `pkv_decode_heavy`, with a window): once the window is full the new row replaces the generated row with
+    the least accumulated attention among all but the R - H - 1 most recent (`pkv_decode_attn_heavy`). The layer's state,
+    updated on the device by every step: `heavy_scores` fp32 [B, H, R] and `heavy_gen` int32 [B, H, R] (the accumulated
+    attention and the generation index of the row in each slot past P) and `victim` int32 [B*H] (the row the next step
+    replaces). Slots still fill in order and are then replaced in place, so `rows_host` is the window's. None: the ring."""
 
     rows_host = seq_seen = None    # held per sequence here (set in __init__), not derived from `length` as in the base class
 
     def __init__(self, k_buf: torch.Tensor, v_buf: torch.Tensor, rows_host, seq_seen, group: int = 1, window: Optional[int] = None,
-                 prompt_rows=None, generated=None):
+                 prompt_rows=None, generated=None, heavy: Optional[int] = None, heavy_state=None):
         self.group = int(group)
         self.rows_host = [[int(r) for r in row] for row in rows_host]
         self.seq_seen = [int(s) for s in seq_seen]
@@ -241,6 +248,15 @@ class PkvBatchCacheLayer(PkvCacheLayer):
             self.prompt_rows_host = [list(r) for r in (prompt_rows if prompt_rows is not None else self.rows_host)]
             self.generated = [int(g) for g in generated] if generated is not None else [0] * len(self.rows_host)
             self.prompt_rows = self._device_counts(self.prompt_rows_host, k_buf.device)
+        self.heavy = None if heavy is None else int(heavy)
+        if self.heavy is not None:
+            assert self.window is not None and 0 <= self.heavy < self.window
+            B, H = k_buf.shape[:2]
+            if heavy_state is None:    # a new cache: nothing generated yet, so no slot is read before the step that fills it
+                heavy_state = (torch.zeros(B, H, self.window, dtype=torch.float32, device=k_buf.device),
+                               torch.full((B, H, self.window), -1, dtype=torch.int32, device=k_buf.device),
+                               torch.full((B * H,), -1, dtype=torch.int32, device=k_buf.device))
+            self.heavy_scores, self.heavy_gen, self.victim = heavy_state
         self.rows = self._device_rows(k_buf.device)
         super().__init__(k_buf, v_buf, max(max(r) for r in self.rows_host), max(self.seq_seen))
 
@@ -292,6 +308,11 @@ class PkvBatchCacheLayer(PkvCacheLayer):
 
     def decode(self, backend, q, k_new, v_new, static=None, softmax_scale: float = 0.0) -> torch.Tensor:
         # rows = layer.rows[b, h] + 1 (+ the step counter in the static loop); G > 1: each KV head read once for its group
+        if self.heavy is not None:
+            return backend.decode_attn_heavy(q, self.k_buf, self.v_buf, 1, k_new, v_new, self.prompt_rows, self.window, self.heavy,
+                                             self.heavy_scores, self.heavy_gen, self.victim, rows=self.rows,
+                                             **_devlen_args(self, static), scratch=getattr(static, "heavy_scratch", None),
+                                             softmax_scale=softmax_scale, scales=self._scales(), gqa=self.group > 1)
         if self.window is not None:
             return backend.decode_attn_window(q, self.k_buf, self.v_buf, 1, k_new, v_new, self.prompt_rows, self.window,
                                               rows=self.rows, **_devlen_args(self, static), softmax_scale=softmax_scale,
@@ -328,9 +349,10 @@ class PkvBatchCacheLayer(PkvCacheLayer):
             return (None, None, None, 0, None, *dst), [0] * H, 0
         if not isinstance(src, PkvCacheLayer) or _form(src) != _form(self):
             raise ValueError(f"admit: a {type(src).__name__} (group {getattr(src, 'group', 1)}, decode window "
-                             f"{getattr(src, 'window', None)}) cannot enter a {type(self).__name__} of group {self.group}, "
-                             f"decode window {self.window}: FP8 and 16-bit caches, and caches of different groups or decode "
-                             "windows, do not mix")
+                             f"{getattr(src, 'window', None)}, heavy hitters {getattr(src, 'heavy', None)}) cannot enter a "
+                             f"{type(self).__name__} of group {self.group}, decode window {self.window}, heavy hitters "
+                             f"{self.heavy}: FP8 and 16-bit caches, and caches of different groups, decode windows or heavy "
+                             "hitters (pkv_decode_heavy), do not mix")
         if src.k_buf.shape[0] != 1 or src.k_buf.shape[1] != H or src.k_buf.shape[3] != D or src.dtype != self.dtype \
                 or src.device != self.device:
             raise ValueError(f"admit: the source must be one prompt of {H} heads, head_dim {D}, {self.dtype} on {self.device}; "
@@ -350,6 +372,11 @@ class PkvBatchCacheLayer(PkvCacheLayer):
             self.prompt_rows_host[slot] = list(rows_host)
             self.generated[slot] = 0
             self.prompt_rows[slot * H:(slot + 1) * H].copy_(torch.tensor(rows_host, dtype=torch.int32))
+        if self.heavy is not None:
+            # a new sequence starts with no generated rows; reset in place, where a captured decode graph reads the state
+            self.heavy_scores[slot].zero_()
+            self.heavy_gen[slot].fill_(-1)
+            self.victim[slot * len(rows_host):(slot + 1) * len(rows_host)].fill_(-1)
         self.length = max(max(r) for r in self.rows_host)
         self.seen_tokens = max(self.seq_seen)
         self._refresh_views()
@@ -388,6 +415,21 @@ def decode_window(config) -> Optional[int]:
         return None
     if isinstance(v, bool) or not isinstance(v, int) or v < 1:
         raise ValueError(f"pkv_decode_window={v!r}: expected None or an int >= 1")
+    return int(v)
+
+
+def decode_heavy(config) -> Optional[int]:
+    """The knob `pkv_decode_heavy` of a model config: None (the default: the decode window replaces its oldest row) or H, an
+    int with 1 <= H <= R - 1 under `pkv_decode_window` = R: the window keeps its R - H most recent generated rows, and each
+    new row replaces the one with the least accumulated attention among the others (H2O's heavy hitters, DESIGN.md §4.9)."""
+    v = getattr(config, "pkv_decode_heavy", None)
+    if v is None:
+        return None
+    window = decode_window(config)
+    if window is None:
+        raise ValueError(f"pkv_decode_heavy={v!r} needs the decode window (pkv_decode_window = R)")
+    if isinstance(v, bool) or not isinstance(v, int) or not 1 <= v <= window - 1:
+        raise ValueError(f"pkv_decode_heavy={v!r}: expected None or an int in [1, R - 1] = [1, {window - 1}]")
     return int(v)
 
 
@@ -477,15 +519,16 @@ def quantize_caches_fp8(past_key_values, backend) -> int:
 
 def _form(layer) -> tuple:
     """What decides whether two compacted layers may share a batch: FP8 or 16-bit, the group (GQA-shared caches) and the
-    decode window."""
-    return isinstance(layer, PkvFp8CacheLayer), layer.group, layer.window
+    decode window with its heavy hitters."""
+    return isinstance(layer, PkvFp8CacheLayer), layer.group, layer.window, layer.heavy
 
 
 def _window_args(layer) -> dict:
-    """The decode-window state of a layer as `PkvBatchCacheLayer` keyword arguments."""
+    """The decode-window state of a layer (with its heavy-hitter state) as `PkvBatchCacheLayer` keyword arguments."""
     if layer.window is None:
         return {}
-    return dict(window=layer.window, prompt_rows=layer.prompt_rows_host, generated=layer.generated)
+    heavy = {} if layer.heavy is None else dict(heavy=layer.heavy, heavy_state=(layer.heavy_scores, layer.heavy_gen, layer.victim))
+    return dict(window=layer.window, prompt_rows=layer.prompt_rows_host, generated=layer.generated, **heavy)
 
 
 def join_caches(caches, reserve: int = 0):
@@ -504,10 +547,10 @@ def join_caches(caches, reserve: int = 0):
         raise RuntimeError("join_caches needs caches prefilled by the patched forward on every layer "
                            "(method 'fullkv' and stock caches are not compacted)")
     forms = {_form(l) for l in layers}
-    if len({window for _, _, window in forms}) > 1:
-        raise ValueError("join_caches: caches of different decode windows cannot be joined together (set pkv_decode_window the "
-                         "same for every prompt)")
-    if len({group for _, group, _ in forms}) > 1:
+    if len({form[2:] for form in forms}) > 1:
+        raise ValueError("join_caches: caches of different decode windows cannot be joined together (set pkv_decode_window and "
+                         "pkv_decode_heavy the same for every prompt)")
+    if len({form[1] for form in forms}) > 1:
         raise ValueError("join_caches: GQA-shared and per-query-head caches (or caches of different groups) cannot be joined "
                          "together (set pkv_gqa_shared the same for every prompt)")
     if len(forms) > 1:
@@ -538,6 +581,9 @@ def join_caches(caches, reserve: int = 0):
         win = {}
         if l0.window is not None:
             win = dict(window=l0.window, prompt_rows=[l.prompt_rows_host[0] for l in src], generated=[l.generated[0] for l in src])
+            if l0.heavy is not None:
+                win.update(heavy=l0.heavy, heavy_state=(torch.cat([l.heavy_scores for l in src]), torch.cat([l.heavy_gen for l in src]),
+                                                        torch.cat([l.victim for l in src])))
         out.layers.append(cls(*bufs, rows, [l.seq_seen[0] for l in src], l0.group, **win))
     return out
 

@@ -596,7 +596,7 @@ struct DecodeScales {
 // argument is checked.
 static int decode(const char* fn, const pkv_decode_desc* d, bool shared, const DecodeScales* scales, bool host_length, int32_t num_seqs,
                   int64_t cache_stride_b, const int32_t* rows, const int32_t* step_dev, int64_t max_length, void* stream,
-                  int64_t window = 0, const int32_t* prompt_rows = nullptr) {
+                  int64_t window = 0, const int32_t* prompt_rows = nullptr, const pkv_decode_heavy* heavy = nullptr) {
     int rc = host_length ? PKV_OK : check_devlen_args(fn, num_seqs, rows, step_dev, max_length);
     if (rc) return rc;
     if (scales && (!scales->k || !scales->v)) return fail(PKV_ERR_INVALID_ARG, "%s: null scale pointer", fn);
@@ -631,6 +631,15 @@ static int decode(const char* fn, const pkv_decode_desc* d, bool shared, const D
     a.step_dev = step_dev;
     a.window = window;
     a.prompt_rows = prompt_rows;
+    if (heavy) {
+        const uint64_t need = pkv_decode_heavy_workspace_bytes(num_seqs, a.Hq, window);
+        if (heavy->scratch_bytes < need) return fail(PKV_ERR_WORKSPACE, "%s: heavy scratch of %llu bytes required", fn, (unsigned long long)need);
+        a.victim = heavy->victim;
+        a.hv_scratch = static_cast<float*>(heavy->scratch);
+        a.hv_scores = heavy->scores;
+        a.hv_gen = heavy->gen;
+        a.heavy = heavy->heavy;
+    }
     DeviceGuard guard(d->device);
     const cudaError_t e = launch_decode(a, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, fn);
@@ -662,8 +671,8 @@ int pkv_decode_attn_batch_gqa_fp8(const pkv_decode_desc* d, int32_t num_seqs, in
     return decode("pkv_decode_attn_batch_gqa_fp8", d, true, &scales, false, num_seqs, cache_stride_b, rows, step_dev, max_length, stream);
 }
 
-int pkv_decode_attn_window(const pkv_decode_desc* d, const pkv_decode_window* w, void* stream) {
-    const char* fn = "pkv_decode_attn_window";
+// The checks of the window arguments, then the decode (with the heavy-hitter state when `h` is set).
+static int decode_window(const char* fn, const pkv_decode_desc* d, const pkv_decode_window* w, const pkv_decode_heavy* h, void* stream) {
     if (!w || w->struct_bytes != sizeof(pkv_decode_window))
         return fail(PKV_ERR_INVALID_ARG, "%s: null pkv_decode_window or struct_bytes != %zu (ABI mismatch)", fn, sizeof(pkv_decode_window));
     if (w->window < 1) return fail(PKV_ERR_INVALID_ARG, "%s: window=%lld must be >= 1", fn, (long long)w->window);
@@ -671,7 +680,29 @@ int pkv_decode_attn_window(const pkv_decode_desc* d, const pkv_decode_window* w,
     if ((w->k_scale == nullptr) != (w->v_scale == nullptr)) return fail(PKV_ERR_INVALID_ARG, "%s: null scale pointer", fn);
     const DecodeScales scales{w->k_scale, w->v_scale, w->scale_stride_h, w->scale_stride_b};
     return decode(fn, d, w->gqa_shared != 0, w->k_scale ? &scales : nullptr, false, w->num_seqs, w->cache_stride_b, w->rows,
-                  w->step_dev, w->max_length, stream, w->window, w->prompt_rows);
+                  w->step_dev, w->max_length, stream, w->window, w->prompt_rows, h);
+}
+
+int pkv_decode_attn_window(const pkv_decode_desc* d, const pkv_decode_window* w, void* stream) {
+    return decode_window("pkv_decode_attn_window", d, w, nullptr, stream);
+}
+
+uint64_t pkv_decode_heavy_workspace_bytes(int32_t num_seqs, int32_t num_q_heads, int64_t window) {
+    if (num_seqs < 1 || num_q_heads < 1 || window < 1) return 0;
+    return uint64_t(num_seqs) * uint64_t(num_q_heads) * uint64_t(window + 2) * sizeof(float);
+}
+
+int pkv_decode_attn_heavy(const pkv_decode_desc* d, const pkv_decode_window* w, const pkv_decode_heavy* h, void* stream) {
+    const char* fn = "pkv_decode_attn_heavy";
+    if (!h || h->struct_bytes != sizeof(pkv_decode_heavy))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null pkv_decode_heavy or struct_bytes != %zu (ABI mismatch)", fn, sizeof(pkv_decode_heavy));
+    if (w && w->struct_bytes == sizeof(pkv_decode_window) && (h->heavy < 0 || h->heavy >= w->window))
+        return fail(PKV_ERR_INVALID_ARG, "%s: heavy=%lld outside [0, window - 1 = %lld]", fn, (long long)h->heavy, (long long)w->window - 1);
+    if (d && (!d->k_new || !d->v_new)) return fail(PKV_ERR_INVALID_ARG, "%s: the heavy-hitter step appends a row: k_new / v_new required", fn);
+    const auto bad = [](const void* ptr) { return !ptr || (reinterpret_cast<uintptr_t>(ptr) & 3u); };
+    if (bad(h->scores) || bad(h->gen) || bad(h->victim) || bad(h->scratch))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned scores / gen / victim / scratch", fn);
+    return decode_window(fn, d, w, h, stream);
 }
 
 int pkv_cache_quantize_fp8(int32_t dtype, int32_t num_seqs, int32_t num_heads, int32_t head_dim, int32_t device, int32_t num_layers,

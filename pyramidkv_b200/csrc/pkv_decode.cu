@@ -35,7 +35,20 @@ struct DecodeParams {
     const int32_t* rows;      // + rows[s*(cache heads) + c] (rows of each sequence and cache head: joined prompts, AdaKV / HeadKV)
     int64_t window;           // decode window R (0: off): rows past prompt_rows[s*(cache heads) + c] form a ring of R rows
     const int32_t* prompt_rows;
+    // heavy-hitter window (pkv_decode_attn_heavy): the slot of the next row past a full window, the per-step scratch and the
+    // accumulated state (decode_heavy_kernel)
+    int32_t* victim;     // [num_seqs*(cache heads)] absolute row index
+    float* hv_logit;     // [num_seqs*Hq][window] s of each attended generated row (index row - P)
+    float* hv_ml;        // [num_seqs*Hq][2] (m, l) the output of the step is normalised by
+    float* hv_scores;    // [num_seqs*(cache heads)][window] accumulated attention A of the row in each slot
+    int32_t* hv_gen;     // [num_seqs*(cache heads)][window] generation index of the row in each slot
+    int64_t heavy;       // H: rows past the R - H most recent that may stay
+    int heads_per_cache;
 };
+
+// Decode window modes (template parameter of decode_kernel): none, the ring (oldest row replaced) and heavy hitters (the
+// row decode_heavy_kernel chose replaced).
+enum WindowMode { kNoWindow = 0, kRing = 1, kHeavy = 2 };
 
 // Row formats. A lane holds kElems elements of a row (one 128-bit load). score() and weight() give the softmax input of a
 // row and the factor of its V elements, with the roundings the fp32 online softmax below is defined by.
@@ -69,11 +82,15 @@ struct RowsE4M3 {   // E4M3 rows with one fp32 scale per row for K and for V (pk
 // the launch was checked against) is treated as 0: nothing is read or written but the output, which becomes NaN.
 // With a decode window (window > 0, pkv_decode_attn_window) the count n past P = prompt_rows[...] wraps: once n > P + window
 // the new row goes to P + (n-1-P) mod window and P + window rows are attended, with the split rule of that count.
+// Heavy mode (pkv_decode_attn_heavy) goes to victim[s*(cache heads) + c] instead (a victim outside [P, P + window) is treated
+// as an out-of-range count), stores the softmax input s of every attended generated row r >= P and query head (the lane of
+// piece 0, which holds the reduced dot) at hv_logit[head][r - P], and with nsplit == 1 the (m, l) the output is divided by
+// at hv_ml[head] (decode_combine_kernel stores them otherwise). The output arithmetic is the ring's.
 //
 // Registers: the GH = 1 forms must stay within the ceilings of their occupancy, 80 per thread for 16-bit rows (3 CTAs per
-// SM; 64-79 now) and 128 for E4M3 rows (2 CTAs per SM; at 128 now, no headroom). ptxas -v prints the counts. The window is a
-// template parameter so that the launches without one keep the code (and the speed) they had before it existed.
-template <typename T, int D, typename Rows, int GH, bool kWindow>
+// SM; 64-79 now) and 128 for E4M3 rows (2 CTAs per SM; at 128 now, no headroom). ptxas -v prints the counts. The window mode
+// is a template parameter so that the launches without one keep the code (and the speed) they had before it existed.
+template <typename T, int D, typename Rows, int GH, int kMode>
 __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodeParams p) {
     using Elem = typename Rows::Elem;
     constexpr int E = Rows::kElems;
@@ -102,17 +119,27 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
     if (p.step_dev) rows += int64_t(__ldg(p.step_dev));
     if (p.rows) rows += int64_t(__ldg(p.rows + sc));
     int64_t ring_row = rows - 1;
-    if constexpr (kWindow) {
-        // decode window: the prompt's P rows stay, appended row j (= n-1-P) lives at P + j mod R, and P + R rows are
-        // attended once the ring is full (before that the rows are those of the unwindowed launch)
+    [[maybe_unused]] int64_t P = 0;
+    if constexpr (kMode != kNoWindow) {
+        // decode window: the prompt's P rows stay, appended row j (= n-1-P) lives at P + j mod R (heavy: at the victim), and
+        // P + R rows are attended once the window is full (before that the rows are those of the unwindowed launch)
         if (rows >= 1) {
-            const int64_t P = int64_t(__ldg(p.prompt_rows + sc));
-            if (P < 0) rows = 0;
-            else if (rows > P + p.window) { ring_row = P + (rows - 1 - P) % p.window; rows = P + p.window; }
+            P = int64_t(__ldg(p.prompt_rows + sc));
+            if (P < 0) {
+                rows = 0;
+            } else if (rows > P + p.window) {
+                if constexpr (kMode == kHeavy) {
+                    ring_row = int64_t(p.victim[sc]);
+                    rows = (ring_row >= P && ring_row < P + p.window) ? P + p.window : 0;
+                } else {
+                    ring_row = P + (rows - 1 - P) % p.window;
+                    rows = P + p.window;
+                }
+            }
         }
     }
     if (rows < 1 || rows > p.max_rows) rows = 0;
-    const int64_t new_row = kWindow ? ring_row : rows - 1;
+    const int64_t new_row = kMode != kNoWindow ? ring_row : rows - 1;
     const int64_t ns = min(int64_t(p.nsplit), decode_splits_for(p.Hq, rows, p.num_sms));
     const int64_t chunk = (rows + ns - 1) / ns;
     const int64_t r_begin = int64_t(split) * chunk;
@@ -208,6 +235,10 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
                     // Explicit roundings, so that the compiler cannot contract differently for different GH (a*b + c*d around
                     // either product, or dot * scale into s - mn): every head gets the bits of its per-query-head cache.
                     const float s = Rows::score(dot, ks[u], p.scale);
+                    if constexpr (kMode == kHeavy) {   // (32-bit: a row index fits, and the E4M3 GH = 4 form has no registers to spare)
+                        const int rel = int(rb - P) + sub + u * kDecodeWarps * RPW;   // generated row rel = r - P
+                        if (piece == 0 && rel >= 0) p.hv_logit[(sh0 + i) * p.window + rel] = s;
+                    }
                     const float mn = fmaxf(m[i], s);
                     const float corr = expf(m[i] - mn), pe = expf(s - mn);
                     l[i] = __fmaf_rn(l[i], corr, pe);
@@ -258,6 +289,9 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
         }
         if (p.nsplit == 1) {
             p.out[(sh0 + i) * D + d] = DT<T>::from_f32(at / lt);
+            if constexpr (kMode == kHeavy) {
+                if (d == 0) { p.hv_ml[2 * (sh0 + i)] = mn; p.hv_ml[2 * (sh0 + i) + 1] = lt; }
+            }
         } else {
             float* w = p.ws + ((sh0 + i) * p.nsplit + split) * (2 + D);
             if (d == 0) { w[0] = mn; w[1] = lt; }
@@ -266,7 +300,7 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_kernel(const DecodePara
     }
 }
 
-template <typename T, int D>
+template <typename T, int D, bool kHeavy>
 __global__ void decode_combine_kernel(const DecodeParams p) {   // one CTA per (sequence, head)
     const int64_t h = blockIdx.x;
     const int d = threadIdx.x;
@@ -281,6 +315,89 @@ __global__ void decode_combine_kernel(const DecodeParams p) {   // one CTA per (
         at += w[s * (2 + D) + 2 + d] * c;
     }
     p.out[h * D + d] = DT<T>::from_f32(at / lt);
+    if constexpr (kHeavy) {
+        if (d == 0) { p.hv_ml[2 * h] = mn; p.hv_ml[2 * h + 1] = lt; }
+    }
+}
+
+// 512 threads: one pass over the slots of a window up to 512 rows. The kernel is latency-bound (a few dependent loads per
+// slot), so each thread issues all of its slot's loads before the arithmetic.
+constexpr int kHeavyThreads = 512;
+constexpr int kHeavyMaxGroup = 8;   // query heads per cache head: 1, or a GQA group of 2, 4 or 8
+
+// (A, generation index) of a victim candidate; the smaller A wins, ties go to the smaller generation index. A total order on
+// the distinct generation indices, so the reduction order does not change the winner.
+struct HeavyPick {
+    float a;
+    int32_t g, slot;
+};
+__device__ __forceinline__ bool heavy_before(const HeavyPick& x, const HeavyPick& y) { return x.a < y.a || (x.a == y.a && x.g < y.g); }
+
+// The heavy-hitter bookkeeping of one decode step, after the decode (and combine) launch: one CTA per (sequence, cache head).
+// With n, P and the appended slot as decode_kernel derived them (the same out-of-range rule: nothing is written), the row
+// appended as generation j = n-1-P starts from A = 0 with gen = j; every held generated row (slots [0, min(j+1, R)) past P)
+// adds sum_h expf(s - m_h) / l_h over the query heads reading this cache head, in ascending head order, in fp32; and when the
+// next step's count n + 1 exceeds P + R, victim = P + the slot of the smallest A among the rows of generation index
+// <= j + 1 - (R - H). Each thread owns whole slots, so every value is one fixed sequence of fp32 operations: no atomics.
+__global__ void __launch_bounds__(kHeavyThreads) decode_heavy_kernel(const DecodeParams p) {
+    __shared__ HeavyPick s_best[kHeavyThreads / 32];
+    const int64_t sc = blockIdx.x;
+    const int heads = p.Hq / p.heads_per_cache;   // cache heads per sequence
+    const int64_t sh0 = (sc / heads) * p.Hq + (sc % heads) * p.heads_per_cache;
+    int64_t n = p.T;
+    if (p.step_dev) n += int64_t(__ldg(p.step_dev));
+    if (p.rows) n += int64_t(__ldg(p.rows + sc));
+    const int64_t P = int64_t(__ldg(p.prompt_rows + sc)), R = p.window;
+    if (n < 1 || P < 0 || n <= P || min(n, P + R) > p.max_rows) return;   // out of range, or an append inside the prompt
+    const int64_t slot = n > P + R ? int64_t(p.victim[sc]) : n - 1;
+    if (slot < P || slot >= P + R) return;
+    const int64_t j = n - 1 - P, held = min(j + 1, R), k_new = slot - P;
+    const bool pick = j + 1 >= R;
+    const int64_t last = j + 1 - (R - p.heavy);   // the candidates' largest generation index
+    float* A = p.hv_scores + sc * R;
+    int32_t* gen = p.hv_gen + sc * R;
+    HeavyPick best{INFINITY, INT32_MAX, -1};
+    float m[kHeavyMaxGroup], l[kHeavyMaxGroup];
+#pragma unroll
+    for (int h = 0; h < kHeavyMaxGroup; ++h) {
+        if (h < p.heads_per_cache) { m[h] = p.hv_ml[2 * (sh0 + h)]; l[h] = p.hv_ml[2 * (sh0 + h) + 1]; }
+    }
+    for (int64_t k = threadIdx.x; k < held; k += kHeavyThreads) {
+        float s[kHeavyMaxGroup];
+#pragma unroll
+        for (int h = 0; h < kHeavyMaxGroup; ++h) {
+            if (h < p.heads_per_cache) s[h] = p.hv_logit[(sh0 + h) * R + k];
+        }
+        float a = 0.f;
+        int32_t g = int32_t(j);
+        if (k == k_new) gen[k] = g;
+        else { a = A[k]; g = gen[k]; }
+        float sum = 0.f;   // ascending head order
+#pragma unroll
+        for (int h = 0; h < kHeavyMaxGroup; ++h) {
+            if (h < p.heads_per_cache) sum = __fadd_rn(sum, __fdiv_rn(expf(__fsub_rn(s[h], m[h])), l[h]));
+        }
+        a = __fadd_rn(a, sum);
+        A[k] = a;
+        const HeavyPick c{a, g, int32_t(k)};
+        if (pick && g <= last && heavy_before(c, best)) best = c;
+    }
+    if (!pick) return;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        HeavyPick c;
+        c.a = __shfl_xor_sync(0xffffffffu, best.a, o);
+        c.g = __shfl_xor_sync(0xffffffffu, best.g, o);
+        c.slot = __shfl_xor_sync(0xffffffffu, best.slot, o);
+        if (heavy_before(c, best)) best = c;
+    }
+    if ((threadIdx.x & 31) == 0) s_best[threadIdx.x >> 5] = best;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < kHeavyThreads / 32; ++w)
+            if (heavy_before(s_best[w], best)) best = s_best[w];
+        p.victim[sc] = best.slot < 0 ? -1 : int32_t(P + best.slot);   // -1 (no candidate: A is NaN): the next step is out of range
+    }
 }
 
 template <int D>
@@ -310,41 +427,52 @@ DecodeParams make_params(const DecodeArgs& a) {
     p.rows = a.rows;
     p.window = a.window;
     p.prompt_rows = a.prompt_rows;
+    p.victim = a.victim;
+    p.hv_logit = a.hv_scratch;
+    p.hv_ml = a.hv_scratch ? a.hv_scratch + int64_t(a.num_seqs) * a.Hq * a.window : nullptr;
+    p.hv_scores = a.hv_scores;
+    p.hv_gen = a.hv_gen;
+    p.heavy = a.heavy;
+    p.heads_per_cache = a.heads_per_cache;
     return p;
 }
 
-template <typename T, int D, typename Rows, bool kWindow>
+template <typename T, int D, typename Rows, int kMode>
 cudaError_t launch_decode_t(const DecodeArgs& a, cudaStream_t st) {
     const DecodeParams p = make_params(a);
     // query heads per CTA: 1 on a cache per query head; on a shared cache the whole group, for E4M3 at most 4 (the registers
     // of eight heads do not fit)
     const int GH = a.heads_per_cache == 1 ? 1 : Rows::kE4M3 ? min(a.G, 4) : a.G;
     const dim3 grid(unsigned(a.nsplit), unsigned(a.Hq / GH), unsigned(a.num_seqs));
-    if (GH == 1) decode_kernel<T, D, Rows, 1, kWindow><<<grid, kDecodeThreads, 0, st>>>(p);
-    else if (GH == 2) decode_kernel<T, D, Rows, 2, kWindow><<<grid, kDecodeThreads, 0, st>>>(p);
-    else if (GH == 4) decode_kernel<T, D, Rows, 4, kWindow><<<grid, kDecodeThreads, 0, st>>>(p);
+    if (GH == 1) decode_kernel<T, D, Rows, 1, kMode><<<grid, kDecodeThreads, 0, st>>>(p);
+    else if (GH == 2) decode_kernel<T, D, Rows, 2, kMode><<<grid, kDecodeThreads, 0, st>>>(p);
+    else if (GH == 4) decode_kernel<T, D, Rows, 4, kMode><<<grid, kDecodeThreads, 0, st>>>(p);
     else if (!Rows::kE4M3 && GH == 8) {
-        if constexpr (!Rows::kE4M3) decode_kernel<T, D, Rows, 8, kWindow><<<grid, kDecodeThreads, 0, st>>>(p);
+        if constexpr (!Rows::kE4M3) decode_kernel<T, D, Rows, 8, kMode><<<grid, kDecodeThreads, 0, st>>>(p);
     } else {
         return cudaErrorInvalidValue;   // no instantiation for this group size
     }
     count_launch();
     if (a.nsplit > 1) {
-        decode_combine_kernel<T, D><<<unsigned(int64_t(a.num_seqs) * a.Hq), D, 0, st>>>(p);
+        decode_combine_kernel<T, D, kMode == kHeavy><<<unsigned(int64_t(a.num_seqs) * a.Hq), D, 0, st>>>(p);
+        count_launch();
+    }
+    if constexpr (kMode == kHeavy) {
+        decode_heavy_kernel<<<unsigned(int64_t(a.num_seqs) * (a.Hq / a.heads_per_cache)), kHeavyThreads, 0, st>>>(p);
         count_launch();
     }
     return cudaGetLastError();
 }
 
-template <typename T, int D, bool kWindow>
+template <typename T, int D, int kMode>
 cudaError_t launch_decode_rows(const DecodeArgs& a, cudaStream_t st) {
-    return a.k_scale ? launch_decode_t<T, D, RowsE4M3, kWindow>(a, st) : launch_decode_t<T, D, Rows16<T>, kWindow>(a, st);
+    return a.k_scale ? launch_decode_t<T, D, RowsE4M3, kMode>(a, st) : launch_decode_t<T, D, Rows16<T>, kMode>(a, st);
 }
 
-template <bool kWindow>
+template <int kMode>
 cudaError_t launch_decode_w(const DecodeArgs& a, cudaStream_t st) {
-    if (a.dtype == PKV_BF16) return a.D == 128 ? launch_decode_rows<__nv_bfloat16, 128, kWindow>(a, st) : launch_decode_rows<__nv_bfloat16, 64, kWindow>(a, st);
-    return a.D == 128 ? launch_decode_rows<__half, 128, kWindow>(a, st) : launch_decode_rows<__half, 64, kWindow>(a, st);
+    if (a.dtype == PKV_BF16) return a.D == 128 ? launch_decode_rows<__nv_bfloat16, 128, kMode>(a, st) : launch_decode_rows<__nv_bfloat16, 64, kMode>(a, st);
+    return a.D == 128 ? launch_decode_rows<__half, 128, kMode>(a, st) : launch_decode_rows<__half, 64, kMode>(a, st);
 }
 
 }  // namespace
@@ -352,7 +480,8 @@ cudaError_t launch_decode_w(const DecodeArgs& a, cudaStream_t st) {
 int decode_num_splits(int Hq, int64_t T, int num_sms) { return int(decode_splits_for(Hq, T, num_sms)); }
 
 cudaError_t launch_decode(const DecodeArgs& a, cudaStream_t st) {
-    return a.window > 0 ? launch_decode_w<true>(a, st) : launch_decode_w<false>(a, st);
+    if (a.victim) return launch_decode_w<kHeavy>(a, st);
+    return a.window > 0 ? launch_decode_w<kRing>(a, st) : launch_decode_w<kNoWindow>(a, st);
 }
 
 cudaError_t launch_append(const DecodeArgs& a, cudaStream_t st) {

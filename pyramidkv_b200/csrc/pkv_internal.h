@@ -132,6 +132,13 @@ struct DecodeArgs {
     // P = prompt_rows[s*(cache heads) + c], is stored at P + (n-1-P) mod window and P + window rows are attended
     int64_t window = 0;
     const int32_t* prompt_rows = nullptr;
+    // heavy-hitter window (pkv_decode_attn_heavy) when victim is set: past P + window the new row goes to victim[s*(cache
+    // heads) + c], and decode_heavy_kernel updates the state and picks the next victim. hv_scratch: [num_seqs*Hq][window]
+    // logits then [num_seqs*Hq][2] (m, l)
+    int32_t* victim = nullptr;
+    float *hv_scratch = nullptr, *hv_scores = nullptr;
+    int32_t* hv_gen = nullptr;
+    int64_t heavy = 0;
 };
 // split count for T rows (decode_num_splits); shared by the launch and the decode kernel
 __host__ __device__ inline int64_t decode_splits_for(int64_t Hq, int64_t T, int64_t num_sms) {

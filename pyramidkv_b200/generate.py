@@ -158,6 +158,7 @@ def _backend(model):
 class _StaticState:
     step: torch.Tensor        # int32 [1]: decode steps already taken in this static run (read by the decode kernel)
     workspace: torch.Tensor   # split-T partials, shared by all layers (launches are stream-ordered)
+    heavy_scratch: Optional[torch.Tensor] = None   # knob pkv_decode_heavy: the per-step logits, shared by all layers
 
 
 class StaticDecoder:
@@ -209,6 +210,8 @@ class StaticDecoder:
         self.backend = model.model.layers[0].self_attn.kv_cluster.backend
         self.state = _StaticState(step=torch.zeros(1, dtype=torch.int32, device=dev),
                                   workspace=self.backend.decode_workspace(bsz * layers[0].num_q_heads, layers[0].k_buf.shape[3], dev))
+        if layers[0].heavy is not None:
+            self.state.heavy_scratch = self.backend.decode_heavy_workspace(bsz, layers[0].num_q_heads, layers[0].window, dev)
         self.ids = first_token.reshape(bsz, 1).to(device=dev, dtype=torch.long).clone()
         self.pos = torch.tensor(layers[0].seq_seen, dtype=torch.long, device=dev).reshape(bsz, 1)
         self.cursor = torch.zeros(1, dtype=torch.long, device=dev)
@@ -278,8 +281,10 @@ class StaticDecoder:
     def _counters(self) -> list:
         """The device tensors a step advances (restored after the warm-up step of a capture)."""
         idx = self.sampling.index if self.sampling is not None else None
+        # the heavy-hitter state a step updates (knob pkv_decode_heavy): restored so that the captured step starts from it
+        heavy = [t for l in self.layers if l.heavy is not None for t in (l.heavy_scores, l.heavy_gen, l.victim)]
         return [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done, idx, self.window_rows)
-                if t is not None]
+                if t is not None] + heavy
 
     def _capture(self) -> None:
         # warm up on a side stream (lazy initialisation, cuBLAS workspaces), restore the counters, then capture

@@ -96,6 +96,16 @@ class CudaBackend:
         return ops.decode_attn_window(q, k_buf, v_buf, length, k_new, v_new, prompt_rows, window, rows, step, max_length,
                                       workspace, out, softmax_scale, scales, gqa)
 
+    # -- heavy hitters in the decode window (model.config.pkv_decode_heavy = H): the least-attended generated row leaves --
+    def decode_attn_heavy(self, q, k_buf, v_buf, length, k_new, v_new, prompt_rows, window, heavy, scores, gen, victim, rows=None,
+                          step=None, max_length=0, workspace=None, scratch=None, out=None, softmax_scale=0.0, scales=None,
+                          gqa=False):
+        return ops.decode_attn_heavy(q, k_buf, v_buf, length, k_new, v_new, prompt_rows, window, heavy, scores, gen, victim, rows,
+                                     step, max_length, workspace, scratch, out, softmax_scale, scales, gqa)
+
+    def decode_heavy_workspace(self, num_seqs, num_q_heads, window, device):
+        return torch.empty(ops.decode_heavy_workspace_bytes(num_seqs, num_q_heads, window), dtype=torch.uint8, device=device)
+
     # -- continuous batching: one prompt's compacted cache into one slot of a batched cache --
     def cache_install(self, layers, slot, step):
         ops.cache_install(layers, slot, step)

@@ -10,7 +10,7 @@ from typing import Dict, Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import METHODS, POOLING, SCORE_KERNELS, DecodeDesc, DecodeWindow, EvictDesc, RopeDesc, WsLayout
+from ._lib import METHODS, POOLING, SCORE_KERNELS, DecodeDesc, DecodeHeavy, DecodeWindow, EvictDesc, RopeDesc, WsLayout
 
 _DTYPES = {torch.bfloat16: 0, torch.float16: 1}
 
@@ -431,11 +431,13 @@ def decode_attn_batch(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor,
 
 
 def _decode_batch(entry, what, q, k_buf, v_buf, scales, length, k_new, v_new, rows, step, max_length, workspace, out,
-                  softmax_scale, gqa: bool = False, window: int = 0, prompt_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
+                  softmax_scale, gqa: bool = False, window: int = 0, prompt_rows: Optional[torch.Tensor] = None,
+                  heavy=None) -> torch.Tensor:
     """The checks and the descriptor of the batched decode launches, then the launch of the C entry point `entry`.
     `scales`: (k_scale, v_scale) of an FP8 cache, or None. `gqa`: a GQA-shared cache (k_buf / v_buf [B, Hkv, capacity, D],
-    q [B, Hq, D]). `window` > 0: the decode window over `prompt_rows` (`pkv_decode_attn_window`)."""
-    _require_cuda(q, k_buf, v_buf, k_new, v_new, rows, step, workspace, out, prompt_rows, *(scales or ()))
+    q [B, Hq, D]). `window` > 0: the decode window over `prompt_rows` (`pkv_decode_attn_window`); with `heavy` = (H, scores,
+    gen, victim, scratch) its heavy hitters (`pkv_decode_attn_heavy`)."""
+    _require_cuda(q, k_buf, v_buf, k_new, v_new, rows, step, workspace, out, prompt_rows, *(scales or ()), *(heavy or ())[1:])
     if scales is not None:
         _check_fp8_buffers(k_buf, v_buf, scales[0], scales[1], what)
     elif k_buf.dim() != 4 or k_buf.shape != v_buf.shape or k_buf.stride() != v_buf.stride() or k_buf.stride(3) != 1 \
@@ -508,7 +510,22 @@ def _decode_batch(entry, what, q, k_buf, v_buf, scales, length, k_new, v_new, ro
         if scales is not None:
             w.k_scale, w.v_scale = scales[0].data_ptr(), scales[1].data_ptr()
             w.scale_stride_h, w.scale_stride_b = scales[0].stride(1), scales[0].stride(0)
-        _lib.check(_lib.lib().pkv_decode_attn_window(C.byref(d), C.byref(w), torch.cuda.current_stream(q.device).cuda_stream))
+        stream = torch.cuda.current_stream(q.device).cuda_stream
+        if heavy is not None:
+            H_, scores, gen, victim, scratch = heavy
+            for t, dt, n in ((scores, torch.float32, B * H * window), (gen, torch.int32, B * H * window), (victim, torch.int32, B * H)):
+                if t.dtype != dt or t.numel() != n or not t.is_contiguous():
+                    raise ValueError(f"{what}: scores / gen / victim must be contiguous {dt} device tensors of {n} elements")
+            if scratch is None:
+                scratch = _heavy_scratch(q.device, decode_heavy_workspace_bytes(B, Hq, window))
+            hv = DecodeHeavy()
+            hv.struct_bytes = C.sizeof(DecodeHeavy)
+            hv.heavy = int(H_)
+            hv.scores, hv.gen, hv.victim = scores.data_ptr(), gen.data_ptr(), victim.data_ptr()
+            hv.scratch, hv.scratch_bytes = scratch.data_ptr(), scratch.numel() * scratch.element_size()
+            _lib.check(_lib.lib().pkv_decode_attn_heavy(C.byref(d), C.byref(w), C.byref(hv), stream))
+        else:
+            _lib.check(_lib.lib().pkv_decode_attn_window(C.byref(d), C.byref(w), stream))
         return out
     args = (C.byref(d), B, k_buf.stride(0), rows.data_ptr() if rows is not None else None,
             step.data_ptr() if step is not None else None, max_length)
@@ -628,6 +645,47 @@ def decode_attn_window(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor
         raise ValueError(f"decode_attn_window: window={window} must be >= 1")
     return _decode_batch("pkv_decode_attn_window", "decode_attn_window", q, k_buf, v_buf, scales, length, k_new, v_new, rows, step, max_length, workspace, out,
                          softmax_scale, gqa=gqa, window=int(window), prompt_rows=prompt_rows)
+
+
+# ---- the heavy-hitter decode window (include/pkv.h: pkv_decode_attn_heavy) ----
+_heavy_scratches: Dict[Tuple[int, int], torch.Tensor] = {}
+
+
+def _heavy_scratch(device: torch.device, nbytes: int) -> torch.Tensor:
+    """The per-step logit and (m, l) scratch of a host-launched heavy step: one growing buffer per (device, stream), like
+    `_workspace` (the static loops pass their own, which a captured graph keeps)."""
+    key = (device.index if device.index is not None else torch.cuda.current_device(),
+           torch.cuda.current_stream(device).cuda_stream)
+    t = _heavy_scratches.get(key)
+    if t is None or t.numel() < nbytes:
+        t = torch.empty(max(nbytes, 1 << 16), dtype=torch.uint8, device=device)
+        _heavy_scratches[key] = t
+    return t
+
+
+def decode_heavy_workspace_bytes(num_seqs: int, num_q_heads: int, window: int) -> int:
+    """Bytes of the per-step scratch of `decode_attn_heavy` (`pkv_decode_heavy_workspace_bytes`)."""
+    return int(_lib.lib().pkv_decode_heavy_workspace_bytes(int(num_seqs), int(num_q_heads), int(window)))
+
+
+def decode_attn_heavy(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor, length: int, k_new: torch.Tensor,
+                      v_new: torch.Tensor, prompt_rows: torch.Tensor, window: int, heavy: int, scores: torch.Tensor,
+                      gen: torch.Tensor, victim: torch.Tensor, rows: Optional[torch.Tensor] = None,
+                      step: Optional[torch.Tensor] = None, max_length: int = 0, workspace: Optional[torch.Tensor] = None,
+                      scratch: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, softmax_scale: float = 0.0,
+                      scales=None, gqa: bool = False) -> torch.Tensor:
+    """`decode_attn_window` whose full window replaces the generated row with the least accumulated attention instead of
+    the oldest, keeping the R - H most recent rows (`pkv_decode_attn_heavy`, include/pkv.h). `heavy` = H in [0, R - 1];
+    `scores` fp32, `gen` int32 (each [B, H_cache, R]) and `victim` int32 [B*H_cache] are the layer's state, updated in
+    place; `scratch` (uint8, `decode_heavy_workspace_bytes(B, Hq, R)` bytes; default: a buffer per stream) holds the
+    per-step logits, shared by every layer. Graph-replayable. Returns out [B, Hq, D]."""
+    if int(window) < 1 or not 0 <= int(heavy) < int(window):
+        raise ValueError(f"decode_attn_heavy: window={window}, heavy={heavy}: expected window >= 1 and 0 <= heavy < window")
+    if k_new is None or v_new is None:
+        raise ValueError("decode_attn_heavy: the step appends a row: k_new and v_new are required")
+    return _decode_batch("pkv_decode_attn_heavy", "decode_attn_heavy", q, k_buf, v_buf, scales, length, k_new, v_new, rows, step,
+                         max_length, workspace, out, softmax_scale, gqa=gqa, window=int(window), prompt_rows=prompt_rows,
+                         heavy=(int(heavy), scores, gen, victim, scratch))
 
 
 # ---- continuous batching: admission into one slot of a batched cache (include/pkv.h: pkv_cache_install) ----

@@ -100,7 +100,7 @@ class PipelineRunner:
         if getattr(stage.config, "pkv_gqa_shared", False):
             raise NotImplementedError("the GQA-shared cache (pkv_gqa_shared) is installed in the batched row-count form that the "
                                       "layer-sliced pipeline does not decode; it keeps the per-query-head cache")
-        if getattr(stage.config, "pkv_decode_window", None) is not None:
+        if getattr(stage.config, "pkv_decode_window", None) is not None or getattr(stage.config, "pkv_decode_heavy", None) is not None:
             raise NotImplementedError("the decode window (pkv_decode_window) holds every layer in the batched row-count form "
                                       "that the layer-sliced pipeline does not decode")
         self.stage, self.group = stage, group

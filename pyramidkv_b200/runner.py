@@ -316,7 +316,7 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
               backend_factory: Optional[Callable] = None, out_path: Optional[str] = None, tag: Optional[dict] = None,
               decode_loop: str = "hf", floor: float = 0.2, head_beta: float = 1.01, head_path: str = "",
               capacity_ratio: float = -1, eval_batch_size: int = 1, kv_cache_dtype: str = "auto",
-              gqa_shared: bool = False, decode_window: Optional[int] = None) -> List[dict]:
+              gqa_shared: bool = False, decode_window: Optional[int] = None, decode_heavy: Optional[int] = None) -> List[dict]:
     """prompts: iterable of (name, prompt_tokens, max_new_tokens). One JSON record per prompt (also appended to out_path).
     eval_batch_size N > 1: consecutive prompts with the same max_new_tokens are decoded N at a time (static loops only;
     each prompt is still prefilled alone, so its prefill_ms, cache rows and tokens are its own).
@@ -326,6 +326,8 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
     "gqa_shared". FullKV, AdaKV and HeadKV refuse it.
     decode_window R: each sequence keeps its compacted prompt plus its last R decoded tokens (model.config.pkv_decode_window);
     the records then carry "decode_window". FullKV refuses it.
+    decode_heavy H (with decode_window R): the window keeps its R - H most recent decoded tokens and, of the others, those
+    with the most accumulated attention (model.config.pkv_decode_heavy); the records then carry "decode_heavy".
     decode_loop "continuous": every prompt goes through one greedy_generate_continuous with eval_batch_size slots, whatever
     its max_new_tokens; each record keeps its own prefill_ms, cache rows and tokens and carries the run's "continuous" block
     (slots, decode_steps, occupancy, aggregate_tok_per_s) instead of a per-prompt decode rate."""
@@ -339,6 +341,8 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
                                   + ("keeps HF's own cache" if canonical_method(method) == "fullkv" else "sets budgets per query head"))
     if decode_window is not None and canonical_method(method) == "fullkv":
         raise NotImplementedError("--decode_window bounds the compacted cache of an eviction method; FullKV keeps HF's own cache")
+    if decode_heavy is not None and canonical_method(method) == "fullkv":
+        raise NotImplementedError("--decode_heavy chooses the rows of the decode window; FullKV keeps HF's own cache")
     if eval_batch_size < 1:
         raise ValueError(f"eval_batch_size must be >= 1, got {eval_batch_size}")
     continuous = decode_loop == "continuous"
@@ -368,6 +372,10 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
             from .cache import decode_window as decode_window_knob
             model.config.pkv_decode_window = decode_window
             decode_window_knob(model.config)           # rejects a bad value before any prompt runs
+        if decode_heavy is not None:
+            from .cache import decode_heavy as decode_heavy_knob
+            model.config.pkv_decode_heavy = decode_heavy
+            decode_heavy_knob(model.config)            # rejects a bad value (or a missing window) before any prompt runs
         records = []
         prompts = list(prompts)
         if (eval_batch_size > 1 or continuous) and max_capacity_prompt == -1 and capacity_ratio != -1 and len({p[1] for p in prompts}) > 1:
@@ -381,6 +389,7 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
                        **({"kv_cache_dtype": kv_cache_dtype} if kv_cache_dtype != "auto" else {}),
                        **({"gqa_shared": True} if gqa_shared else {}),
                        **({"decode_window": int(decode_window)} if decode_window is not None else {}),
+                       **({"decode_heavy": int(decode_heavy)} if decode_heavy is not None else {}),
                        "dtype": str(dtype).replace("torch.", ""), "data": "synthetic token ids, random-init weights", **(tag or {}),
                        "prompt_tokens": r.prompt_tokens, "new_tokens": r.new_tokens, "prefill_ms": r.prefill_ms,
                        **({} if continuous else {"decode_tok_per_s": r.decode_tok_per_s}), **extra,

@@ -64,6 +64,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--decode_window", type=int, default=None,
                    help="keep each sequence's cache at its compacted prompt plus its last R decoded tokens (fixed memory for "
                         "any generation length); default: every decoded token stays")
+    p.add_argument("--decode_heavy", type=int, default=None,
+                   help="with --decode_window R: keep the R - H most recent decoded tokens and, in the other H slots, the "
+                        "tokens with the most accumulated attention (H2O heavy hitters, 1 <= H <= R - 1); default: the "
+                        "oldest token leaves")
     return p
 
 
@@ -98,7 +102,7 @@ def main(argv=None, backend_factory=None, device=None):
                             floor=args.floor, head_beta=args.head_beta, head_path=args.head_path,
                             capacity_ratio=args.max_capacity_prompts_ratio, eval_batch_size=args.eval_batch_size,
                             kv_cache_dtype=args.kv_cache_dtype, gqa_shared=args.gqa_shared,
-                            decode_window=args.decode_window)
+                            decode_window=args.decode_window, decode_heavy=args.decode_heavy)
     n = len(recs)
     print(json.dumps({"summary": True, "arch": arch, "method": method, "max_capacity_prompts": capacity, "examples": n,
                       "mean_prefill_ms": sum(r["prefill_ms"] for r in recs) / n,

@@ -47,6 +47,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--decode_window", type=int, default=None,
                    help="keep each sequence's cache at its compacted prompt plus its last R decoded tokens (fixed memory for "
                         "any generation length); default: every decoded token stays")
+    p.add_argument("--decode_heavy", type=int, default=None,
+                   help="with --decode_window R: keep the R - H most recent decoded tokens and, in the other H slots, the "
+                        "tokens with the most accumulated attention (H2O heavy hitters, 1 <= H <= R - 1); default: the "
+                        "oldest token leaves")
     return p
 
 
@@ -64,7 +68,7 @@ def main(argv=None, backend_factory=None, device=None):
     recs = runner.run_suite(arch, args.method, args.max_capacity_prompt, prompts, device=device, dtype=getattr(torch, args.dtype),
                             attn_implementation=args.attn_implementation, backend_factory=backend_factory, out_path=out,
                             tag={"runner": "needle"}, decode_loop=args.decode_loop, kv_cache_dtype=args.kv_cache_dtype, gqa_shared=args.gqa_shared,
-                            decode_window=args.decode_window)
+                            decode_window=args.decode_window, decode_heavy=args.decode_heavy)
     print(json.dumps({"summary": True, "arch": arch, "method": runner.canonical_method(args.method),
                       "max_capacity_prompt": args.max_capacity_prompt, "contexts": [r["prompt_tokens"] for r in recs],
                       "prefill_ms": [round(r["prefill_ms"], 3) for r in recs],

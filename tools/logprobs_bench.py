@@ -110,13 +110,14 @@ def loop_numbers(model, dev, prompt_len, steps=64):
     return out
 
 
-def _knobs(model, budget, fp8=False, gqa=False, window=None):
+def _knobs(model, budget, fp8=False, gqa=False, window=None, heavy=None):
     for layer in model.model.layers:                               # run_longbench.py:253-261
         c = layer.self_attn.config
         c.window_size, c.max_capacity_prompt, c.kernel_size, c.pooling = 8, budget, 7, "maxpool"
     model.config.pkv_kv_cache_dtype = "fp8_e4m3" if fp8 else None
     model.config.pkv_gqa_shared = bool(gqa)
     model.config.pkv_decode_window = window
+    model.config.pkv_decode_heavy = heavy
 
 
 def _diff(e, ref_lp, ref_top1):
@@ -147,7 +148,8 @@ def fidelity(model, dev, n_prompts, prompt_len, cont_len, budgets):
     with contextlib.redirect_stdout(io.StringIO()):
         replace_llama("pyramidkv")
     forms = [("bf16", {}), ("fp8", dict(fp8=True)), ("gqa_shared", dict(gqa=True)), ("gqa_shared_fp8", dict(fp8=True, gqa=True)),
-             ("window_256", dict(window=256)), ("window_1024", dict(window=1024))]
+             ("window_256", dict(window=256)), ("window_1024", dict(window=1024)),
+             ("heavy_256_128", dict(window=256, heavy=128)), ("heavy_1024_512", dict(window=1024, heavy=512))]
     rows = []
     for budget in budgets:
         base = None
