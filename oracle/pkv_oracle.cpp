@@ -223,7 +223,8 @@ void pkvo_window_mean(const uint16_t* probs, int dt, int Hq, int W, int64_t S, u
 // (optional) report, per head, the scaled values above / equal to the threshold *thr_out.
 int pkvo_adakv_capacities(const uint16_t* score, int dt, int H, int64_t n, int64_t base, float one_minus_floor,
                           int64_t floor_capacity, int normalize, int32_t* caps, int64_t* cnt_gt, int64_t* cnt_eq,
-                          uint16_t* thr_out, uint16_t* scaled_out /* optional [H][n]: the (normalised) scores the flat top-k sees */) {
+                          uint16_t* thr_out, uint16_t* scaled_out /* optional [H][n]: the (normalised) scores the flat top-k sees */,
+                          float* ratio_out /* optional [H]: ratio_h (1 without normalize) */) {
     if (H <= 0 || base < 1 || base > n) return 1;
     std::vector<uint16_t> scaled(size_t(H) * size_t(n));
     for (int h = 0; h < H; ++h) {
@@ -237,8 +238,9 @@ int pkvo_adakv_capacities(const uint16_t* score, int dt, int H, int64_t n, int64
             double top = 0.0, all = 0.0;
             for (int64_t j = 0; j < n; ++j) { all += double(srt[size_t(j)]); if (j < base) top += double(srt[size_t(j)]); }
             const float s_top = round_dt(float(top), dt), s_all = round_dt(float(all), dt);      // .sum(dim=-1) in the model dtype
-            ratio = round_dt(s_top / s_all, dt);
+            ratio = round_dt(s_top / s_all, dt);        // 0 / 0 = NaN for a head whose scores are all zero
         }
+        if (ratio_out) ratio_out[h] = ratio;
         for (int64_t j = 0; j < n; ++j)
             scaled[size_t(h) * size_t(n) + size_t(j)] = normalize ? from_f32(to_f32(row[j], dt) * ratio, dt) : row[j];
     }
@@ -247,7 +249,10 @@ int pkvo_adakv_capacities(const uint16_t* score, int dt, int H, int64_t n, int64
     std::vector<float> flat(scaled.size());
     for (size_t i = 0; i < scaled.size(); ++i) flat[i] = to_f32(scaled[i], dt);
     std::vector<float> tmp(flat);
-    std::nth_element(tmp.begin(), tmp.begin() + (K - 1), tmp.end(), [](float a, float b) { return a > b; });
+    // NaN (the scaled scores of a NaN-ratio head) ranks above every value and equals every NaN, as in torch.sort / topk
+    const auto above = [](float a, float b) { return (std::isnan(a) && !std::isnan(b)) || a > b; };
+    const auto same = [](float a, float b) { return (std::isnan(a) && std::isnan(b)) || a == b; };
+    std::nth_element(tmp.begin(), tmp.begin() + (K - 1), tmp.end(), above);
     const float thr = tmp[size_t(K - 1)];
     if (thr_out) *thr_out = from_f32(thr, dt);
     int64_t need = K;
@@ -255,7 +260,7 @@ int pkvo_adakv_capacities(const uint16_t* score, int dt, int H, int64_t n, int64
     for (int h = 0; h < H; ++h)
         for (int64_t j = 0; j < n; ++j) {
             const float x = flat[size_t(h) * size_t(n) + size_t(j)];
-            if (x > thr) ++gt[size_t(h)]; else if (x == thr) ++eq[size_t(h)];
+            if (above(x, thr)) ++gt[size_t(h)]; else if (same(x, thr)) ++eq[size_t(h)];
         }
     for (int h = 0; h < H; ++h) need -= gt[size_t(h)];
     for (int h = 0; h < H; ++h) {

@@ -62,7 +62,7 @@ def lib():
         L.pkvo_key_norms.restype = None
         L.pkvo_window_mean.argtypes = [p, i32, i32, i32, i64, p]
         L.pkvo_window_mean.restype = None
-        L.pkvo_adakv_capacities.argtypes = [p, i32, i32, i64, i64, C.c_float, i64, i32, p, p, p, p, p]
+        L.pkvo_adakv_capacities.argtypes = [p, i32, i32, i64, i64, C.c_float, i64, i32, p, p, p, p, p, p]
         L.pkvo_adakv_capacities.restype = i32
         L.pkvo_rope_inplace.argtypes = [p, i32, i32, i64, i32, i64, i64, p, p, i64]
         L.pkvo_rope_inplace.restype = None
@@ -176,9 +176,11 @@ def adakv_scores(q, k, window_size, kernel_size=7, pooling="maxpool"):
     return pool(out, kernel_size, pooling)
 
 
-def adakv_capacities(score, base_capacity, floor_ratio=0.2, normalize=True, details=False):
+def adakv_capacities(score, base_capacity, floor_ratio=0.2, normalize=True, details=False, ratio_out=None):
     """Per-head budgets (pyramidkv_utils.py:702-717) under the CUDA path's tie rule. score [H, n] -> int32 [H]
-    (details=True: also counts above / equal to the global threshold and the threshold itself)."""
+    (details=True: also counts above / equal to the global threshold and the threshold itself). A head whose scores are
+    all zero has ratio 0 / 0 = NaN under `normalize`; its scaled scores rank above every value, as in torch.
+    `ratio_out`: a float32 [H] tensor that receives every head's ratio (1 without `normalize`)."""
     import numpy as np
     x = score.contiguous()
     H, n = x.shape
@@ -188,7 +190,8 @@ def adakv_capacities(score, base_capacity, floor_ratio=0.2, normalize=True, deta
     scaled = torch.empty_like(x) if details else None
     rc = lib().pkvo_adakv_capacities(x.data_ptr(), _dt(x), H, n, base_capacity, float(np.float32(1 - floor_ratio)),
                                      int(base_capacity * floor_ratio), int(bool(normalize)), caps.data_ptr(), gt.data_ptr(),
-                                     eq.data_ptr(), thr.data_ptr(), scaled.data_ptr() if details else None)
+                                     eq.data_ptr(), thr.data_ptr(), scaled.data_ptr() if details else None,
+                                     ratio_out.data_ptr() if ratio_out is not None else None)
     if rc:
         raise ValueError("oracle: base_capacity out of range")
     return (caps, gt, eq, thr, scaled) if details else caps

@@ -117,6 +117,11 @@ def adakv_scores(K, Q, W, kernel_size, pooling):
     raise ValueError("Pooling method not supported")
 
 
+def adakv_ratio(srt, base_capacity):
+    """ratio_weight (pyramidkv_utils.py:707) of scores sorted descending: sum of the top `base_capacity` over the sum of all."""
+    return srt[..., :base_capacity].sum(dim=-1, keepdim=True) / srt.sum(dim=-1, keepdim=True)
+
+
 def adakv_capacities(score, base_capacity, floor_ratio, normalize, tie_rule="torch"):
     """Per-head budgets of AdaKVCluster.update_kv (pyramidkv_utils.py:702-717): the heads share num_heads * base_capacity
     slots in proportion to how many of the globally largest (optionally normalised) scores they own, mixed with a floor.
@@ -130,8 +135,7 @@ def adakv_capacities(score, base_capacity, floor_ratio, normalize, tie_rule="tor
         srt = srt.to(score.dtype)
     adaptive = srt
     if normalize:
-        ratio = srt[..., :base_capacity].sum(dim=-1, keepdim=True) / srt.sum(dim=-1, keepdim=True)
-        adaptive = adaptive * ratio
+        adaptive = adaptive * adakv_ratio(srt, base_capacity)
     flat = adaptive.reshape(bsz, n * H)
     if tie_rule == "torch":
         top = torch.topk(flat, k=H * base_capacity, dim=-1).indices

@@ -17,6 +17,8 @@ import torch
 
 from . import ops
 
+SELECT_MAX_K = 16384          # largest top_k of the select kernels (pkv_topk.cu: topk_supported)
+
 
 class CudaBackend:
     """The product backend: every call lands in libpkv.so."""
@@ -139,17 +141,28 @@ class CudaBackend:
         return ops.adakv_counts(handle["plan"], base_capacity, normalize)
 
     def ragged_finish(self, handle, caps, reserve):
-        """Uniform select of max(caps) rows per head + gather, then the window rows move to [cap_h, cap_h + W)."""
+        """Uniform select of min(max(caps), 16384) rows per head + gather; every head whose budget is above the select
+        kernels' limit then takes its cap_h rows from a stable descending sort of its pooled row (the same (score desc,
+        index asc) order); last, the window rows move to [cap_h, cap_h + W)."""
         q, k, v, W = handle["q"], handle["k"], handle["v"], handle["W"]
         Hq, D = q.shape[0], q.shape[-1]
         kmax = max(caps)
         k_buf = torch.empty(Hq, kmax + W + reserve, D, dtype=k.dtype, device=k.device)
         v_buf = torch.empty_like(k_buf)
-        plan = ops.plan_evict("snapkv", q, k, v, W, kmax, k_buf, v_buf, handle["kernel"], handle["pooling"], workspace=handle["ws"],
+        ksel = min(kmax, SELECT_MAX_K)
+        plan = ops.plan_evict("snapkv", q, k, v, W, ksel, k_buf, v_buf, handle["kernel"], handle["pooling"], workspace=handle["ws"],
                               window_mean=True)
-        if kmax > 0:
+        # AdaKV can hand one head most of the layer's Hq * base slots, and HeadKV's budgets come from a file: either can pass
+        # the select kernels' limit although max_capacity_prompt - W does not
+        pooled = ops.ws_pooled(plan)
+        big = {h: torch.sort(pooled[h].float(), descending=True, stable=True).indices[:c] for h, c in enumerate(caps) if c > SELECT_MAX_K}
+        if ksel > 0:
             ops.run_stage(plan, "topk")
         ops.run_stage(plan, "gather")
+        G = Hq // k.shape[-3]
+        for h, order in big.items():
+            k_buf[h, :order.numel()] = k[h // G].index_select(0, order)
+            v_buf[h, :order.numel()] = v[h // G].index_select(0, order)
         caps_dev = torch.tensor(caps, dtype=torch.int32, device=k.device)
         ops.ragged_place_window(plan, caps_dev)
         return k_buf, v_buf
