@@ -514,6 +514,36 @@ typedef struct pkv_sample_desc {
     uint32_t reserved;
 } pkv_sample_desc;
 int pkv_sample_tokens(const pkv_sample_desc* d, void* stream);
+/* ---- the same draw with repetition, presence and frequency penalties and min-p (DESIGN.md §4.10) ----
+ * Row b also has rho = repetition_penalty[b], presence = presence_penalty[b], frequency = frequency_penalty[b] and
+ * min_p[b] (fp32), its prompt set P (prompt_mask[b*stride + v] != 0) and its generated-token counts
+ * c[v] = counts[b*stride + v] (>= 0). Every operation below is one IEEE fp32 operation (no contraction):
+ *  1. x_v = f32(logit_v).
+ *  2. rho != 1 and (v in P or c[v] > 0): x_v = x_v < 0 ? x_v * rho : x_v / rho (HF's RepetitionPenaltyLogitsProcessor
+ *     over the prompt and generated ids).
+ *  3. c[v] > 0: x_v = (x_v - frequency * f32(c[v])) - presence (vLLM's order; generated tokens only).
+ *  4. Rules 1-6 of pkv_sample_tokens on x in place of f32(logit): T == 0 or top_k == 1 gives the argmax of x (first index,
+ *     NaN largest), as does a row whose largest x / T is not finite; top-k and top-p as there; then min-p keeps, of the
+ *     top-p set, the tokens with expf(x_i / T - max_j x_j / T) >= min_p (fp32; the largest always stays).
+ *  5. With PKV_SAMPLE_ADVANCE, counts[b*stride + token] += 1 as well as token_index[b] (not for a token -1).
+ * A row with rho = 1, presence = frequency = 0 and min_p = 0 gets exactly pkv_sample_tokens' token (and its mask and counts
+ * are not read); every row reads the parameters of both structs on the device: rho not in (0, inf), a non-finite presence
+ * or frequency, or min_p outside [0, 1] (or NaN) also give token -1. Same launch properties as pkv_sample_tokens (one CTA
+ * per row, no scratch, no allocation, no synchronisation, graph-replayable). PKV_ERR_INVALID_ARG: those of
+ * pkv_sample_tokens, a null penalty struct or struct_bytes mismatch, null or misaligned parameter arrays (4 bytes) or counts
+ * (4 bytes), a null prompt_mask, stride < vocab. */
+typedef struct pkv_sample_penalty {
+    uint32_t struct_bytes;  /* = sizeof(pkv_sample_penalty) */
+    uint32_t reserved;
+    const float* repetition_penalty;   /* [batch] device arrays; 1: off */
+    const float* presence_penalty;     /* 0: off */
+    const float* frequency_penalty;    /* 0: off */
+    const float* min_p;                /* 0: off */
+    const uint8_t* prompt_mask;        /* uint8 [batch, stride]: nonzero for the row's prompt tokens */
+    int32_t* counts;                   /* int32 [batch, stride]: generated-token counts, updated by the launch */
+    int64_t stride;                    /* elements between rows of prompt_mask and counts, >= vocab */
+} pkv_sample_penalty;
+int pkv_sample_tokens_penalized(const pkv_sample_desc* d, const pkv_sample_penalty* p, void* stream);
 
 /* ---- token log-probabilities: the log-softmax of each row of logits at a token and at its top N (DESIGN.md §4.8) ----
  * Row b (logits[b*logits_stride .. + vocab), bf16 / fp16) is read as the model's raw distribution: x_i = f32(logit_i),

@@ -24,7 +24,7 @@ EXPORTS = [
     "pkv_decode_attn_batch_fp8", "pkv_cache_quantize_fp8", "pkv_decode_attn_batch_gqa", "pkv_decode_attn_batch_gqa_fp8",
     "pkv_evict_pooled_kv_offset", "pkv_cache_install", "pkv_sample_tokens", "pkv_decode_attn_window",
     "pkv_decode_attn_heavy", "pkv_decode_heavy_workspace_bytes",
-    "pkv_token_logprobs",
+    "pkv_token_logprobs", "pkv_sample_tokens_penalized",
 ]
 FLAG_GQA_SHARED = 128          # pkv_evict_desc.flags: one compacted cache per KV head
 
@@ -100,6 +100,14 @@ class SampleDesc(C.Structure):
         ("temperature", C.c_void_p), ("top_k", C.c_void_p), ("top_p", C.c_void_p), ("seed", C.c_void_p),
         ("token_index", C.c_void_p), ("tokens", C.c_void_p), ("tokens_stride", C.c_int64), ("column", C.c_int64),
         ("flags", C.c_uint32), ("reserved", C.c_uint32),
+    ]
+
+
+class SamplePenalty(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("reserved", C.c_uint32),
+        ("repetition_penalty", C.c_void_p), ("presence_penalty", C.c_void_p), ("frequency_penalty", C.c_void_p),
+        ("min_p", C.c_void_p), ("prompt_mask", C.c_void_p), ("counts", C.c_void_p), ("stride", C.c_int64),
     ]
 
 
@@ -207,6 +215,8 @@ def lib() -> C.CDLL:
     L.pkv_cache_install.restype = i32
     L.pkv_sample_tokens.argtypes = [C.POINTER(SampleDesc), p]
     L.pkv_sample_tokens.restype = i32
+    L.pkv_sample_tokens_penalized.argtypes = [C.POINTER(SampleDesc), C.POINTER(SamplePenalty), p]
+    L.pkv_sample_tokens_penalized.restype = i32
     L.pkv_token_logprobs.argtypes = [C.POINTER(LogprobsDesc), p]
     L.pkv_token_logprobs.restype = i32
     if L.pkv_version() != 3:

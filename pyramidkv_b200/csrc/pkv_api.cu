@@ -890,8 +890,8 @@ int pkv_update_flatten_view(void* dst, const void* src, const void* state, const
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "flatten append launch");
 }
 
-int pkv_sample_tokens(const pkv_sample_desc* d, void* stream) {
-    const char* fn = "pkv_sample_tokens";
+// The checks of pkv_sample_tokens, then its launch, or the penalized one when `pen` is set (already checked).
+static int sample(const char* fn, const pkv_sample_desc* d, const pkv_sample_penalty* pen, void* stream) {
     if (!d) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
     if (d->struct_bytes != sizeof(pkv_sample_desc))
         return fail(PKV_ERR_INVALID_ARG, "pkv_sample_desc.struct_bytes=%u, library expects %zu (ABI mismatch)", d->struct_bytes, sizeof(pkv_sample_desc));
@@ -918,8 +918,29 @@ int pkv_sample_tokens(const pkv_sample_desc* d, void* stream) {
     a.tokens = d->tokens; a.tokens_ld = d->tokens_stride; a.col = d->column;
     a.advance = (d->flags & PKV_SAMPLE_ADVANCE) != 0;
     DeviceGuard guard(d->device);
-    const cudaError_t e = launch_sample(a, static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "sample launch");
+    if (!pen) {
+        const cudaError_t e = launch_sample(a, static_cast<cudaStream_t>(stream));
+        return e == cudaSuccess ? PKV_OK : fail_cuda(e, "sample launch");
+    }
+    if (pen->stride < d->vocab) return fail(PKV_ERR_INVALID_ARG, "%s: stride=%lld < vocab=%lld", fn, (long long)pen->stride, (long long)d->vocab);
+    PenaltyArgs p;
+    p.repetition = pen->repetition_penalty; p.presence = pen->presence_penalty; p.frequency = pen->frequency_penalty;
+    p.min_p = pen->min_p; p.mask = pen->prompt_mask; p.counts = pen->counts; p.ld = pen->stride;
+    const cudaError_t e = launch_sample_penalized(a, p, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "penalized sample launch");
+}
+
+int pkv_sample_tokens(const pkv_sample_desc* d, void* stream) { return sample("pkv_sample_tokens", d, nullptr, stream); }
+
+int pkv_sample_tokens_penalized(const pkv_sample_desc* d, const pkv_sample_penalty* pen, void* stream) {
+    const char* fn = "pkv_sample_tokens_penalized";
+    if (!pen || pen->struct_bytes != sizeof(pkv_sample_penalty))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null pkv_sample_penalty or struct_bytes != %zu (ABI mismatch)", fn, sizeof(pkv_sample_penalty));
+    const auto bad = [](const void* ptr, uintptr_t align) { return !ptr || (reinterpret_cast<uintptr_t>(ptr) & (align - 1)); };
+    if (bad(pen->repetition_penalty, 4) || bad(pen->presence_penalty, 4) || bad(pen->frequency_penalty, 4) || bad(pen->min_p, 4))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned repetition / presence / frequency penalty or min_p (4 bytes)", fn);
+    if (bad(pen->prompt_mask, 1) || bad(pen->counts, 4)) return fail(PKV_ERR_INVALID_ARG, "%s: null prompt_mask, or null or misaligned counts (4 bytes)", fn);
+    return sample(fn, d, pen, stream);
 }
 
 int pkv_token_logprobs(const pkv_logprobs_desc* d, void* stream) {

@@ -202,6 +202,17 @@ struct SampleArgs {
     bool advance;               // token_index[b] += 1 after the draw
 };
 cudaError_t launch_sample(const SampleArgs& a, cudaStream_t st);
+// the penalties and min-p of pkv_sample_tokens_penalized, per row b
+struct PenaltyArgs {
+    const float* repetition;    // [B] device parameters
+    const float* presence;
+    const float* frequency;
+    const float* min_p;
+    const uint8_t* mask;        // prompt_mask[b * ld + v]
+    int32_t* counts;            // counts[b * ld + v], incremented at the drawn token with SampleArgs::advance
+    int64_t ld;
+};
+cudaError_t launch_sample_penalized(const SampleArgs& a, const PenaltyArgs& p, cudaStream_t st);
 
 // log-probabilities of one row of logits at a token and at its top N (pkv_logprobs.cu): one CTA per row
 constexpr int kMaxTopLogprobs = 20;

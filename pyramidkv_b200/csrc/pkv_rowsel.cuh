@@ -23,6 +23,14 @@ __device__ __forceinline__ uint32_t okey(uint32_t b) {
     return (b & 0x8000u) ? (~b & 0xffffu) : (b | 0x8000u);
 }
 __device__ __forceinline__ uint16_t key_bits(uint32_t k) { return uint16_t((k & 0x8000u) ? (k & 0x7fffu) : (~k & 0xffffu)); }
+// the same for fp32 values (the penalized sampler, whose values are not 16-bit logits); for a bf16 logit l,
+// okey32(f32(l)) == okey(bits(l)) << 16
+__device__ __forceinline__ uint32_t okey32(float v) {
+    uint32_t b = __float_as_uint(v);
+    if ((b & 0x7fffffffu) == 0) b = 0;
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float key_value32(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
 
 __device__ __forceinline__ unsigned long long fixed_mass(float x, float m) {
     return __float2ull_rn(expf(x - m) * kFixScale);

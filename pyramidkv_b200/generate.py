@@ -29,7 +29,11 @@ while the captured step graph keeps replaying unchanged.
 All three loops are greedy by default. `sampling=SamplingParams(...)` (or one per prompt) draws each token instead - the
 prefill's with token index t = 0, decode step n's with t = n - with temperature, top-k, top-p and a per-request seed, one
 `pkv_sample_tokens` launch per step for the whole batch in place of the argmax (DESIGN.md §4.6). A request's tokens depend
-only on its logits, its parameters and its seed, not on its batch position, slot or the graph.
+only on its logits, its parameters and its seed, not on its batch position, slot or the graph. Its repetition, presence and
+frequency penalties and min-p (HF's RepetitionPenaltyLogitsProcessor and MinPLogitsWarper, vLLM's presence / frequency
+penalties) are applied on the device from a per-row prompt mask and generated-token count table, in one
+`pkv_sample_tokens_penalized` launch per step instead (DESIGN.md §4.10); `SamplingParams(temperature=0,
+repetition_penalty=r)` is HF's `generate(do_sample=False, repetition_penalty=r)`.
 
 `logprobs=N` (0 to 20) in any of the three loops also returns one `TokenLogprobs` per prompt: the log-probability of every
 generated token and the N most likely tokens at each position, under the model's raw distribution (log_softmax of the
@@ -39,6 +43,7 @@ log-probabilities over the compacted cache: the likelihood a cache form gives a 
 """
 from __future__ import annotations
 
+import math
 import time
 from dataclasses import dataclass
 from typing import List, Optional
@@ -50,13 +55,21 @@ from .cache import PkvBatchCacheLayer, PkvCacheLayer, admit_cache, join_caches, 
 
 @dataclass(frozen=True)
 class SamplingParams:
-    """One request's sampling settings, applied in HF's warper order: temperature, top-k, top-p, then the draw.
-    temperature 0 or top_k 1: the greedy token. top_k 0 and top_p 1 switch those filters off. The temperature is used as an
-    fp32 value; the 64-bit seed and the token index key the Philox stream of the Gumbel-max draw (DESIGN.md §4.6)."""
+    """One request's sampling settings, applied in HF's order: repetition penalty, temperature, top-k, top-p, min-p, then
+    the draw. temperature 0 or top_k 1: the greedy token (of the penalized logits). top_k 0 and top_p 1 switch those filters
+    off. The temperature is used as an fp32 value; the 64-bit seed and the token index key the Philox stream of the
+    Gumbel-max draw (DESIGN.md §4.6). repetition_penalty (> 0; 1: off) divides the positive and multiplies the negative
+    logits of the prompt's and the generated tokens; presence_penalty and frequency_penalty (0: off) subtract, from each
+    generated token's logit, the penalty and the penalty times its count (vLLM's order, after the repetition penalty); min_p
+    (in [0, 1]; 0: off) drops the tokens whose probability is below min_p times the largest (DESIGN.md §4.10)."""
     temperature: float = 1.0
     top_k: int = 0
     top_p: float = 1.0
     seed: int = 0
+    repetition_penalty: float = 1.0
+    presence_penalty: float = 0.0
+    frequency_penalty: float = 0.0
+    min_p: float = 0.0
 
     def __post_init__(self):
         if not float(self.temperature) >= 0.0:
@@ -67,6 +80,19 @@ class SamplingParams:
             raise ValueError(f"SamplingParams: top_p must be in (0, 1], got {self.top_p}")
         if int(self.seed) != self.seed or not 0 <= int(self.seed) < 2 ** 64:
             raise ValueError(f"SamplingParams: seed must be an integer in [0, 2^64), got {self.seed}")
+        if not 0.0 < float(self.repetition_penalty) < math.inf:
+            raise ValueError(f"SamplingParams: repetition_penalty must be finite and > 0, got {self.repetition_penalty}")
+        for name in ("presence_penalty", "frequency_penalty"):
+            if not math.isfinite(float(getattr(self, name))):
+                raise ValueError(f"SamplingParams: {name} must be finite, got {getattr(self, name)}")
+        if not 0.0 <= float(self.min_p) <= 1.0:
+            raise ValueError(f"SamplingParams: min_p must be in [0, 1], got {self.min_p}")
+
+    @property
+    def penalized(self) -> bool:
+        """Some penalty or min-p is on: the draw needs the request's prompt and generated tokens."""
+        return (float(self.repetition_penalty) != 1.0 or float(self.presence_penalty) != 0.0
+                or float(self.frequency_penalty) != 0.0 or float(self.min_p) != 0.0)
 
 
 def _seed_i64(seed: int) -> int:
@@ -74,23 +100,71 @@ def _seed_i64(seed: int) -> int:
     return seed - 2 ** 64 if seed >= 2 ** 63 else seed      # the same 64 bits in an int64 tensor
 
 
+_PENALTY_FIELDS = ("repetition_penalty", "presence_penalty", "frequency_penalty", "min_p")
+
+
 class SamplingState:
     """The per-row device state `sample_tokens` reads: parameters and the token index of each row (sequence or slot).
-    Rows are rewritten in place (`set_row`), so a captured graph keeps its pointers."""
+    Rows are rewritten in place (`set_row`), so a captured graph keeps its pointers.
 
-    def __init__(self, params: List[SamplingParams], device, index: int = 0):
+    With penalties (some request sets one, or `penalties=True` for rows that may later take such a request), also the
+    state `sample_tokens_penalized` reads: the four penalty parameters per row, the prompt mask (uint8 [B, vocab]) and the
+    generated-token counts (int32 [B, vocab]), built from `prompts` (one id tensor per row) and `first` (each row's token
+    drawn so far, counted once; None: nothing generated yet). B * vocab * 5 bytes, allocated only then."""
+
+    def __init__(self, params: List[SamplingParams], device, index: int = 0, vocab: Optional[int] = None, prompts=None,
+                 first: Optional[torch.Tensor] = None, penalties: bool = False):
         self.temperature = torch.tensor([float(p.temperature) for p in params], dtype=torch.float32, device=device)
         self.top_k = torch.tensor([min(int(p.top_k), 2 ** 31 - 1) for p in params], dtype=torch.int32, device=device)
         self.top_p = torch.tensor([float(p.top_p) for p in params], dtype=torch.float32, device=device)
         self.seed = torch.tensor([_seed_i64(p.seed) for p in params], dtype=torch.int64, device=device)
         self.index = torch.full((len(params),), int(index), dtype=torch.int64, device=device)
+        self.penalized = bool(penalties) or any(p.penalized for p in params)
+        if not self.penalized:
+            return
+        if vocab is None or prompts is None or len(prompts) != len(params):
+            raise ValueError("SamplingState: penalties need the vocabulary size and one prompt per row")
+        for name in _PENALTY_FIELDS:
+            setattr(self, name, torch.tensor([float(getattr(p, name)) for p in params], dtype=torch.float32, device=device))
+        self.prompt_mask = torch.zeros(len(params), int(vocab), dtype=torch.uint8, device=device)
+        self.counts = torch.zeros(len(params), int(vocab), dtype=torch.int32, device=device)
+        for row, ids in enumerate(prompts):
+            self._set_history(row, ids, None if first is None else first.reshape(-1)[row])
 
-    def set_row(self, row: int, p: SamplingParams, index: int) -> None:
+    def _set_history(self, row: int, prompt: torch.Tensor, first: Optional[torch.Tensor]) -> None:
+        ids = torch.as_tensor(prompt).reshape(-1).to(device=self.counts.device, dtype=torch.long)
+        V = self.counts.shape[1]
+        if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= V):
+            raise ValueError(f"SamplingState: prompt ids outside [0, {V})")
+        self.prompt_mask[row].zero_()
+        self.prompt_mask[row].index_fill_(0, ids, 1)
+        self.counts[row].zero_()
+        if first is not None:
+            self.counts[row].index_fill_(0, torch.as_tensor(first).reshape(1).to(device=self.counts.device, dtype=torch.long), 1)
+
+    def set_row(self, row: int, p: SamplingParams, index: int, prompt=None, first: Optional[torch.Tensor] = None) -> None:
+        """Row `row` takes the parameters `p` at token index `index`; with penalties, its prompt mask becomes `prompt`'s
+        ids and its counts count `first` (the token drawn so far) once."""
+        if p.penalized and not self.penalized:
+            raise ValueError("SamplingState.set_row: a request with penalties or min-p needs a state built with penalties")
+        if self.penalized and prompt is None:
+            raise ValueError("SamplingState.set_row: a state with penalties needs the row's prompt ids")
         self.temperature[row] = float(p.temperature)
         self.top_k[row] = min(int(p.top_k), 2 ** 31 - 1)
         self.top_p[row] = float(p.top_p)
         self.seed[row] = _seed_i64(p.seed)
         self.index[row] = int(index)
+        if self.penalized:
+            for name in _PENALTY_FIELDS:
+                getattr(self, name)[row] = float(getattr(p, name))
+            self._set_history(row, prompt, first)
+
+    def draw(self, backend, logits, out, col, advance=True) -> None:
+        """One launch for every row: `sample_tokens`, or `sample_tokens_penalized` when the state has penalties."""
+        if self.penalized:
+            backend.sample_tokens_penalized(logits, self, out, col, advance)
+        else:
+            backend.sample_tokens(logits, self, out, col, advance)
 
 
 def _sampling_list(sampling, n: int, what: str):
@@ -169,21 +243,23 @@ class StaticDecoder:
     `cache.join_caches`; first_token: the token the prefill produced per sequence ([B] or [B, 1] int64).
     eos_token_id (int or list): a sequence that produced one is done - it keeps decoding in lock-step, but its tokens are
     `pad_token_id` from then on (on the device: `done` [B]); None masks nothing. sampling: None (greedy: the argmax) or one
-    SamplingParams per sequence, whose first decode step draws with token index 1 (the prefill's token is t = 0).
+    SamplingParams per sequence, whose first decode step draws with token index 1 (the prefill's token is t = 0); with
+    penalties or min-p, `prompts` gives each sequence's prompt ids (the first token counts as generated).
     logprobs: None, or N: each step also writes the log-probability of its token and the top N into `self.logprobs`
     (`_LogprobBuffers`, column = the step). forced: None, or int64 [B, max_steps]: step n takes forced[:, n] as its token
     instead of the argmax (teacher forcing; it is then the next step's input, and with `logprobs` the token scored)."""
 
     def __init__(self, model, cache, first_token: torch.Tensor, max_steps: int, use_graph: Optional[bool] = None,
                  eos_token_id=None, pad_token_id: int = 0, sampling: Optional[List[SamplingParams]] = None,
-                 logprobs: Optional[int] = None, forced: Optional[torch.Tensor] = None):
+                 logprobs: Optional[int] = None, forced: Optional[torch.Tensor] = None, prompts=None):
         layers = [l for l in cache.layers if isinstance(l, PkvCacheLayer)]
         if len(layers) != model.config.num_hidden_layers:
             raise RuntimeError("StaticDecoder needs a cache prefilled by the patched forward on every layer "
                                "(method 'fullkv' and stock caches go through model.generate)")
         for l in layers:
             l.reserve(int(max_steps))                      # off the per-token path: no reallocation while the graph lives
-        self._setup(model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling, logprobs)
+        self._setup(model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling, logprobs,
+                    prompts)
         if forced is not None:
             if sampling is not None:
                 raise ValueError("StaticDecoder: forced tokens and sampling exclude each other")
@@ -200,7 +276,7 @@ class StaticDecoder:
             self._stop_finished()
 
     def _setup(self, model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling,
-               logprobs=None) -> None:
+               logprobs=None, prompts=None, penalties=False) -> None:
         """The state both decoders hold: the step counter and workspace the decode launches read, the per-sequence input
         ids and positions, the token buffer [B, max_steps] and its cursor, the EOS ids, when sampling, the per-sequence
         sampling state with the buffer the sampled tokens land in, and with `logprobs` the buffers of the log-probabilities."""
@@ -229,7 +305,8 @@ class StaticDecoder:
         if sampling is not None:
             if len(sampling) != bsz:
                 raise ValueError(f"{len(sampling)} SamplingParams for {bsz} sequences")
-            self.sampling = SamplingState(sampling, dev, index=1)
+            self.sampling = SamplingState(sampling, dev, index=1, vocab=model.lm_head.weight.shape[0], prompts=prompts,
+                                          first=self.ids, penalties=penalties)
             self.sampled = torch.zeros(bsz, 1, dtype=torch.long, device=dev)
         self.forced = None
         self.logprobs = None if logprobs is None else _LogprobBuffers(bsz, self.max_steps, int(logprobs), dev)
@@ -250,7 +327,7 @@ class StaticDecoder:
         if self.forced is not None:
             tok = self.forced.index_select(1, self.cursor)                # [B, 1]
         elif self.sampling is not None:
-            self.backend.sample_tokens(logits, self.sampling, self.sampled, 0)
+            self.sampling.draw(self.backend, logits, self.sampled, 0)
             tok = self.sampled
         else:
             tok = logits.argmax(dim=-1, keepdim=True)                     # [B, 1]
@@ -281,10 +358,11 @@ class StaticDecoder:
     def _counters(self) -> list:
         """The device tensors a step advances (restored after the warm-up step of a capture)."""
         idx = self.sampling.index if self.sampling is not None else None
+        counts = self.sampling.counts if self.sampling is not None and self.sampling.penalized else None
         # the heavy-hitter state a step updates (knob pkv_decode_heavy): restored so that the captured step starts from it
         heavy = [t for l in self.layers if l.heavy is not None for t in (l.heavy_scores, l.heavy_gen, l.victim)]
-        return [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done, idx, self.window_rows)
-                if t is not None] + heavy
+        return [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done, idx, counts,
+                            self.window_rows) if t is not None] + heavy
 
     def _capture(self) -> None:
         # warm up on a side stream (lazy initialisation, cuBLAS workspaces), restore the counters, then capture
@@ -361,7 +439,8 @@ def _prefill(model, input_ids: torch.Tensor, sampling: Optional[SamplingParams] 
         first = logits.argmax(dim=-1, keepdim=True)
     else:
         first = torch.zeros(1, 1, dtype=torch.long, device=logits.device)
-        _backend(model).sample_tokens(logits, SamplingState([sampling], logits.device, index=0), first, 0, advance=False)
+        st = SamplingState([sampling], logits.device, index=0, vocab=logits.shape[1], prompts=[input_ids])
+        st.draw(_backend(model), logits, first, 0, advance=False)
     if logprobs is None:
         return first, cache
     return first, cache, _score(model, logits, first, logprobs)
@@ -397,7 +476,7 @@ def greedy_generate(model, input_ids: torch.Tensor, max_new_tokens: int, use_gra
         windowed = eos and getattr(cache.layers[0], "window", None) is not None
         dec = StaticDecoder(model, cache, first, max_new_tokens - 1, use_graph=use_graph,
                             eos_token_id=sorted(eos) if windowed else None, sampling=None if sampling is None else [sampling],
-                            logprobs=logprobs)
+                            logprobs=logprobs, prompts=[input_ids])
         keep = max_new_tokens - 1
         if not eos:
             toks.append(dec.run(max_new_tokens - 1).clone())
@@ -457,7 +536,7 @@ def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None
     gen = torch.empty(len(ids), 0, dtype=torch.long)
     if steps and not all(t in eos for t in first_host):
         dec = StaticDecoder(model, cache, first, steps, use_graph=use_graph, eos_token_id=sorted(eos) if eos else None,
-                            pad_token_id=pad_token_id, sampling=samp, logprobs=logprobs)
+                            pad_token_id=pad_token_id, sampling=samp, logprobs=logprobs, prompts=ids)
         while dec.taken < steps:
             dec.run(min(max(1, check_every) if eos else steps, steps - dec.taken))
             if eos and bool(dec.done.all()):                            # one device-to-host read per chunk
@@ -490,16 +569,17 @@ class ContinuousDecoder(StaticDecoder):
     buffer holds one chunk, [B, chunk]; `run_chunk` replays `steps` steps, reads them with one device-to-host copy and
     resets the cursor in place. Between chunks `admit` copies a prefilled prompt into a slot and `park` empties one; both
     write the buffers and row counts in place, so the captured graph keeps replaying. `grow_for` reallocates the buffers
-    when an admission needs more rows; the graph is then captured again."""
+    when an admission needs more rows; the graph is then captured again. `prompts` (each slot's prompt ids) and `penalties`
+    (keep the penalty state even when no starting request needs it, for later admissions) as in `SamplingState`."""
 
     def __init__(self, model, cache, first_token: torch.Tensor, left, chunk: int, use_graph: Optional[bool] = None,
                  eos_token_id=None, pad_token_id: int = 0, sampling: Optional[List[SamplingParams]] = None,
-                 logprobs: Optional[int] = None):
+                 logprobs: Optional[int] = None, prompts=None, penalties: bool = False):
         layers = [l for l in cache.layers if isinstance(l, PkvBatchCacheLayer)]
         if len(layers) != model.config.num_hidden_layers or len(layers) != len(cache.layers):
             raise RuntimeError("ContinuousDecoder needs a batched cache (cache.join_caches) on every layer")
         self._setup(model, cache, layers, first_token, max(1, int(chunk)), use_graph, eos_token_id, pad_token_id, sampling,
-                    logprobs)
+                    logprobs, prompts, penalties)
         # every layer's row counts are rows of one tensor, so one op per step stops them growing for the done slots
         self.rows_all = torch.stack([l.rows for l in layers])
         for i, l in enumerate(layers):
@@ -552,14 +632,16 @@ class ContinuousDecoder(StaticDecoder):
             self.graph = None
         return grew
 
-    def admit(self, slot: int, src_cache, first_token: torch.Tensor, left: int, sampling: Optional[SamplingParams] = None) -> None:
+    def admit(self, slot: int, src_cache, first_token: torch.Tensor, left: int, sampling: Optional[SamplingParams] = None,
+              prompt=None) -> None:
         """Slot `slot` continues the prefilled prompt `src_cache` (first token `first_token`, `left` decode steps); a sampling
-        decoder takes the request's `sampling` parameters, its next token drawn with token index 1."""
+        decoder takes the request's `sampling` parameters, its next token drawn with token index 1, and with penalties its
+        prompt mask (`prompt`: the prompt ids) and counts (the first token once) are rebuilt in place."""
         if (sampling is None) != (self.sampling is None):
             raise ValueError("admit: pass sampling parameters exactly when the decoder samples")
-        admit_cache(self.cache, slot, src_cache, self.state.step, self.backend)
         if sampling is not None:
-            self.sampling.set_row(slot, sampling, 1)
+            self.sampling.set_row(slot, sampling, 1, prompt, first_token)     # checks the request before the slot changes
+        admit_cache(self.cache, slot, src_cache, self.state.step, self.backend)
         self.ids[slot] = first_token.reshape(-1)[:1].to(self.ids.device)
         self.pos[slot] = self.layers[0].seq_seen[slot]
         self.left[slot] = int(left)
@@ -646,7 +728,8 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     slot_req = list(range(B))
     dec = ContinuousDecoder(model, cache, torch.cat(firsts), [0 if finished(b) else caps[b] - 1 for b in range(B)], chunk,
                             use_graph=use_graph, eos_token_id=sorted(eos) if eos else None, pad_token_id=pad_token_id,
-                            sampling=None if samp is None else samp[:B], logprobs=logprobs)
+                            sampling=None if samp is None else samp[:B], logprobs=logprobs, prompts=ids[:B],
+                            penalties=samp is not None and any(p.penalized for p in samp))
     waiting = B
     while True:
         for s in range(B):
@@ -660,7 +743,7 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
                 if finished(i):
                     continue
                 stats["regrowths"] += int(dec.grow_for(single, caps[i]))
-                dec.admit(s, single, first, caps[i] - 1, None if samp is None else samp[i])
+                dec.admit(s, single, first, caps[i] - 1, None if samp is None else samp[i], ids[i])
                 stats["admissions"] += 1
                 slot_req[s] = i
             if slot_req[s] is None:

@@ -119,6 +119,9 @@ class CudaBackend:
     def sample_tokens(self, logits, params, out, col, advance=True):
         ops.sample_tokens(logits, params, out, col, advance)
 
+    def sample_tokens_penalized(self, logits, params, out, col, advance=True):
+        ops.sample_tokens_penalized(logits, params, out, col, advance)
+
     # -- token log-probabilities: the raw log-softmax at a token and at the row's top N --
     def token_logprobs(self, logits, tokens, out_lp, out_ids, out_top, col=0, tokens_col=0, cursor=None):
         ops.token_logprobs(logits, tokens, out_lp, out_ids, out_top, col, tokens_col, cursor)

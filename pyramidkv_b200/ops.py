@@ -791,17 +791,27 @@ def sample_tokens(logits: torch.Tensor, params, out: torch.Tensor, col: int, adv
     own parameters. `params` holds the per-row DEVICE tensors `temperature` (float32 [B]), `top_k` (int32), `top_p`
     (float32), `seed` (int64, the 64 seed bits) and `index` (int64, the row's token index t; incremented in place when
     `advance`) - generate.SamplingState. Nothing is read back: the launch replays in a CUDA graph."""
-    _require_cuda(logits, out, params.temperature, params.top_k, params.top_p, params.seed, params.index)
-    if logits.dim() != 2 or logits.stride(1) != 1:
-        raise ValueError(f"sample_tokens: logits must be [B, V] with contiguous rows, got {tuple(logits.shape)}")
-    B, V = logits.shape
-    if out.dim() != 2 or out.dtype != torch.long or out.shape[0] != B or out.stride(1) != 1:
-        raise ValueError(f"sample_tokens: out must be an int64 [B={B}, n] tensor with contiguous rows")
-    for name, dt in (("temperature", torch.float32), ("top_k", torch.int32), ("top_p", torch.float32), ("seed", torch.int64),
-                     ("index", torch.int64)):
+    d = _sample_desc("sample_tokens", logits, params, out, col, advance)
+    _lib.check(_lib.lib().pkv_sample_tokens(C.byref(d), torch.cuda.current_stream(logits.device).cuda_stream))
+
+
+def _check_row_params(fn, logits, params, fields):
+    B = logits.shape[0]
+    for name, dt in fields:
         t = getattr(params, name)
         if t.dtype != dt or t.numel() != B or not t.is_contiguous() or t.device != logits.device:
-            raise ValueError(f"sample_tokens: params.{name} must be a contiguous {dt} tensor of B = {B} elements on {logits.device}")
+            raise ValueError(f"{fn}: params.{name} must be a contiguous {dt} tensor of B = {B} elements on {logits.device}")
+
+
+def _sample_desc(fn, logits, params, out, col, advance):
+    _require_cuda(logits, out, params.temperature, params.top_k, params.top_p, params.seed, params.index)
+    if logits.dim() != 2 or logits.stride(1) != 1:
+        raise ValueError(f"{fn}: logits must be [B, V] with contiguous rows, got {tuple(logits.shape)}")
+    B, V = logits.shape
+    if out.dim() != 2 or out.dtype != torch.long or out.shape[0] != B or out.stride(1) != 1:
+        raise ValueError(f"{fn}: out must be an int64 [B={B}, n] tensor with contiguous rows")
+    _check_row_params(fn, logits, params, (("temperature", torch.float32), ("top_k", torch.int32), ("top_p", torch.float32),
+                                           ("seed", torch.int64), ("index", torch.int64)))
     d = _lib.SampleDesc()
     d.struct_bytes = C.sizeof(_lib.SampleDesc)
     d.dtype = _dtype_code(logits)
@@ -812,7 +822,35 @@ def sample_tokens(logits: torch.Tensor, params, out: torch.Tensor, col: int, adv
     d.seed, d.token_index = params.seed.data_ptr(), params.index.data_ptr()
     d.tokens, d.tokens_stride, d.column = out.data_ptr(), out.stride(0) if B > 1 else out.shape[1], int(col)
     d.flags = _lib.SAMPLE_ADVANCE if advance else 0
-    _lib.check(_lib.lib().pkv_sample_tokens(C.byref(d), torch.cuda.current_stream(logits.device).cuda_stream))
+    return d
+
+
+def sample_tokens_penalized(logits: torch.Tensor, params, out: torch.Tensor, col: int, advance: bool = True) -> None:
+    """`sample_tokens` with repetition, presence and frequency penalties and min-p (include/pkv.h:
+    pkv_sample_tokens_penalized, DESIGN.md §4.10), in ONE launch. `params` also holds the per-row DEVICE tensors
+    `repetition_penalty`, `presence_penalty`, `frequency_penalty`, `min_p` (float32 [B]), `prompt_mask` (uint8 [B, S],
+    nonzero for the row's prompt tokens) and `counts` (int32 [B, S], the row's generated-token counts; with `advance` the
+    drawn token's count is incremented in place), S >= V with contiguous rows. A row whose new parameters are at their
+    defaults (1, 0, 0, 0) gets `sample_tokens`' token."""
+    fn = "sample_tokens_penalized"
+    d = _sample_desc(fn, logits, params, out, col, advance)
+    B, V = logits.shape
+    _check_row_params(fn, logits, params, [(n, torch.float32) for n in ("repetition_penalty", "presence_penalty",
+                                                                        "frequency_penalty", "min_p")])
+    mask, counts = params.prompt_mask, params.counts
+    _require_cuda(mask, counts)
+    if (mask.dim() != 2 or mask.dtype != torch.uint8 or counts.dtype != torch.int32 or mask.shape != counts.shape
+            or mask.shape[0] != B or mask.shape[1] < V or not mask.is_contiguous() or not counts.is_contiguous()
+            or mask.device != logits.device or counts.device != logits.device):
+        raise ValueError(f"{fn}: params.prompt_mask / params.counts must be contiguous uint8 / int32 [B={B}, S >= V={V}] "
+                         f"tensors on {logits.device}")
+    p = _lib.SamplePenalty()
+    p.struct_bytes = C.sizeof(_lib.SamplePenalty)
+    p.repetition_penalty, p.presence_penalty = params.repetition_penalty.data_ptr(), params.presence_penalty.data_ptr()
+    p.frequency_penalty, p.min_p = params.frequency_penalty.data_ptr(), params.min_p.data_ptr()
+    p.prompt_mask, p.counts, p.stride = mask.data_ptr(), counts.data_ptr(), mask.shape[1]
+    _lib.check(_lib.lib().pkv_sample_tokens_penalized(C.byref(d), C.byref(p),
+                                                      torch.cuda.current_stream(logits.device).cuda_stream))
 
 
 # ---- token log-probabilities (include/pkv.h: pkv_token_logprobs, DESIGN.md §4.8) ----
