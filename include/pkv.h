@@ -545,6 +545,80 @@ typedef struct pkv_sample_penalty {
 } pkv_sample_penalty;
 int pkv_sample_tokens_penalized(const pkv_sample_desc* d, const pkv_sample_penalty* p, void* stream);
 
+/* ---- generation constraints: the per-row rule terms of one step, from the row's token history (DESIGN.md §4.11) ----
+ * Row b has a history h = history[b*history_stride ..] of n = history_len[b] token ids (its prompt, then every token
+ * generated so far), prompt_len[b], flags[b] (PKV_RULE_*), no-repeat n-gram size N = ngram[b] (0: off), min_new =
+ * min_new_tokens[b], and n_seq[b] rule sequences: sequence j has the tokens seq_tokens[b*tokens_stride + seq_off[b*
+ * seq_stride + j] .. seq_off[.. + j + 1]) (length L >= 1), the kind seq_kind[b*seq_stride + j] and, for a bias, the fp32
+ * value seq_bias[b*seq_stride + j]. One CTA per row:
+ *  0. With `append`, h[n] = append[b*append_stride + append_column] and history_len[b] = n + 1 first (not when n already
+ *     equals history_stride: a full history takes no more tokens).
+ *  1. PKV_RULE_BIAS: bias[b*bias_stride + v] = 0 for every v < vocab, then, for each run of consecutive bias sequences
+ *     with one last token v (the caller orders them: the single-token one first, then in its own order), bias[v] =
+ *     (((0 + w_1) + m_2 w_2) + ...), where m_j w_j is w_j when the sequence applies and 0 otherwise; a single-token sequence
+ *     always applies, a longer one when L <= n and its first L - 1 tokens equal the last L - 1 of h (HF's
+ *     SequenceBiasLogitsProcessor, its dict order and its skip of sequences longer than the context).
+ *  2. PKV_RULE_BAN | PKV_RULE_BAD: the 2 * W words (W = ceil(vocab / 32)) of ban[b*ban_stride ..] are cleared; bit v of
+ *     words [0, W) ("set to -inf") is set for every token N > 0 bans (the last token of every N-gram of h whose first N - 1
+ *     tokens are the last N - 1 of h: HF's NoRepeatNGramLogitsProcessor, nothing while n + 1 < N) and, while n -
+ *     prompt_len[b] < min_new, for each of the n_eos ids eos[] (HF's MinNewTokensLengthLogitsProcessor); bit v of words
+ *     [W, 2W) ("add -inf") for the last token of every bad-word sequence that applies as in 1 (HF's
+ *     NoBadWordsLogitsProcessor; the caller drops the single-token bad words equal to an EOS id).
+ *  3. stop[b] = 1 when a stop sequence equals the last L tokens of h (L <= n), else 0.
+ * Token ids outside [0, vocab) in h, in the sequences or in eos[] ban nothing. A row with flags 0 only appends and writes
+ * stop[b] = 0. No allocation, no synchronisation, fixed launch arguments: graph-replayable. PKV_ERR_INVALID_ARG: batch
+ * outside [1, 2^20], vocab outside [1, 2^24], a null or misaligned (4 bytes; 8 for append) pointer, a null eos with n_eos
+ * > 0, strides smaller than what they index (history_stride < 1, bias_stride < vocab, ban_stride < 2W, seq_stride < 2,
+ * tokens_stride < 1, append_column outside [0, append_stride)). The device tables must hold n_seq[b] + 1 offsets per row
+ * (n_seq[b] < seq_stride) and the sequences' tokens; they are not checked. */
+#define PKV_RULE_BIAS 1     /* flags[b]: sequence bias */
+#define PKV_RULE_BAN 2      /* no-repeat n-grams or min_new_tokens: "set to -inf" */
+#define PKV_RULE_BAD 4      /* bad words: "add -inf" */
+#define PKV_RULE_STOP 8     /* stop sequences */
+#define PKV_SEQ_BIAS 0      /* seq_kind values */
+#define PKV_SEQ_BAD 1
+#define PKV_SEQ_STOP 2
+typedef struct pkv_token_rules_desc {
+    uint32_t struct_bytes;  /* = sizeof(pkv_token_rules_desc) */
+    int32_t device;
+    int32_t batch;
+    int32_t vocab;
+    int32_t* history; int64_t history_stride;   /* int32 [batch, history_stride] */
+    int32_t* history_len;                       /* [batch] device arrays */
+    const int32_t* prompt_len;
+    const int32_t* flags;
+    const int32_t* ngram;
+    const int32_t* min_new_tokens;
+    const int32_t* n_seq;
+    const int32_t* seq_off; const int32_t* seq_kind; const float* seq_bias; int64_t seq_stride;   /* [batch, seq_stride] */
+    const int32_t* seq_tokens; int64_t tokens_stride;                                                /* [batch, tokens_stride] */
+    const int32_t* eos; int32_t n_eos;          /* the EOS ids of min_new_tokens */
+    int32_t reserved;
+    const int64_t* append; int64_t append_stride; int64_t append_column;   /* optional (null): the token to append */
+    float* bias; int64_t bias_stride;           /* fp32 [batch, bias_stride] */
+    uint32_t* ban; int64_t ban_stride;          /* uint32 [batch, ban_stride] */
+    uint8_t* stop;                              /* [batch] */
+} pkv_token_rules_desc;
+int pkv_token_rules(const pkv_token_rules_desc* d, void* stream);
+
+/* ---- the penalized draw with the rule terms of pkv_token_rules (DESIGN.md §4.11) ----
+ * Row b with f = flags[b]: x_v = f32(logit_v); f & PKV_RULE_BIAS: x_v = x_v + bias[b*bias_stride + v]; then steps 2-3 of
+ * pkv_sample_tokens_penalized; then f & PKV_RULE_BAN and bit v of the "set" words of ban[b*ban_stride ..]: x_v = -inf;
+ * otherwise, f & PKV_RULE_BAD: x_v = x_v + (-inf if bit v of the "add" words is set, else 0) (so a +inf logit becomes
+ * NaN, as in HF); then steps 4-5 of pkv_sample_tokens_penalized on x. Each operation is one IEEE fp32 operation. A row with
+ * f & 7 == 0 reads none of bias and ban and gets exactly pkv_sample_tokens_penalized's token. Same launch properties as
+ * pkv_sample_tokens. PKV_ERR_INVALID_ARG: those of pkv_sample_tokens_penalized, a null rules struct or struct_bytes
+ * mismatch, null or misaligned (4 bytes) flags / bias / ban, bias_stride < vocab, ban_stride < 2 * ceil(vocab / 32). */
+typedef struct pkv_sample_rules {
+    uint32_t struct_bytes;  /* = sizeof(pkv_sample_rules) */
+    uint32_t reserved;
+    const int32_t* flags;                      /* [batch] */
+    const float* bias; int64_t bias_stride;    /* as written by pkv_token_rules */
+    const uint32_t* ban; int64_t ban_stride;
+} pkv_sample_rules;
+int pkv_sample_tokens_constrained(const pkv_sample_desc* d, const pkv_sample_penalty* p, const pkv_sample_rules* r,
+                                  void* stream);
+
 /* ---- token log-probabilities: the log-softmax of each row of logits at a token and at its top N (DESIGN.md §4.8) ----
  * Row b (logits[b*logits_stride .. + vocab), bf16 / fp16) is read as the model's raw distribution: x_i = f32(logit_i),
  * temperature 1, no filters (whatever a sampler does with the row). With m = max_i x_i and Z = sum_i expf(x_i - m), summed

@@ -24,8 +24,10 @@ EXPORTS = [
     "pkv_decode_attn_batch_fp8", "pkv_cache_quantize_fp8", "pkv_decode_attn_batch_gqa", "pkv_decode_attn_batch_gqa_fp8",
     "pkv_evict_pooled_kv_offset", "pkv_cache_install", "pkv_sample_tokens", "pkv_decode_attn_window",
     "pkv_decode_attn_heavy", "pkv_decode_heavy_workspace_bytes",
-    "pkv_token_logprobs", "pkv_sample_tokens_penalized",
+    "pkv_token_logprobs", "pkv_sample_tokens_penalized", "pkv_token_rules", "pkv_sample_tokens_constrained",
 ]
+RULE_BIAS, RULE_BAN, RULE_BAD, RULE_STOP = 1, 2, 4, 8     # pkv_token_rules_desc.flags[b]
+SEQ_BIAS, SEQ_BAD, SEQ_STOP = 0, 1, 2                     # pkv_token_rules_desc.seq_kind
 FLAG_GQA_SHARED = 128          # pkv_evict_desc.flags: one compacted cache per KV head
 
 
@@ -108,6 +110,26 @@ class SamplePenalty(C.Structure):
         ("struct_bytes", C.c_uint32), ("reserved", C.c_uint32),
         ("repetition_penalty", C.c_void_p), ("presence_penalty", C.c_void_p), ("frequency_penalty", C.c_void_p),
         ("min_p", C.c_void_p), ("prompt_mask", C.c_void_p), ("counts", C.c_void_p), ("stride", C.c_int64),
+    ]
+
+
+class TokenRulesDesc(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("device", C.c_int32), ("batch", C.c_int32), ("vocab", C.c_int32),
+        ("history", C.c_void_p), ("history_stride", C.c_int64), ("history_len", C.c_void_p), ("prompt_len", C.c_void_p),
+        ("flags", C.c_void_p), ("ngram", C.c_void_p), ("min_new_tokens", C.c_void_p), ("n_seq", C.c_void_p),
+        ("seq_off", C.c_void_p), ("seq_kind", C.c_void_p), ("seq_bias", C.c_void_p), ("seq_stride", C.c_int64),
+        ("seq_tokens", C.c_void_p), ("tokens_stride", C.c_int64), ("eos", C.c_void_p), ("n_eos", C.c_int32),
+        ("reserved", C.c_int32), ("append", C.c_void_p), ("append_stride", C.c_int64), ("append_column", C.c_int64),
+        ("bias", C.c_void_p), ("bias_stride", C.c_int64), ("ban", C.c_void_p), ("ban_stride", C.c_int64),
+        ("stop", C.c_void_p),
+    ]
+
+
+class SampleRules(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("reserved", C.c_uint32), ("flags", C.c_void_p),
+        ("bias", C.c_void_p), ("bias_stride", C.c_int64), ("ban", C.c_void_p), ("ban_stride", C.c_int64),
     ]
 
 
@@ -217,6 +239,10 @@ def lib() -> C.CDLL:
     L.pkv_sample_tokens.restype = i32
     L.pkv_sample_tokens_penalized.argtypes = [C.POINTER(SampleDesc), C.POINTER(SamplePenalty), p]
     L.pkv_sample_tokens_penalized.restype = i32
+    L.pkv_token_rules.argtypes = [C.POINTER(TokenRulesDesc), p]
+    L.pkv_token_rules.restype = i32
+    L.pkv_sample_tokens_constrained.argtypes = [C.POINTER(SampleDesc), C.POINTER(SamplePenalty), C.POINTER(SampleRules), p]
+    L.pkv_sample_tokens_constrained.restype = i32
     L.pkv_token_logprobs.argtypes = [C.POINTER(LogprobsDesc), p]
     L.pkv_token_logprobs.restype = i32
     if L.pkv_version() != 3:

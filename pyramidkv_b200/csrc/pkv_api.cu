@@ -890,8 +890,10 @@ int pkv_update_flatten_view(void* dst, const void* src, const void* state, const
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "flatten append launch");
 }
 
-// The checks of pkv_sample_tokens, then its launch, or the penalized one when `pen` is set (already checked).
-static int sample(const char* fn, const pkv_sample_desc* d, const pkv_sample_penalty* pen, void* stream) {
+// The checks of pkv_sample_tokens, then its launch, or the penalized one when `pen` is set, or the constrained one when `rules`
+// is also set (both already checked).
+static int sample(const char* fn, const pkv_sample_desc* d, const pkv_sample_penalty* pen, void* stream,
+                  const pkv_sample_rules* rules = nullptr) {
     if (!d) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
     if (d->struct_bytes != sizeof(pkv_sample_desc))
         return fail(PKV_ERR_INVALID_ARG, "pkv_sample_desc.struct_bytes=%u, library expects %zu (ABI mismatch)", d->struct_bytes, sizeof(pkv_sample_desc));
@@ -926,21 +928,87 @@ static int sample(const char* fn, const pkv_sample_desc* d, const pkv_sample_pen
     PenaltyArgs p;
     p.repetition = pen->repetition_penalty; p.presence = pen->presence_penalty; p.frequency = pen->frequency_penalty;
     p.min_p = pen->min_p; p.mask = pen->prompt_mask; p.counts = pen->counts; p.ld = pen->stride;
-    const cudaError_t e = launch_sample_penalized(a, p, static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "penalized sample launch");
+    if (!rules) {
+        const cudaError_t e = launch_sample_penalized(a, p, static_cast<cudaStream_t>(stream));
+        return e == cudaSuccess ? PKV_OK : fail_cuda(e, "penalized sample launch");
+    }
+    const int64_t W = (d->vocab + 31) / 32;
+    if (rules->bias_stride < d->vocab || rules->ban_stride < 2 * W)
+        return fail(PKV_ERR_INVALID_ARG, "%s: bias_stride=%lld < vocab=%lld or ban_stride=%lld < %lld", fn, (long long)rules->bias_stride,
+                    (long long)d->vocab, (long long)rules->ban_stride, (long long)(2 * W));
+    RuleTermArgs q;
+    q.flags = rules->flags; q.bias = rules->bias; q.bias_ld = rules->bias_stride; q.ban = rules->ban; q.ban_ld = rules->ban_stride;
+    q.W = int(W);
+    const cudaError_t e = launch_sample_constrained(a, p, q, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "constrained sample launch");
 }
 
 int pkv_sample_tokens(const pkv_sample_desc* d, void* stream) { return sample("pkv_sample_tokens", d, nullptr, stream); }
 
-int pkv_sample_tokens_penalized(const pkv_sample_desc* d, const pkv_sample_penalty* pen, void* stream) {
-    const char* fn = "pkv_sample_tokens_penalized";
+static int check_penalty(const char* fn, const pkv_sample_penalty* pen) {
     if (!pen || pen->struct_bytes != sizeof(pkv_sample_penalty))
         return fail(PKV_ERR_INVALID_ARG, "%s: null pkv_sample_penalty or struct_bytes != %zu (ABI mismatch)", fn, sizeof(pkv_sample_penalty));
     const auto bad = [](const void* ptr, uintptr_t align) { return !ptr || (reinterpret_cast<uintptr_t>(ptr) & (align - 1)); };
     if (bad(pen->repetition_penalty, 4) || bad(pen->presence_penalty, 4) || bad(pen->frequency_penalty, 4) || bad(pen->min_p, 4))
         return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned repetition / presence / frequency penalty or min_p (4 bytes)", fn);
     if (bad(pen->prompt_mask, 1) || bad(pen->counts, 4)) return fail(PKV_ERR_INVALID_ARG, "%s: null prompt_mask, or null or misaligned counts (4 bytes)", fn);
-    return sample(fn, d, pen, stream);
+    return PKV_OK;
+}
+
+int pkv_sample_tokens_penalized(const pkv_sample_desc* d, const pkv_sample_penalty* pen, void* stream) {
+    const char* fn = "pkv_sample_tokens_penalized";
+    const int rc = check_penalty(fn, pen);
+    return rc ? rc : sample(fn, d, pen, stream);
+}
+
+int pkv_sample_tokens_constrained(const pkv_sample_desc* d, const pkv_sample_penalty* pen, const pkv_sample_rules* r,
+                                  void* stream) {
+    const char* fn = "pkv_sample_tokens_constrained";
+    int rc = check_penalty(fn, pen);
+    if (rc) return rc;
+    if (!r || r->struct_bytes != sizeof(pkv_sample_rules))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null pkv_sample_rules or struct_bytes != %zu (ABI mismatch)", fn, sizeof(pkv_sample_rules));
+    const auto bad = [](const void* ptr, uintptr_t align) { return !ptr || (reinterpret_cast<uintptr_t>(ptr) & (align - 1)); };
+    if (bad(r->flags, 4) || bad(r->bias, 4) || bad(r->ban, 4))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned flags / bias / ban (4 bytes)", fn);
+    return sample(fn, d, pen, stream, r);
+}
+
+int pkv_token_rules(const pkv_token_rules_desc* d, void* stream) {
+    const char* fn = "pkv_token_rules";
+    if (!d) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
+    if (d->struct_bytes != sizeof(pkv_token_rules_desc))
+        return fail(PKV_ERR_INVALID_ARG, "pkv_token_rules_desc.struct_bytes=%u, library expects %zu (ABI mismatch)", d->struct_bytes, sizeof(pkv_token_rules_desc));
+    if (d->batch < 1 || d->batch > (1 << 20)) return fail(PKV_ERR_INVALID_ARG, "%s: batch=%d outside [1, 2^20]", fn, d->batch);
+    if (d->vocab < 1 || d->vocab > (1 << 24)) return fail(PKV_ERR_INVALID_ARG, "%s: vocab=%d outside [1, 2^24]", fn, d->vocab);
+    const int64_t W = (int64_t(d->vocab) + 31) / 32;
+    if (d->history_stride < 1 || d->history_stride > INT32_MAX || d->bias_stride < d->vocab || d->ban_stride < 2 * W ||
+        d->seq_stride < 2 || d->tokens_stride < 1 || d->n_eos < 0)
+        return fail(PKV_ERR_INVALID_ARG, "%s: history_stride=%lld, bias_stride=%lld (vocab %d), ban_stride=%lld (>= %lld), seq_stride=%lld, "
+                    "tokens_stride=%lld or n_eos=%d out of range", fn, (long long)d->history_stride, (long long)d->bias_stride, d->vocab,
+                    (long long)d->ban_stride, (long long)(2 * W), (long long)d->seq_stride, (long long)d->tokens_stride, d->n_eos);
+    const auto bad = [](const void* ptr, uintptr_t align) { return !ptr || (reinterpret_cast<uintptr_t>(ptr) & (align - 1)); };
+    if (bad(d->history, 4) || bad(d->history_len, 4) || bad(d->prompt_len, 4) || bad(d->flags, 4) || bad(d->ngram, 4) ||
+        bad(d->min_new_tokens, 4) || bad(d->n_seq, 4) || bad(d->seq_off, 4) || bad(d->seq_kind, 4) || bad(d->seq_bias, 4) ||
+        bad(d->seq_tokens, 4) || bad(d->bias, 4) || bad(d->ban, 4) || bad(d->stop, 1) || (d->n_eos > 0 && bad(d->eos, 4)))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned device array (4 bytes)", fn);
+    if (d->append && ((reinterpret_cast<uintptr_t>(d->append) & 7u) || d->append_column < 0 || d->append_column >= d->append_stride))
+        return fail(PKV_ERR_INVALID_ARG, "%s: misaligned append (8 bytes) or append_column=%lld outside [0, append_stride=%lld)", fn,
+                    (long long)d->append_column, (long long)d->append_stride);
+    const DevInfo* di = nullptr;
+    const int rc = device_info(d->device, &di);
+    if (rc) return rc;
+    TokenRulesArgs a;
+    a.B = d->batch; a.V = d->vocab; a.W = int(W); a.n_eos = d->n_eos;
+    a.hist = d->history; a.hist_ld = d->history_stride; a.hist_len = d->history_len; a.prompt_len = d->prompt_len;
+    a.flags = d->flags; a.ngram = d->ngram; a.min_new = d->min_new_tokens; a.n_seq = d->n_seq;
+    a.seq_off = d->seq_off; a.seq_kind = d->seq_kind; a.seq_bias = d->seq_bias; a.seq_ld = d->seq_stride;
+    a.seq_tok = d->seq_tokens; a.tok_ld = d->tokens_stride; a.eos = d->eos;
+    a.append = d->append; a.append_ld = d->append_stride; a.append_col = d->append_column;
+    a.bias = d->bias; a.bias_ld = d->bias_stride; a.ban = d->ban; a.ban_ld = d->ban_stride; a.stop = d->stop;
+    DeviceGuard guard(d->device);
+    const cudaError_t e = launch_token_rules(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "token rules launch");
 }
 
 int pkv_token_logprobs(const pkv_logprobs_desc* d, void* stream) {

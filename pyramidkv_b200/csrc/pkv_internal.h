@@ -213,6 +213,36 @@ struct PenaltyArgs {
     int64_t ld;
 };
 cudaError_t launch_sample_penalized(const SampleArgs& a, const PenaltyArgs& p, cudaStream_t st);
+// the rule terms of pkv_sample_tokens_constrained, per row b (flags: PKV_RULE_*)
+struct RuleTermArgs {
+    const int32_t* flags;       // [B]
+    const float* bias;          // bias[b * bias_ld + v]
+    int64_t bias_ld;
+    const uint32_t* ban;        // words [0, W) of row b: set to -inf; [W, 2W): add -inf
+    int64_t ban_ld;
+    int W;
+};
+cudaError_t launch_sample_constrained(const SampleArgs& a, const PenaltyArgs& p, const RuleTermArgs& q, cudaStream_t st);
+
+// the per-row rule terms of one step from the token history (pkv_rules.cu): one CTA per row
+struct TokenRulesArgs {
+    int B, V, W, n_eos;
+    int32_t* hist; int64_t hist_ld;
+    int32_t* hist_len;
+    const int32_t* prompt_len;
+    const int32_t* flags;
+    const int32_t* ngram;
+    const int32_t* min_new;
+    const int32_t* n_seq;
+    const int32_t* seq_off; const int32_t* seq_kind; const float* seq_bias; int64_t seq_ld;
+    const int32_t* seq_tok; int64_t tok_ld;
+    const int32_t* eos;
+    const int64_t* append; int64_t append_ld, append_col;   // optional
+    float* bias; int64_t bias_ld;
+    uint32_t* ban; int64_t ban_ld;
+    uint8_t* stop;
+};
+cudaError_t launch_token_rules(const TokenRulesArgs& a, cudaStream_t st);
 
 // log-probabilities of one row of logits at a token and at its top N (pkv_logprobs.cu): one CTA per row
 constexpr int kMaxTopLogprobs = 20;

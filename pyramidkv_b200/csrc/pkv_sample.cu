@@ -258,6 +258,12 @@ struct PenRow {
     bool use_mask;      // repetition_penalty != 1
     bool pen;           // some penalty is on: counts (and the mask) are read
     float rho, pres, freq;
+    // the rule terms of the constrained form (pkv_sample_tokens_constrained); rules = 0 in the penalized form
+    int rules;          // PKV_RULE_BIAS | PKV_RULE_BAN | PKV_RULE_BAD of the row
+    bool vec_bias;      // 16-byte bias loads
+    const float* bias;
+    const uint32_t* ban;
+    int W;
 };
 
 __device__ __forceinline__ float penalize(const PenRow& r, float x, uint32_t in_prompt, int c) {
@@ -266,13 +272,15 @@ __device__ __forceinline__ float penalize(const PenRow& r, float x, uint32_t in_
     return x;
 }
 
-// x of elements 4g .. 4g+3 (those past V are not meaningful: callers test i < V)
-template <typename E>
-__device__ __forceinline__ void load_x4(const PenRow& r, int g, float (&x)[4]) {
-    uint32_t bb[4];
-    load4(r.lg, g, r.V, r.vec, bb);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) x[j] = DT<E>::to_f32(uint16_t(bb[j]));
+// the bans of element i after the penalties: set to -inf (n-grams, min_new_tokens), else add -inf or 0 (bad words)
+__device__ __forceinline__ float ban_term(const PenRow& r, float x, int i) {
+    if ((r.rules & PKV_RULE_BAN) && ((__ldg(r.ban + (i >> 5)) >> (i & 31)) & 1u)) return -INFINITY;
+    if (r.rules & PKV_RULE_BAD) x = __fadd_rn(x, ((__ldg(r.ban + r.W + (i >> 5)) >> (i & 31)) & 1u) ? -INFINITY : 0.f);
+    return x;
+}
+
+// steps 2-3 (the penalties) on elements 4g .. 4g+3
+__device__ __forceinline__ void penalize4(const PenRow& r, int g, float (&x)[4]) {
     if (!r.pen) return;
     const int i = 4 * g;
     int c[4];
@@ -296,18 +304,48 @@ __device__ __forceinline__ void load_x4(const PenRow& r, int g, float (&x)[4]) {
     for (int j = 0; j < 4; ++j) x[j] = penalize(r, x[j], mk[j], c[j]);
 }
 
-template <typename E>
+// x of elements 4g .. 4g+3 (those past V are not meaningful: callers test i < V); kRules adds the rule terms
+template <typename E, bool kRules>
+__device__ __forceinline__ void load_x4(const PenRow& r, int g, float (&x)[4]) {
+    uint32_t bb[4];
+    load4(r.lg, g, r.V, r.vec, bb);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) x[j] = DT<E>::to_f32(uint16_t(bb[j]));
+    const int i = 4 * g;
+    if (kRules && (r.rules & PKV_RULE_BIAS)) {
+        if (r.vec_bias && i + 3 < r.V) {
+            const float4 bv = __ldg(reinterpret_cast<const float4*>(r.bias) + g);
+            x[0] = __fadd_rn(x[0], bv.x); x[1] = __fadd_rn(x[1], bv.y); x[2] = __fadd_rn(x[2], bv.z); x[3] = __fadd_rn(x[3], bv.w);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if (i + j < r.V) x[j] = __fadd_rn(x[j], __ldg(r.bias + i + j));
+        }
+    }
+    penalize4(r, g, x);
+    if (kRules && (r.rules & (PKV_RULE_BAN | PKV_RULE_BAD))) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (i + j < r.V) x[j] = ban_term(r, x[j], i + j);
+    }
+}
+
+template <typename E, bool kRules>
 __device__ __forceinline__ float load_x1(const PenRow& r, int i) {
-    const float x = DT<E>::to_f32(__ldg(r.lg + i));
-    if (!r.pen) return x;
-    return penalize(r, x, r.use_mask ? uint32_t(__ldg(r.mask + i)) : 0u, __ldg(r.cnt + i));
+    float x = DT<E>::to_f32(__ldg(r.lg + i));
+    if (kRules && (r.rules & PKV_RULE_BIAS)) x = __fadd_rn(x, __ldg(r.bias + i));
+    if (r.pen) x = penalize(r, x, r.use_mask ? uint32_t(__ldg(r.mask + i)) : 0u, __ldg(r.cnt + i));
+    if (kRules && (r.rules & (PKV_RULE_BAN | PKV_RULE_BAD))) x = ban_term(r, x, i);
+    return x;
 }
 
 // The walks of sample_kernel, over 32-bit keys of x (okey32) in four 8-bit digits: the penalties do not keep the order of
 // the logits. Level 0 histograms the top digit; level lv > 0 the digit below `prefix` (the lv digits chosen so far).
-template <typename E>
+// kRules (pkv_sample_tokens_constrained) adds the rule terms of RuleTermArgs to x; rows with none read nothing of them.
+template <typename E, bool kRules>
 __global__ void __launch_bounds__(kThreads, 1) sample_penalized_kernel(const __grid_constant__ SampleArgs a,
-                                                                       const __grid_constant__ PenaltyArgs p) {
+                                                                       const __grid_constant__ PenaltyArgs p,
+                                                                       const __grid_constant__ RuleTermArgs q) {
     __shared__ Shared S;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     Hist& H = *reinterpret_cast<Hist*>(smem_raw);
@@ -326,6 +364,11 @@ __global__ void __launch_bounds__(kThreads, 1) sample_penalized_kernel(const __g
     const float minp = p.min_p[row];
     r.use_mask = r.rho != 1.f;
     r.pen = r.use_mask || r.pres != 0.f || r.freq != 0.f;
+    r.rules = kRules ? (q.flags[row] & (PKV_RULE_BIAS | PKV_RULE_BAN | PKV_RULE_BAD)) : 0;
+    r.bias = kRules ? q.bias + int64_t(row) * q.bias_ld : nullptr;
+    r.ban = kRules ? q.ban + int64_t(row) * q.ban_ld : nullptr;
+    r.W = q.W;
+    r.vec_bias = (reinterpret_cast<uintptr_t>(r.bias) & 15u) == 0;
     const float T = a.temperature[row];
     const int K = a.top_k[row];
     const float P = a.top_p[row];
@@ -342,7 +385,7 @@ __global__ void __launch_bounds__(kThreads, 1) sample_penalized_kernel(const __g
     int bi = 0x7fffffff;
     for (int g = tid; 4 * g < V; g += kThreads) {
         float x[4];
-        load_x4<E>(r, g, x);
+        load_x4<E, kRules>(r, g, x);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int i = 4 * g + j;
@@ -367,7 +410,7 @@ __global__ void __launch_bounds__(kThreads, 1) sample_penalized_kernel(const __g
                     const int hs = 32 - 8 * lv, ds = 24 - 8 * lv;
                     for (int g = tid; 4 * g < V; g += kThreads) {
                         float x[4];
-                        load_x4<E>(r, g, x);
+                        load_x4<E, kRules>(r, g, x);
 #pragma unroll
                         for (int j = 0; j < 4; ++j) {
                             const uint32_t k = okey32(x[j]);
@@ -390,7 +433,7 @@ __global__ void __launch_bounds__(kThreads, 1) sample_penalized_kernel(const __g
         unsigned long long z = 0;
         for (int g = tid; 4 * g < V; g += kThreads) {
             float x[4];
-            load_x4<E>(r, g, x);
+            load_x4<E, kRules>(r, g, x);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 if (4 * g + j < V) {
@@ -417,7 +460,7 @@ __global__ void __launch_bounds__(kThreads, 1) sample_penalized_kernel(const __g
                     const int hs = 32 - 8 * lv, ds = 24 - 8 * lv;
                     for (int g = tid; 4 * g < V; g += kThreads) {
                         float x[4];
-                        load_x4<E>(r, g, x);
+                        load_x4<E, kRules>(r, g, x);
 #pragma unroll
                         for (int j = 0; j < 4; ++j) {
                             const uint32_t k = okey32(x[j]);
@@ -444,7 +487,7 @@ __global__ void __launch_bounds__(kThreads, 1) sample_penalized_kernel(const __g
             unsigned long long above = 0, ties = 0;
             for (int g = tid; 4 * g < V; g += kThreads) {
                 float x[4];
-                load_x4<E>(r, g, x);
+                load_x4<E, kRules>(r, g, x);
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     if (4 * g + j < V) {
@@ -459,7 +502,7 @@ __global__ void __launch_bounds__(kThreads, 1) sample_penalized_kernel(const __g
             const unsigned long long e_tau = fixed_mass(tau, m);
             const unsigned long long need = (e_tau && above < target) ? (target - above + e_tau - 1) / e_tau : 1;
             if (need < ties)
-                cut = nth_index(S, V, (long long)need, [&](int i) { return __fdiv_rn(load_x1<E>(r, i), T) == tau; });
+                cut = nth_index(S, V, (long long)need, [&](int i) { return __fdiv_rn(load_x1<E, kRules>(r, i), T) == tau; });
         }
         // Gumbel-max over the kept set {y > tau} + {y == tau, index <= cut}, less the tokens min-p drops
         float bs = -INFINITY;
@@ -468,7 +511,7 @@ __global__ void __launch_bounds__(kThreads, 1) sample_penalized_kernel(const __g
         const uint32_t t0 = uint32_t(uint64_t(t)), t1 = uint32_t(uint64_t(t) >> 32);
         for (int g = tid; 4 * g < V; g += kThreads) {
             float x[4];
-            load_x4<E>(r, g, x);
+            load_x4<E, kRules>(r, g, x);
             bool keep[4], any = false;
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
@@ -499,12 +542,12 @@ __global__ void __launch_bounds__(kThreads, 1) sample_penalized_kernel(const __g
     }
 }
 
-template <typename E>
-cudaError_t launch_sample_penalized_t(const SampleArgs& a, const PenaltyArgs& p, cudaStream_t st) {
-    const cudaError_t attr =
-        cudaFuncSetAttribute(sample_penalized_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kHistBytes));
+template <typename E, bool kRules>
+cudaError_t launch_sample_penalized_t(const SampleArgs& a, const PenaltyArgs& p, const RuleTermArgs& q, cudaStream_t st) {
+    const cudaError_t attr = cudaFuncSetAttribute(sample_penalized_kernel<E, kRules>,
+                                                  cudaFuncAttributeMaxDynamicSharedMemorySize, int(kHistBytes));
     if (attr != cudaSuccess) return attr;
-    sample_penalized_kernel<E><<<a.B, kThreads, kHistBytes, st>>>(a, p);
+    sample_penalized_kernel<E, kRules><<<a.B, kThreads, kHistBytes, st>>>(a, p, q);
     count_launch();
     return cudaGetLastError();
 }
@@ -516,7 +559,14 @@ cudaError_t launch_sample(const SampleArgs& a, cudaStream_t st) {
 }
 
 cudaError_t launch_sample_penalized(const SampleArgs& a, const PenaltyArgs& p, cudaStream_t st) {
-    return a.dtype == PKV_BF16 ? launch_sample_penalized_t<__nv_bfloat16>(a, p, st) : launch_sample_penalized_t<__half>(a, p, st);
+    const RuleTermArgs none{};
+    return a.dtype == PKV_BF16 ? launch_sample_penalized_t<__nv_bfloat16, false>(a, p, none, st)
+                               : launch_sample_penalized_t<__half, false>(a, p, none, st);
+}
+
+cudaError_t launch_sample_constrained(const SampleArgs& a, const PenaltyArgs& p, const RuleTermArgs& q, cudaStream_t st) {
+    return a.dtype == PKV_BF16 ? launch_sample_penalized_t<__nv_bfloat16, true>(a, p, q, st)
+                               : launch_sample_penalized_t<__half, true>(a, p, q, st);
 }
 
 }  // namespace pkv

@@ -33,7 +33,12 @@ only on its logits, its parameters and its seed, not on its batch position, slot
 frequency penalties and min-p (HF's RepetitionPenaltyLogitsProcessor and MinPLogitsWarper, vLLM's presence / frequency
 penalties) are applied on the device from a per-row prompt mask and generated-token count table, in one
 `pkv_sample_tokens_penalized` launch per step instead (DESIGN.md §4.10); `SamplingParams(temperature=0,
-repetition_penalty=r)` is HF's `generate(do_sample=False, repetition_penalty=r)`.
+repetition_penalty=r)` is HF's `generate(do_sample=False, repetition_penalty=r)`. Its generation constraints (sequence
+bias, no-repeat n-grams, bad words, min_new_tokens and stop sequences: HF's SequenceBias, NoRepeatNGram, NoBadWords and
+MinNewTokensLength processors and a stopping criterion over the ids) read each row's token history on the device - its
+whole prompt, however much of it the compacted cache keeps, then every generated token - through one `pkv_token_rules`
+launch after each draw and one `pkv_sample_tokens_constrained` launch in place of the penalized one (DESIGN.md §4.11). A
+sequence that completes a stop sequence ends there like one that emitted EOS.
 
 `logprobs=N` (0 to 20) in any of the three loops also returns one `TokenLogprobs` per prompt: the log-probability of every
 generated token and the N most likely tokens at each position, under the model's raw distribution (log_softmax of the
@@ -44,6 +49,7 @@ log-probabilities over the compacted cache: the likelihood a cache form gives a 
 from __future__ import annotations
 
 import math
+import operator
 import time
 from dataclasses import dataclass
 from typing import List, Optional
@@ -61,7 +67,11 @@ class SamplingParams:
     Gumbel-max draw (DESIGN.md §4.6). repetition_penalty (> 0; 1: off) divides the positive and multiplies the negative
     logits of the prompt's and the generated tokens; presence_penalty and frequency_penalty (0: off) subtract, from each
     generated token's logit, the penalty and the penalty times its count (vLLM's order, after the repetition penalty); min_p
-    (in [0, 1]; 0: off) drops the tokens whose probability is below min_p times the largest (DESIGN.md §4.10)."""
+    (in [0, 1]; 0: off) drops the tokens whose probability is below min_p times the largest (DESIGN.md §4.10).
+    The constraints (DESIGN.md §4.11; every default leaves its rule off) come first, in HF's order around the penalties:
+    sequence_bias ((token-id tuple, bias) pairs), no_repeat_ngram_size, bad_words_ids (token-id tuples), min_new_tokens
+    (EOS is banned until that many tokens are generated), and stop_sequences (token-id tuples: the sequence ends with the
+    token that completes one, kept). Lists are frozen to tuples."""
     temperature: float = 1.0
     top_k: int = 0
     top_p: float = 1.0
@@ -70,6 +80,11 @@ class SamplingParams:
     presence_penalty: float = 0.0
     frequency_penalty: float = 0.0
     min_p: float = 0.0
+    sequence_bias: tuple = ()
+    no_repeat_ngram_size: int = 0
+    bad_words_ids: tuple = ()
+    min_new_tokens: int = 0
+    stop_sequences: tuple = ()
 
     def __post_init__(self):
         if not float(self.temperature) >= 0.0:
@@ -87,12 +102,107 @@ class SamplingParams:
                 raise ValueError(f"SamplingParams: {name} must be finite, got {getattr(self, name)}")
         if not 0.0 <= float(self.min_p) <= 1.0:
             raise ValueError(f"SamplingParams: min_p must be in [0, 1], got {self.min_p}")
+        bias = []
+        for pair in self.sequence_bias:
+            if len(pair) != 2:
+                raise ValueError(f"SamplingParams: sequence_bias takes (token ids, bias) pairs, got {pair!r}")
+            ids, w = _token_ids(pair[0], "sequence_bias"), _finite(pair[1])
+            if w is None:
+                raise ValueError(f"SamplingParams: sequence_bias values must be finite numbers, got {pair[1]!r}")
+            if any(ids == b[0] for b in bias):
+                raise ValueError(f"SamplingParams: sequence_bias repeats the sequence {ids}")
+            bias.append((ids, w))
+        object.__setattr__(self, "sequence_bias", tuple(bias))
+        for name in ("bad_words_ids", "stop_sequences"):
+            object.__setattr__(self, name, tuple(_token_ids(s, name) for s in getattr(self, name)))
+        for name in ("no_repeat_ngram_size", "min_new_tokens"):
+            v = getattr(self, name)
+            if isinstance(v, bool) or int(v) != v or int(v) < 0:
+                raise ValueError(f"SamplingParams: {name} must be an integer >= 0, got {v!r}")
+            object.__setattr__(self, name, int(v))
 
     @property
     def penalized(self) -> bool:
         """Some penalty or min-p is on: the draw needs the request's prompt and generated tokens."""
         return (float(self.repetition_penalty) != 1.0 or float(self.presence_penalty) != 0.0
                 or float(self.frequency_penalty) != 0.0 or float(self.min_p) != 0.0)
+
+    @property
+    def constrained(self) -> bool:
+        """Some generation constraint is on: the draw needs the request's token history."""
+        return bool(self.sequence_bias or self.no_repeat_ngram_size or self.bad_words_ids or self.min_new_tokens
+                    or self.stop_sequences)
+
+
+def _finite(w) -> Optional[float]:
+    """A bias value as a Python float (numpy scalars and 0-d tensors included), or None when it is not a finite number."""
+    if isinstance(w, (bool, str, bytes)):
+        return None
+    try:
+        v = float(w)
+    except (TypeError, ValueError):
+        return None
+    return v if math.isfinite(v) else None
+
+
+def _token_ids(seq, what: str) -> tuple:
+    """A sequence of token ids (Python or numpy integers, integer tensors) as a tuple of Python ints."""
+    err = ValueError(f"SamplingParams: every {what} sequence must be a non-empty sequence of token ids >= 0, got {seq!r}")
+    if isinstance(seq, (str, bytes)):
+        raise err
+    try:
+        items = list(seq)
+    except TypeError:
+        raise err from None
+    ids = []
+    for t in items:
+        if isinstance(t, bool):
+            raise err
+        try:
+            v = operator.index(t)
+        except TypeError:
+            raise err from None
+        if v < 0:
+            raise err
+        ids.append(v)
+    if not ids:
+        raise err
+    return tuple(ids)
+
+
+class _StopTail:
+    """The host's stop check of one sequence: `push` each generated token (the prefill's first) and it tells whether the
+    sequence ends there, at an EOS id or at the last token of one of `p`'s stop sequences. It keeps the sequence's last
+    tokens, prompt included, as many as its longest stop sequence: a stop sequence may start inside the prompt."""
+
+    def __init__(self, prompt: torch.Tensor, eos: set, p: Optional[SamplingParams]):
+        self.eos = eos
+        self.stops = () if p is None else p.stop_sequences
+        self.k = max((len(q) for q in self.stops), default=0)
+        self.tail = prompt.reshape(-1)[-self.k:].tolist() if self.k else []
+
+    def push(self, token) -> bool:
+        t = int(token)
+        if self.k:
+            self.tail.append(t)
+            del self.tail[: -self.k]
+        return t in self.eos or any(tuple(self.tail[len(self.tail) - len(q):]) == q for q in self.stops
+                                    if len(q) <= len(self.tail))
+
+
+def _rule_tables(p: SamplingParams, eos: set):
+    """One request's rules as pkv_token_rules reads them: (flags, n-gram size, min_new_tokens, [(tokens, kind, bias)]).
+    Bias sequences are grouped by their last token (the single-token one first, then in the request's order: the order of
+    HF's sums); single-token bad words equal to an EOS id are dropped, and min_new_tokens needs an EOS id, as in HF."""
+    from . import _lib
+    bias = sorted(((s, w) for s, w in p.sequence_bias), key=lambda sw: (sw[0][-1], len(sw[0]) != 1))
+    bad = [s for s in p.bad_words_ids if not (len(s) == 1 and s[0] in eos)]
+    min_new = p.min_new_tokens if eos else 0
+    seqs = ([(s, _lib.SEQ_BIAS, w) for s, w in bias] + [(s, _lib.SEQ_BAD, 0.0) for s in bad]
+            + [(s, _lib.SEQ_STOP, 0.0) for s in p.stop_sequences])
+    flags = ((_lib.RULE_BIAS if bias else 0) | (_lib.RULE_BAN if p.no_repeat_ngram_size or min_new else 0)
+             | (_lib.RULE_BAD if bad else 0) | (_lib.RULE_STOP if p.stop_sequences else 0))
+    return flags, p.no_repeat_ngram_size, min_new, seqs
 
 
 def _seed_i64(seed: int) -> int:
@@ -110,16 +220,25 @@ class SamplingState:
     With penalties (some request sets one, or `penalties=True` for rows that may later take such a request), also the
     state `sample_tokens_penalized` reads: the four penalty parameters per row, the prompt mask (uint8 [B, vocab]) and the
     generated-token counts (int32 [B, vocab]), built from `prompts` (one id tensor per row) and `first` (each row's token
-    drawn so far, counted once; None: nothing generated yet). B * vocab * 5 bytes, allocated only then."""
+    drawn so far, counted once; None: nothing generated yet). B * vocab * 5 bytes, allocated only then.
+
+    With constraints (some request sets one, or `constraints=True`), also the state of `token_rules` and
+    `sample_tokens_constrained` (it implies the penalty state): each row's token history (int32 [B, cap]: the prompt, then
+    `first`, then one token per `rules(append=...)`; `history` reserves cap >= the longest prompt + `history` tokens), its
+    rules packed into flat tables, the `eos` ids the rules use, and their per-step outputs: bias (float32 [B, vocab]), the
+    two ban bitmaps (int32 [B, 2 * ceil(vocab / 32)]) and the stop flags (bool [B, 1]). `rules` must run once before the
+    first constrained draw (the decoders and the prefill do)."""
 
     def __init__(self, params: List[SamplingParams], device, index: int = 0, vocab: Optional[int] = None, prompts=None,
-                 first: Optional[torch.Tensor] = None, penalties: bool = False):
+                 first: Optional[torch.Tensor] = None, penalties: bool = False, constraints: bool = False, eos=None,
+                 history: int = 0):
         self.temperature = torch.tensor([float(p.temperature) for p in params], dtype=torch.float32, device=device)
         self.top_k = torch.tensor([min(int(p.top_k), 2 ** 31 - 1) for p in params], dtype=torch.int32, device=device)
         self.top_p = torch.tensor([float(p.top_p) for p in params], dtype=torch.float32, device=device)
         self.seed = torch.tensor([_seed_i64(p.seed) for p in params], dtype=torch.int64, device=device)
         self.index = torch.full((len(params),), int(index), dtype=torch.int64, device=device)
-        self.penalized = bool(penalties) or any(p.penalized for p in params)
+        self.constrained = bool(constraints) or any(p.constrained for p in params)
+        self.penalized = bool(penalties) or self.constrained or any(p.penalized for p in params)
         if not self.penalized:
             return
         if vocab is None or prompts is None or len(prompts) != len(params):
@@ -130,6 +249,86 @@ class SamplingState:
         self.counts = torch.zeros(len(params), int(vocab), dtype=torch.int32, device=device)
         for row, ids in enumerate(prompts):
             self._set_history(row, ids, None if first is None else first.reshape(-1)[row])
+        if not self.constrained:
+            return
+        B, V = len(params), int(vocab)
+        self.vocab = V
+        self.rule_eos = _eos_set(eos)
+        self.eos = torch.tensor(sorted(self.rule_eos) or [0], dtype=torch.int32, device=device)
+        self.n_eos = len(self.rule_eos)
+        cap = max(int(torch.as_tensor(ids).numel()) for ids in prompts) + (first is not None) + int(history)
+        self.history = torch.zeros(B, max(1, cap), dtype=torch.int32, device=device)
+        for name in ("history_len", "prompt_len", "rule_flags", "ngram", "min_new", "n_seq"):
+            setattr(self, name, torch.zeros(B, dtype=torch.int32, device=device))
+        self.seq_off = torch.zeros(B, 2, dtype=torch.int32, device=device)
+        self.seq_kind = torch.zeros(B, 2, dtype=torch.int32, device=device)
+        self.seq_bias = torch.zeros(B, 2, dtype=torch.float32, device=device)
+        self.seq_tokens = torch.zeros(B, 1, dtype=torch.int32, device=device)
+        self.bias = torch.zeros(B, V, dtype=torch.float32, device=device)
+        self.ban = torch.zeros(B, 2 * ((V + 31) // 32), dtype=torch.int32, device=device)
+        self.stop = torch.zeros(B, 1, dtype=torch.bool, device=device)
+        for row, (p, ids) in enumerate(zip(params, prompts)):
+            self._set_rules(row, p, ids, None if first is None else first.reshape(-1)[row])
+
+    def _check_ids(self, p: SamplingParams, prompt) -> None:
+        """Every id of `prompt` and of `p`'s rule sequences is in [0, vocab)."""
+        V = self.counts.shape[1]
+        ids = torch.as_tensor(prompt).reshape(-1)
+        if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= V):
+            raise ValueError(f"SamplingState: prompt ids outside [0, {V})")
+        rules = [s for s, _ in p.sequence_bias] + list(p.bad_words_ids) + list(p.stop_sequences)
+        if any(max(s) >= V for s in rules):
+            raise ValueError(f"SamplingState: rule token ids outside [0, {V})")
+
+    def _grow(self, name: str, cols: int) -> bool:
+        t = getattr(self, name)
+        if t.shape[1] >= cols:
+            return False
+        new = torch.zeros(t.shape[0], max(cols, 2 * t.shape[1]), dtype=t.dtype, device=t.device)
+        new[:, : t.shape[1]] = t
+        setattr(self, name, new)
+        return True
+
+    def _set_rules(self, row: int, p: SamplingParams, prompt, first) -> bool:
+        """Row `row`'s history (prompt, then `first`) and packed rules; True when a table was reallocated."""
+        flags, ngram, min_new, seqs = _rule_tables(p, self.rule_eos)
+        self._check_ids(p, prompt)
+        hist = torch.as_tensor(prompt).reshape(-1).to(torch.int32)
+        n_prompt = hist.numel()
+        if first is not None:
+            hist = torch.cat([hist, torch.as_tensor(first).reshape(1).to(device=hist.device, dtype=torch.int32)])
+        toks = [t for s, _, _ in seqs for t in s]
+        off = [0]
+        for s, _, _ in seqs:
+            off.append(off[-1] + len(s))
+        grew = self._grow("history", hist.numel())
+        grew |= self._grow("seq_tokens", max(1, len(toks)))
+        for name in ("seq_off", "seq_kind", "seq_bias"):
+            grew |= self._grow(name, len(seqs) + 1)
+        dev = self.history.device
+        self.history[row].zero_()
+        self.history[row, : hist.numel()] = hist.to(dev)
+        self.history_len[row] = hist.numel()
+        self.prompt_len[row] = n_prompt
+        self.rule_flags[row] = flags
+        self.ngram[row] = ngram
+        self.min_new[row] = min_new
+        self.n_seq[row] = len(seqs)
+        self.seq_off[row, : len(off)] = torch.tensor(off, dtype=torch.int32, device=dev)
+        if seqs:
+            self.seq_kind[row, : len(seqs)] = torch.tensor([k for _, k, _ in seqs], dtype=torch.int32, device=dev)
+            self.seq_bias[row, : len(seqs)] = torch.tensor([w for _, _, w in seqs], dtype=torch.float32, device=dev)
+            self.seq_tokens[row, : len(toks)] = torch.tensor(toks, dtype=torch.int32, device=dev)
+        return grew
+
+    def rules(self, backend, append: Optional[torch.Tensor] = None) -> None:
+        """One `token_rules` launch for every row: with `append` ([B, 1] int64), each row's history takes its token
+        first; then the bias, bans and stop flags of the next draw."""
+        backend.token_rules(self, self.vocab, append, 0)
+
+    def rule_state(self) -> list:
+        """The device tensors `rules(append=...)` advances (restored after the warm-up step of a graph capture)."""
+        return [self.history_len, self.bias, self.ban, self.stop] if self.constrained else []
 
     def _set_history(self, row: int, prompt: torch.Tensor, first: Optional[torch.Tensor]) -> None:
         ids = torch.as_tensor(prompt).reshape(-1).to(device=self.counts.device, dtype=torch.long)
@@ -142,26 +341,41 @@ class SamplingState:
         if first is not None:
             self.counts[row].index_fill_(0, torch.as_tensor(first).reshape(1).to(device=self.counts.device, dtype=torch.long), 1)
 
-    def set_row(self, row: int, p: SamplingParams, index: int, prompt=None, first: Optional[torch.Tensor] = None) -> None:
+    def set_row(self, row: int, p: SamplingParams, index: int, prompt=None, first: Optional[torch.Tensor] = None,
+                history: int = 0) -> bool:
         """Row `row` takes the parameters `p` at token index `index`; with penalties, its prompt mask becomes `prompt`'s
-        ids and its counts count `first` (the token drawn so far) once."""
+        ids and its counts count `first` (the token drawn so far) once; with constraints, its history becomes `prompt` +
+        `first` with room for `history` more tokens, and its rules `p`'s. True when a constraint table was reallocated
+        (a captured graph then holds stale pointers); `rules` must run before the row's next draw."""
         if p.penalized and not self.penalized:
             raise ValueError("SamplingState.set_row: a request with penalties or min-p needs a state built with penalties")
+        if p.constrained and not self.constrained:
+            raise ValueError("SamplingState.set_row: a request with constraints needs a state built with constraints")
         if self.penalized and prompt is None:
             raise ValueError("SamplingState.set_row: a state with penalties needs the row's prompt ids")
+        if self.penalized:
+            self._check_ids(p, prompt)                 # before any of the row's state changes
         self.temperature[row] = float(p.temperature)
         self.top_k[row] = min(int(p.top_k), 2 ** 31 - 1)
         self.top_p[row] = float(p.top_p)
         self.seed[row] = _seed_i64(p.seed)
         self.index[row] = int(index)
+        grew = False
         if self.penalized:
             for name in _PENALTY_FIELDS:
                 getattr(self, name)[row] = float(getattr(p, name))
             self._set_history(row, prompt, first)
+        if self.constrained:
+            grew = self._grow("history", torch.as_tensor(prompt).numel() + (first is not None) + int(history))
+            grew |= self._set_rules(row, p, prompt, first)
+        return grew
 
     def draw(self, backend, logits, out, col, advance=True) -> None:
-        """One launch for every row: `sample_tokens`, or `sample_tokens_penalized` when the state has penalties."""
-        if self.penalized:
+        """One launch for every row: `sample_tokens`, or `sample_tokens_penalized` when the state has penalties, or
+        `sample_tokens_constrained` when it has constraints."""
+        if self.constrained:
+            backend.sample_tokens_constrained(logits, self, out, col, advance)
+        elif self.penalized:
             backend.sample_tokens_penalized(logits, self, out, col, advance)
         else:
             backend.sample_tokens(logits, self, out, col, advance)
@@ -267,6 +481,9 @@ class StaticDecoder:
                 raise ValueError(f"StaticDecoder: forced must be [B={self.ids.shape[0]}, {self.max_steps}], got {tuple(forced.shape)}")
             self.forced = forced.to(device=self.ids.device, dtype=torch.long).contiguous()
         self.done = None if self.eos is None else (self.ids == self.eos[None, :]).any(dim=1, keepdim=True)   # [B, 1]
+        if self.constrained:
+            # a stop sequence completed by the first token; from then on each step ORs in its stop flags
+            self.done = self.sampling.stop.clone() if self.done is None else self.done.logical_or_(self.sampling.stop)
         if layers[0].window is not None and self.done is not None:
             # decode window: a finished sequence's later rows would overwrite ring rows its cache keeps, so its row counts
             # leave the range the kernel attends (it reads and writes nothing; its tokens are pad_token_id anyway)
@@ -276,7 +493,7 @@ class StaticDecoder:
             self._stop_finished()
 
     def _setup(self, model, cache, layers, first_token, max_steps, use_graph, eos_token_id, pad_token_id, sampling,
-               logprobs=None, prompts=None, penalties=False) -> None:
+               logprobs=None, prompts=None, penalties=False, constraints=False, history=None) -> None:
         """The state both decoders hold: the step counter and workspace the decode launches read, the per-sequence input
         ids and positions, the token buffer [B, max_steps] and its cursor, the EOS ids, when sampling, the per-sequence
         sampling state with the buffer the sampled tokens land in, and with `logprobs` the buffers of the log-probabilities."""
@@ -306,8 +523,12 @@ class StaticDecoder:
             if len(sampling) != bsz:
                 raise ValueError(f"{len(sampling)} SamplingParams for {bsz} sequences")
             self.sampling = SamplingState(sampling, dev, index=1, vocab=model.lm_head.weight.shape[0], prompts=prompts,
-                                          first=self.ids, penalties=penalties)
+                                          first=self.ids, penalties=penalties, constraints=constraints,
+                                          eos=eos_token_id, history=self.max_steps if history is None else history)
             self.sampled = torch.zeros(bsz, 1, dtype=torch.long, device=dev)
+            if self.sampling.constrained:
+                self.sampling.rules(self.backend)                         # the first step's rule terms and stop flags
+        self.constrained = self.sampling is not None and self.sampling.constrained
         self.forced = None
         self.logprobs = None if logprobs is None else _LogprobBuffers(bsz, self.max_steps, int(logprobs), dev)
         cache._pkv_static = self.state
@@ -346,7 +567,11 @@ class StaticDecoder:
         nxt = self._greedy_token()
         if self.done is not None:
             nxt = torch.where(self.done, self.pad_token_id, nxt)
-            self.done.logical_or_((nxt == self.eos[None, :]).any(dim=1, keepdim=True))
+            if self.eos is not None:
+                self.done.logical_or_((nxt == self.eos[None, :]).any(dim=1, keepdim=True))
+            if self.constrained:
+                self.sampling.rules(self.backend, self.sampled)           # append the token; the next step's rules
+                self.done.logical_or_(self.sampling.stop)
             if self.window_rows is not None:
                 self._stop_finished()
         self.tokens.index_copy_(1, self.cursor, nxt)
@@ -361,8 +586,9 @@ class StaticDecoder:
         counts = self.sampling.counts if self.sampling is not None and self.sampling.penalized else None
         # the heavy-hitter state a step updates (knob pkv_decode_heavy): restored so that the captured step starts from it
         heavy = [t for l in self.layers if l.heavy is not None for t in (l.heavy_scores, l.heavy_gen, l.victim)]
+        rules = self.sampling.rule_state() if self.sampling is not None else []
         return [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done, idx, counts,
-                            self.window_rows) if t is not None] + heavy
+                            self.window_rows) if t is not None] + heavy + rules
 
     def _capture(self) -> None:
         # warm up on a side stream (lazy initialisation, cuBLAS workspaces), restore the counters, then capture
@@ -431,15 +657,19 @@ def _score(model, logits: torch.Tensor, token: torch.Tensor, top_n: int):
     return lp[0], ids[0], top[0]
 
 
-def _prefill(model, input_ids: torch.Tensor, sampling: Optional[SamplingParams] = None, logprobs: Optional[int] = None):
+def _prefill(model, input_ids: torch.Tensor, sampling: Optional[SamplingParams] = None, logprobs: Optional[int] = None,
+             eos=None):
     """Prefill (+ eviction in every patched layer) of one prompt: (first token [1, 1], cache), and with `logprobs` the
-    first token's log-probability entry (`_score`). The token is the argmax, or with `sampling` drawn with token index 0."""
+    first token's log-probability entry (`_score`). The token is the argmax, or with `sampling` drawn with token index 0
+    (with constraints, under the rules of the prompt as history; `eos`: the EOS ids they use)."""
     logits, cache = _prefill_logits(model, input_ids)
     if sampling is None:
         first = logits.argmax(dim=-1, keepdim=True)
     else:
         first = torch.zeros(1, 1, dtype=torch.long, device=logits.device)
-        st = SamplingState([sampling], logits.device, index=0, vocab=logits.shape[1], prompts=[input_ids])
+        st = SamplingState([sampling], logits.device, index=0, vocab=logits.shape[1], prompts=[input_ids], eos=eos)
+        if st.constrained:
+            st.rules(_backend(model))
         st.draw(_backend(model), logits, first, 0, advance=False)
     if logprobs is None:
         return first, cache
@@ -469,23 +699,26 @@ def greedy_generate(model, input_ids: torch.Tensor, max_new_tokens: int, use_gra
     if sampling is not None and not isinstance(sampling, SamplingParams):
         raise ValueError("greedy_generate: sampling must be a SamplingParams")
     logprobs = _check_logprobs(logprobs, "greedy_generate")
-    first, cache, *entry = _prefill(model, input_ids, sampling, logprobs)
+    first, cache, *entry = _prefill(model, input_ids, sampling, logprobs, sorted(eos))
     toks, parts = [first], entry
-    if max_new_tokens > 1 and not (eos and int(first) in eos):
-        # with a decode window the device stops the sequence at its EOS, so that no later row replaces a kept one
+    tail = _StopTail(input_ids, eos, sampling)
+    if max_new_tokens > 1 and not tail.push(first):
+        # with a decode window the device stops the sequence at its EOS, so that no later row replaces a kept one; the
+        # constraints' rules use the EOS ids too
         windowed = eos and getattr(cache.layers[0], "window", None) is not None
+        constrained = sampling is not None and sampling.constrained
         dec = StaticDecoder(model, cache, first, max_new_tokens - 1, use_graph=use_graph,
-                            eos_token_id=sorted(eos) if windowed else None, sampling=None if sampling is None else [sampling],
-                            logprobs=logprobs, prompts=[input_ids])
+                            eos_token_id=sorted(eos) if eos and (windowed or constrained) else None,
+                            sampling=None if sampling is None else [sampling], logprobs=logprobs, prompts=[input_ids])
         keep = max_new_tokens - 1
-        if not eos:
+        if not eos and not tail.stops:
             toks.append(dec.run(max_new_tokens - 1).clone())
         else:
             done, keep = 0, max_new_tokens - 1
             while done < max_new_tokens - 1:
                 n = min(max(1, check_every), max_new_tokens - 1 - done)
                 got = dec.run(n)[0, done:done + n].tolist()              # one device-to-host read per chunk
-                hit = next((i for i, t in enumerate(got) if t in eos), None)
+                hit = next((i for i, t in enumerate(got) if tail.push(t)), None)
                 done += n
                 if hit is not None:
                     keep = done - n + hit + 1
@@ -523,7 +756,7 @@ def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None
     logprobs = _check_logprobs(logprobs, "greedy_generate_batch")
     firsts, caches, entries = [], [], []
     for i, p in enumerate(ids):
-        f, c, *e = _prefill(model, p, None if samp is None else samp[i], logprobs)
+        f, c, *e = _prefill(model, p, None if samp is None else samp[i], logprobs, sorted(eos))
         firsts.append(f)
         caches.append(c)
         entries.append(e)
@@ -534,19 +767,22 @@ def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None
     first_host = first[:, 0].tolist()
     kept = [0] * len(ids)
     gen = torch.empty(len(ids), 0, dtype=torch.long)
-    if steps and not all(t in eos for t in first_host):
+    tails = [_StopTail(p, eos, None if samp is None else samp[b]) for b, p in enumerate(ids)]
+    stops = any(t.stops for t in tails)
+    ended = [t.push(f) for t, f in zip(tails, first_host)]
+    if steps and not all(ended):
         dec = StaticDecoder(model, cache, first, steps, use_graph=use_graph, eos_token_id=sorted(eos) if eos else None,
                             pad_token_id=pad_token_id, sampling=samp, logprobs=logprobs, prompts=ids)
         while dec.taken < steps:
-            dec.run(min(max(1, check_every) if eos else steps, steps - dec.taken))
-            if eos and bool(dec.done.all()):                            # one device-to-host read per chunk
+            dec.run(min(max(1, check_every) if eos or stops else steps, steps - dec.taken))
+            if dec.done is not None and bool(dec.done.all()):           # one device-to-host read per chunk
                 break
         gen = dec.tokens[:, : dec.taken].cpu()
         for b in range(len(ids)):
-            if first_host[b] in eos:
+            if ended[b]:
                 continue
             row = gen[b].tolist()
-            hit = next((i for i, t in enumerate(row) if t in eos), None)
+            hit = next((i for i, t in enumerate(row) if tails[b].push(t)), None)
             kept[b] = len(row) if hit is None else hit + 1
         if logprobs is not None:
             lp, lp_ids, lp_top = dec.logprobs.host(dec.taken)
@@ -574,12 +810,13 @@ class ContinuousDecoder(StaticDecoder):
 
     def __init__(self, model, cache, first_token: torch.Tensor, left, chunk: int, use_graph: Optional[bool] = None,
                  eos_token_id=None, pad_token_id: int = 0, sampling: Optional[List[SamplingParams]] = None,
-                 logprobs: Optional[int] = None, prompts=None, penalties: bool = False):
+                 logprobs: Optional[int] = None, prompts=None, penalties: bool = False, constraints: bool = False,
+                 history: int = 0):
         layers = [l for l in cache.layers if isinstance(l, PkvBatchCacheLayer)]
         if len(layers) != model.config.num_hidden_layers or len(layers) != len(cache.layers):
             raise RuntimeError("ContinuousDecoder needs a batched cache (cache.join_caches) on every layer")
         self._setup(model, cache, layers, first_token, max(1, int(chunk)), use_graph, eos_token_id, pad_token_id, sampling,
-                    logprobs, prompts, penalties)
+                    logprobs, prompts, penalties, constraints, max([int(n) for n in left] + [int(history)]))
         # every layer's row counts are rows of one tensor, so one op per step stops them growing for the done slots
         self.rows_all = torch.stack([l.rows for l in layers])
         for i, l in enumerate(layers):
@@ -595,6 +832,9 @@ class ContinuousDecoder(StaticDecoder):
         stop = self.left <= 0
         if self.eos is not None:
             stop.logical_or_((nxt == self.eos[None, :]).any(dim=1, keepdim=True))
+        if self.constrained:
+            self.sampling.rules(self.backend, self.sampled)
+            stop.logical_or_(self.sampling.stop)
         self.done.logical_or_(stop)
         self.rows_all.view(len(self.layers), self.done.shape[0], -1).sub_(self.done.view(1, -1, 1).to(torch.int32))
         self.tokens.index_copy_(1, self.cursor, nxt)
@@ -640,7 +880,11 @@ class ContinuousDecoder(StaticDecoder):
         if (sampling is None) != (self.sampling is None):
             raise ValueError("admit: pass sampling parameters exactly when the decoder samples")
         if sampling is not None:
-            self.sampling.set_row(slot, sampling, 1, prompt, first_token)     # checks the request before the slot changes
+            # checks the request before the slot changes; a reallocated constraint table needs a new graph
+            if self.sampling.set_row(slot, sampling, 1, prompt, first_token, history=max(0, int(left))):
+                self.graph = None
+            if self.constrained:
+                self.sampling.rules(self.backend)      # every row's history is unchanged but this slot's
         admit_cache(self.cache, slot, src_cache, self.state.step, self.backend)
         self.ids[slot] = first_token.reshape(-1)[:1].to(self.ids.device)
         self.pos[slot] = self.layers[0].seq_seen[slot]
@@ -706,14 +950,21 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
                  prefill_ms=[0.0] * len(ids), cache_rows_first_last=[[] for _ in ids])
     t_start = time.perf_counter()
 
+    tails = [_StopTail(p, eos, None if samp is None else samp[i]) for i, p in enumerate(ids)]
+    ended = [False] * len(ids)                     # the last token pushed ended the sequence (EOS or stop sequence)
+
+    def push(i, t):
+        gen[i].append(t)
+        ended[i] = tails[i].push(t)
+
     def finished(i):
-        return len(gen[i]) >= max(1, caps[i]) or gen[i][-1] in eos
+        return len(gen[i]) >= max(1, caps[i]) or ended[i]
 
     def prefill(i):
         _sync(dev)
         t0 = time.perf_counter()
-        first, cache, *entry = _prefill(model, ids[i], None if samp is None else samp[i], logprobs)
-        gen[i].append(int(first))                  # waits for the prefill
+        first, cache, *entry = _prefill(model, ids[i], None if samp is None else samp[i], logprobs, sorted(eos))
+        push(i, int(first))                        # waits for the prefill
         lps[i].extend(entry)
         ms = (time.perf_counter() - t0) * 1e3
         stats["prefill_ms"][i] = ms
@@ -729,7 +980,8 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     dec = ContinuousDecoder(model, cache, torch.cat(firsts), [0 if finished(b) else caps[b] - 1 for b in range(B)], chunk,
                             use_graph=use_graph, eos_token_id=sorted(eos) if eos else None, pad_token_id=pad_token_id,
                             sampling=None if samp is None else samp[:B], logprobs=logprobs, prompts=ids[:B],
-                            penalties=samp is not None and any(p.penalized for p in samp))
+                            penalties=samp is not None and any(p.penalized for p in samp),
+                            constraints=samp is not None and any(p.constrained for p in samp), history=max(caps))
     waiting = B
     while True:
         for s in range(B):
@@ -757,7 +1009,7 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
         for s in live:
             r = slot_req[s]
             for j, t in enumerate(toks[s].tolist()):
-                gen[r].append(t)
+                push(r, t)
                 stats["live_slot_steps"] += 1
                 if finished(r):
                     break

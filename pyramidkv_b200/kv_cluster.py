@@ -122,6 +122,12 @@ class CudaBackend:
     def sample_tokens_penalized(self, logits, params, out, col, advance=True):
         ops.sample_tokens_penalized(logits, params, out, col, advance)
 
+    def sample_tokens_constrained(self, logits, params, out, col, advance=True):
+        ops.sample_tokens_constrained(logits, params, out, col, advance)
+
+    def token_rules(self, params, vocab, append=None, col=0):
+        ops.token_rules(params, vocab, append, col)
+
     # -- token log-probabilities: the raw log-softmax at a token and at the row's top N --
     def token_logprobs(self, logits, tokens, out_lp, out_ids, out_top, col=0, tokens_col=0, cursor=None):
         ops.token_logprobs(logits, tokens, out_lp, out_ids, out_top, col, tokens_col, cursor)

@@ -853,6 +853,98 @@ def sample_tokens_penalized(logits: torch.Tensor, params, out: torch.Tensor, col
                                                       torch.cuda.current_stream(logits.device).cuda_stream))
 
 
+def _penalty_struct(fn, logits, params):
+    B, V = logits.shape
+    _check_row_params(fn, logits, params, [(n, torch.float32) for n in ("repetition_penalty", "presence_penalty",
+                                                                        "frequency_penalty", "min_p")])
+    mask, counts = params.prompt_mask, params.counts
+    _require_cuda(mask, counts)
+    if (mask.dim() != 2 or mask.dtype != torch.uint8 or counts.dtype != torch.int32 or mask.shape != counts.shape
+            or mask.shape[0] != B or mask.shape[1] < V or not mask.is_contiguous() or not counts.is_contiguous()
+            or mask.device != logits.device or counts.device != logits.device):
+        raise ValueError(f"{fn}: params.prompt_mask / params.counts must be contiguous uint8 / int32 [B={B}, S >= V={V}] "
+                         f"tensors on {logits.device}")
+    p = _lib.SamplePenalty()
+    p.struct_bytes = C.sizeof(_lib.SamplePenalty)
+    p.repetition_penalty, p.presence_penalty = params.repetition_penalty.data_ptr(), params.presence_penalty.data_ptr()
+    p.frequency_penalty, p.min_p = params.frequency_penalty.data_ptr(), params.min_p.data_ptr()
+    p.prompt_mask, p.counts, p.stride = mask.data_ptr(), counts.data_ptr(), mask.shape[1]
+    return p
+
+
+def _check_rule_tensor(fn, name, t, dtype, rows, min_cols=None):
+    ok = t.dtype == dtype and t.is_cuda and t.is_contiguous() and t.shape[0] == rows
+    if min_cols is not None:
+        ok = ok and t.dim() == 2 and t.shape[1] >= min_cols
+    if not ok:
+        raise ValueError(f"{fn}: {name} must be a contiguous CUDA {dtype} tensor of {rows} rows"
+                         + ("" if min_cols is None else f" and >= {min_cols} columns") + f", got {t.dtype} {tuple(t.shape)}")
+
+
+def sample_tokens_constrained(logits: torch.Tensor, params, out: torch.Tensor, col: int, advance: bool = True) -> None:
+    """`sample_tokens_penalized` with the rule terms `token_rules` wrote (include/pkv.h: pkv_sample_tokens_constrained,
+    DESIGN.md §4.11), in ONE launch: per row, x = f32(logit) + the sequence-bias sum, the penalties, then the bans (set to
+    -inf; bad words add -inf), then the draw. `params` (generate.SamplingState) also holds `rule_flags` (int32 [B]),
+    `bias` (float32 [B, >= V]) and `ban` (int32 [B, >= 2 * ceil(V / 32)]). A row with no rule flag reads none of them and
+    gets `sample_tokens_penalized`' token."""
+    fn = "sample_tokens_constrained"
+    d = _sample_desc(fn, logits, params, out, col, advance)
+    p = _penalty_struct(fn, logits, params)
+    B, V = logits.shape
+    _check_rule_tensor(fn, "params.rule_flags", params.rule_flags, torch.int32, B)
+    _check_rule_tensor(fn, "params.bias", params.bias, torch.float32, B, V)
+    _check_rule_tensor(fn, "params.ban", params.ban, torch.int32, B, 2 * ((V + 31) // 32))
+    r = _lib.SampleRules()
+    r.struct_bytes = C.sizeof(_lib.SampleRules)
+    r.flags = params.rule_flags.data_ptr()
+    r.bias, r.bias_stride = params.bias.data_ptr(), params.bias.shape[1]
+    r.ban, r.ban_stride = params.ban.data_ptr(), params.ban.shape[1]
+    _lib.check(_lib.lib().pkv_sample_tokens_constrained(C.byref(d), C.byref(p), C.byref(r),
+                                                        torch.cuda.current_stream(logits.device).cuda_stream))
+
+
+def token_rules(params, vocab: int, append: Optional[torch.Tensor] = None, col: int = 0) -> None:
+    """One `pkv_token_rules` launch (include/pkv.h, DESIGN.md §4.11) over the per-row DEVICE state of
+    generate.SamplingState: with `append` (int64 [B, n]), first append append[:, col] to each row's history; then write
+    each row's sequence-bias sums (`params.bias`), ban bitmaps (`params.ban`) and stop flag (`params.stop`, bool [B, 1])
+    from its history (`history` int32 [B, cap], `history_len` / `prompt_len` int32 [B]) and rules (`rule_flags`, `ngram`,
+    `min_new` int32 [B]; `n_seq` int32 [B], `seq_off` / `seq_kind` int32 and `seq_bias` float32 [B, S], `seq_tokens` int32
+    [B, T]; `eos` int32 [E], `n_eos`). Nothing is read back: the launch replays in a CUDA graph."""
+    fn = "token_rules"
+    B = params.history.shape[0]
+    V = int(vocab)
+    for name, dt, cols in (("history", torch.int32, 1), ("history_len", torch.int32, None), ("prompt_len", torch.int32, None),
+                           ("rule_flags", torch.int32, None), ("ngram", torch.int32, None), ("min_new", torch.int32, None),
+                           ("n_seq", torch.int32, None), ("seq_off", torch.int32, 2), ("seq_kind", torch.int32, 2),
+                           ("seq_bias", torch.float32, 2), ("seq_tokens", torch.int32, 1), ("bias", torch.float32, V),
+                           ("ban", torch.int32, 2 * ((V + 31) // 32)), ("stop", torch.bool, None)):
+        _check_rule_tensor(fn, f"params.{name}", getattr(params, name), dt, B, cols)
+    if params.seq_off.shape != params.seq_kind.shape or params.seq_off.shape != params.seq_bias.shape:
+        raise ValueError(f"{fn}: params.seq_off, seq_kind and seq_bias must have one shape")
+    d = _lib.TokenRulesDesc()
+    d.struct_bytes = C.sizeof(_lib.TokenRulesDesc)
+    d.device = params.history.device.index if params.history.device.index is not None else torch.cuda.current_device()
+    d.batch, d.vocab = B, V
+    d.history, d.history_stride = params.history.data_ptr(), params.history.shape[1]
+    d.history_len, d.prompt_len = params.history_len.data_ptr(), params.prompt_len.data_ptr()
+    d.flags, d.ngram, d.min_new_tokens, d.n_seq = (params.rule_flags.data_ptr(), params.ngram.data_ptr(),
+                                                   params.min_new.data_ptr(), params.n_seq.data_ptr())
+    d.seq_off, d.seq_kind, d.seq_bias = params.seq_off.data_ptr(), params.seq_kind.data_ptr(), params.seq_bias.data_ptr()
+    d.seq_stride = params.seq_off.shape[1]
+    d.seq_tokens, d.tokens_stride = params.seq_tokens.data_ptr(), params.seq_tokens.shape[1]
+    d.eos, d.n_eos = params.eos.data_ptr(), int(params.n_eos)
+    if append is not None:
+        if append.dtype != torch.long or append.dim() != 2 or append.shape[0] != B or append.stride(1) != 1 or not append.is_cuda:
+            raise ValueError(f"{fn}: append must be an int64 CUDA [B={B}, n] tensor with contiguous rows")
+        if not 0 <= int(col) < append.shape[1]:
+            raise ValueError(f"{fn}: col={col} outside [0, {append.shape[1]}) of append")
+        d.append, d.append_stride, d.append_column = append.data_ptr(), append.stride(0) if B > 1 else append.shape[1], int(col)
+    d.bias, d.bias_stride = params.bias.data_ptr(), params.bias.shape[1]
+    d.ban, d.ban_stride = params.ban.data_ptr(), params.ban.shape[1]
+    d.stop = params.stop.data_ptr()
+    _lib.check(_lib.lib().pkv_token_rules(C.byref(d), torch.cuda.current_stream(params.history.device).cuda_stream))
+
+
 # ---- token log-probabilities (include/pkv.h: pkv_token_logprobs, DESIGN.md §4.8) ----
 def token_logprobs(logits: torch.Tensor, tokens: torch.Tensor, out_lp: torch.Tensor, out_ids: torch.Tensor,
                    out_top: torch.Tensor, col: int = 0, tokens_col: int = 0, cursor: Optional[torch.Tensor] = None) -> None:
