@@ -652,6 +652,82 @@ typedef struct pkv_logprobs_desc {
 } pkv_logprobs_desc;
 int pkv_token_logprobs(const pkv_logprobs_desc* d, void* stream);
 
+/* ---- beam search: HF's `_beam_search` (do_sample=False) on the device (DESIGN.md §4.12) ----
+ * The rules, restated in oracle/beam.py. P prompts of k = num_beams beams each (2 <= k <= 16), beam b = p*k + r. At
+ * iteration t (t tokens generated before it, so each beam's cache holds t generated rows; t = 0 reads the prefill's
+ * logits), with n_eos <= 4 EOS ids and K = max(2, 1 + n_eos) * k <= 80:
+ *  1. pkv_beam_candidates, per beam row: m = max f32(l_v), log Z = logf(sum expf(f32(l_v) - m)) with Z summed exactly in
+ *     64-bit fixed point (pkv_token_logprobs' rule), and the row's top K tokens (logit descending, index ascending) with
+ *     lp_v = (f32(l_v) - m) - log Z. A row with a NaN or +-inf logit has no candidates (lp -inf, id -1).
+ *  2. pkv_beam_step, per prompt (one CTA), every value fp32:
+ *     c. score(r, v) = running[r] + lp_v; the top K of the k rows' entries by (score descending, flat index r*V + v
+ *        ascending) are the candidates c = 0 .. K-1 (the global top K lies inside the union of each row's top K); entries
+ *        of a non-finite row (id -1) come after every token of their row, in row order, and stand for token 0;
+ *     d. hit_c: token v_c is an EOS id, or t + 1 = max_steps (the maximum length);
+ *     e. running: the top k of score_c + (hit_c ? -1e9 : -0), (value descending, c ascending); beam slot a takes the
+ *        a-th: its token, its parent slot r_c and that running score;
+ *     f. pool: x_c = score_c * scale[t][0], then + -1e9 when every pool entry is finished and early_stopping is True, + -1e9
+ *        when the early-stop heuristic already failed, + -1e9 unless hit_c and c < k; the new pool is the top k of the old
+ *        k entries followed by the K x_c (value descending, index ascending); a new entry is finished when hit_c and c < k;
+ *     g. heuristic' = heuristic && any_j (running[0] * scale[t][1] > (finished_j ? min pool score : -1e9));
+ *        done = !heuristic' || (every pool entry finished && early_stopping is True) || t + 1 = max_steps.
+ *     scale[t] = (f32(1 / (t + 1)^length_penalty), f32(1 / L^length_penalty)), the reciprocals taken in double, with L =
+ *     max_steps when early_stopping is "never" and length_penalty > 0, else t + 1: torch's CUDA division of an fp32
+ *     tensor by a Python float d multiplies by f32(1 / d). A done prompt is frozen: its state is not written; its beams take token 0 and keep their rows.
+ *  3. pkv_cache_reorder moves each beam's cache to its parent's: slot a copies the generated rows [diverge[a], t) of slot
+ *     parent[a] (nothing when parent[a] = a), where diverge[a] comes from the common-prefix matrix cp (k x k per prompt,
+ *     generated rows two slots share): diverge[a] = parent[a] == a ? t : cp[a][parent[a]], cp'[a][b] = (pa == pb) ? t :
+ *     cp[pa][pb]. */
+#define PKV_MAX_BEAMS 16
+#define PKV_MAX_BEAM_CANDIDATES 80
+/* Candidates of `rows` rows of logits (bf16 / fp16, logits_stride elements apart), top_k = K <= 80: m [rows], log_z [rows],
+ * cand_lp [rows, K] (fp32) and cand_id [rows, K] (int32), all DEVICE and contiguous. One CTA per row, fixed launch
+ * arguments: it replays in a CUDA graph. PKV_ERR_INVALID_ARG: rows outside [1, 2^20], vocab outside [1, 2^24], stride <
+ * vocab, top_k outside [1, 80], null or misaligned pointers (2 bytes for the logits, 4 for the outputs). */
+int pkv_beam_candidates(int32_t dtype, int32_t device, int32_t rows, int64_t vocab, const void* logits, int64_t logits_stride,
+                        int32_t top_k, float* m, float* log_z, float* cand_lp, int32_t* cand_id, void* stream);
+/* One beam step of every prompt (rule 2 above). Every pointer is DEVICE memory; the iteration t = *step + step_offset is
+ * read on the device, so the launch replays in a CUDA graph. cand_lp / cand_id: [P*k, K] from pkv_beam_candidates, or
+ * with cand_rows_per_prompt = 1 one row per prompt, read for each of its k beams (iteration 0: the prefill's row).
+ * running [P*k] fp32 (initially 0, -1e9, ..., -1e9 per prompt); the pool [P*k]: score (initially -1e9), its (step,
+ * parent, token) handle (int32) and finished flag (uint8, initially 0); heuristic [P] (uint8, initially 1) and done [P]
+ * (initially 0); backpointers bp_token / bp_parent [P*k, max_steps] (int32: iteration t writes column t); cp [P, k, k]
+ * (int32, initially 0); outputs next_token [P*k] (int64), parent and diverge [P*k] (int32). */
+typedef struct pkv_beam_step_desc {
+    uint32_t struct_bytes;        /* = sizeof(pkv_beam_step_desc) */
+    int32_t device;
+    int32_t num_prompts, num_beams, top_k, cand_rows_per_prompt;
+    int32_t n_eos;                /* 0 .. 4 */
+    int32_t early_stopping;       /* 0: False, 1: True, 2: "never" */
+    int32_t max_steps;            /* max_new_tokens */
+    int32_t step_offset;
+    const int32_t* step;
+    const float* cand_lp; const int32_t* cand_id;
+    const int32_t* eos;           /* [n_eos] */
+    const float* scale;           /* [max_steps, 2] */
+    float* running;
+    float* pool_score; int32_t* pool_step; int32_t* pool_parent; int32_t* pool_token; uint8_t* pool_done;
+    uint8_t* heuristic; uint8_t* done;
+    int32_t* bp_token; int32_t* bp_parent;
+    int32_t* cp;
+    int64_t* next_token; int32_t* parent; int32_t* diverge;
+} pkv_beam_step_desc;
+int pkv_beam_step(const pkv_beam_step_desc* d, void* stream);
+/* The beam reorder of num_layers layers of a batched compacted cache of P*k sequences (rule 3 above), one launch per 32
+ * layers, the per-layer tables as kernel parameters; n = *step + step_offset generated rows. Layer l: planes[4l .. 4l+3]
+ * = K, V rows [P*k, num_heads, capacity[l], row_bytes] and, for E4M3 rows, their fp32 scales [P*k, num_heads,
+ * capacity[l]] (NULL for 16-bit rows); base[l] (DEVICE int32 [P*k*num_heads]): the row of generated slot 0 of each
+ * (sequence, head). Without a window generated row j is slot j. With window R > 0 slot j mod R holds the latest position j,
+ * and slot a copies the slots of positions [max(diverge, n - R), n); with heavy != 0 the slots are not position-indexed:
+ * a beam whose parent changed copies every slot [0, min(n, R)) and heavy_scores[l] / heavy_gen[l] ([P*k*num_heads, R])
+ * and victim[l] ([P*k*num_heads]). Prompt rows are never read or written. PKV_ERR_INVALID_ARG: num_beams outside [2,
+ * 16], row_bytes not a positive multiple of 16 up to 256, null or misaligned pointers. */
+int pkv_cache_reorder(int32_t num_prompts, int32_t num_beams, int32_t num_heads, int32_t row_bytes, int32_t device,
+                      int32_t num_layers, int32_t window, int32_t heavy, void* const* planes, const int64_t* capacity,
+                      const int32_t* const* base, float* const* heavy_scores, int32_t* const* heavy_gen,
+                      int32_t* const* victim, const int32_t* parent, const int32_t* diverge, const int32_t* step,
+                      int32_t step_offset, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

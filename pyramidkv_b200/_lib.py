@@ -25,6 +25,7 @@ EXPORTS = [
     "pkv_evict_pooled_kv_offset", "pkv_cache_install", "pkv_sample_tokens", "pkv_decode_attn_window",
     "pkv_decode_attn_heavy", "pkv_decode_heavy_workspace_bytes",
     "pkv_token_logprobs", "pkv_sample_tokens_penalized", "pkv_token_rules", "pkv_sample_tokens_constrained",
+    "pkv_beam_candidates", "pkv_beam_step", "pkv_cache_reorder",
 ]
 RULE_BIAS, RULE_BAN, RULE_BAD, RULE_STOP = 1, 2, 4, 8     # pkv_token_rules_desc.flags[b]
 SEQ_BIAS, SEQ_BAD, SEQ_STOP = 0, 1, 2                     # pkv_token_rules_desc.seq_kind
@@ -147,6 +148,22 @@ class LogprobsDesc(C.Structure):
 MAX_TOP_LOGPROBS = 20         # pkv_logprobs_desc.top_n
 
 
+class BeamStepDesc(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("device", C.c_int32), ("num_prompts", C.c_int32), ("num_beams", C.c_int32),
+        ("top_k", C.c_int32), ("cand_rows_per_prompt", C.c_int32), ("n_eos", C.c_int32), ("early_stopping", C.c_int32),
+        ("max_steps", C.c_int32), ("step_offset", C.c_int32), ("step", C.c_void_p), ("cand_lp", C.c_void_p),
+        ("cand_id", C.c_void_p), ("eos", C.c_void_p), ("scale", C.c_void_p), ("running", C.c_void_p),
+        ("pool_score", C.c_void_p), ("pool_step", C.c_void_p), ("pool_parent", C.c_void_p), ("pool_token", C.c_void_p),
+        ("pool_done", C.c_void_p), ("heuristic", C.c_void_p), ("done", C.c_void_p), ("bp_token", C.c_void_p),
+        ("bp_parent", C.c_void_p), ("cp", C.c_void_p), ("next_token", C.c_void_p), ("parent", C.c_void_p),
+        ("diverge", C.c_void_p),
+    ]
+
+
+MAX_BEAMS, MAX_BEAM_CANDIDATES = 16, 80   # PKV_MAX_BEAMS, PKV_MAX_BEAM_CANDIDATES
+
+
 class PkvError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libpkv error {code}: {msg}")
@@ -245,6 +262,12 @@ def lib() -> C.CDLL:
     L.pkv_sample_tokens_constrained.restype = i32
     L.pkv_token_logprobs.argtypes = [C.POINTER(LogprobsDesc), p]
     L.pkv_token_logprobs.restype = i32
+    L.pkv_beam_candidates.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int64, p, C.c_int64, C.c_int32] + [p] * 5
+    L.pkv_beam_candidates.restype = i32
+    L.pkv_beam_step.argtypes = [C.POINTER(BeamStepDesc), p]
+    L.pkv_beam_step.restype = i32
+    L.pkv_cache_reorder.argtypes = [C.c_int32] * 8 + [p] * 9 + [C.c_int32, p]
+    L.pkv_cache_reorder.restype = i32
     if L.pkv_version() != 3:
         raise RuntimeError(f"libpkv ABI version {L.pkv_version()} != 3; rebuild with `python -m pyramidkv_b200.build --force`")
     _lib = L

@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpkv.so")
-SOURCES = ["pkv_api.cu", "pkv_score.cu", "pkv_score_tc5.cu", "pkv_topk.cu", "pkv_topk_cluster.cu", "pkv_gather.cu", "pkv_decode.cu", "pkv_h2o.cu", "pkv_l2norm.cu", "pkv_rope.cu", "pkv_flatten.cu", "pkv_h2o_tc5.cu", "pkv_adakv.cu", "pkv_evict_fused.cu", "pkv_fp8.cu", "pkv_install.cu", "pkv_sample.cu", "pkv_logprobs.cu", "pkv_rules.cu"]
+SOURCES = ["pkv_api.cu", "pkv_score.cu", "pkv_score_tc5.cu", "pkv_topk.cu", "pkv_topk_cluster.cu", "pkv_gather.cu", "pkv_decode.cu", "pkv_h2o.cu", "pkv_l2norm.cu", "pkv_rope.cu", "pkv_flatten.cu", "pkv_h2o_tc5.cu", "pkv_adakv.cu", "pkv_evict_fused.cu", "pkv_fp8.cu", "pkv_install.cu", "pkv_sample.cu", "pkv_logprobs.cu", "pkv_rules.cu", "pkv_beam.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "--expt-relaxed-constexpr", "-Xptxas", "-v",

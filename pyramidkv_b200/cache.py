@@ -363,6 +363,14 @@ class PkvBatchCacheLayer(PkvCacheLayer):
             raise ValueError(f"admit: {n} rows exceed the capacity {self.capacity} (grow the batch first)")
         return (src.k_buf, src.v_buf, src._scales(), n, src.rows_dev, *dst), rows_host, src.seq_seen[0]
 
+    def _reorder_item(self):
+        """(the `cache_reorder` tuple of this layer): the rows and their scales, the row of each (sequence, head)'s
+        generated slot 0 (its prompt rows), the decode window and the heavy-hitter state."""
+        ks, vs = self._scales() or (None, None)
+        base = self.prompt_rows if self.window is not None else self.rows
+        heavy = None if self.heavy is None else (self.heavy_scores, self.heavy_gen, self.victim)
+        return self.k_buf, self.v_buf, ks, vs, base, self.window, heavy
+
     def _book(self, slot: int, rows_host, seen: int) -> None:
         self.rows_host[slot] = list(rows_host)
         self.seq_seen[slot] = int(seen)
@@ -616,6 +624,20 @@ def admit_cache(batch, slot: int, src, step: torch.Tensor, backend=None) -> None
 def park_cache(batch, slot: int, step: torch.Tensor, backend=None) -> None:
     """`PkvBatchCacheLayer.park` for every layer of the batched cache `batch`, in one launch."""
     _install(batch.layers, slot, None, step, backend)
+
+
+def reorder_caches(batch, num_prompts: int, num_beams: int, parent: torch.Tensor, diverge: torch.Tensor, step: torch.Tensor,
+                   step_offset: int, backend=None) -> None:
+    """Beam search: sequence p * num_beams + a of the batched cache `batch` (`join_caches` of each prompt's cache
+    num_beams times) takes the generated rows of sequence p * num_beams + parent[..] from row diverge[..] on, in every
+    layer, in one launch per 32 layers (`pkv_cache_reorder`; n = *step + step_offset generated rows, read on the device)."""
+    if backend is None:
+        from .kv_cluster import _default_backend as backend
+    for i, l in enumerate(batch.layers):
+        if not isinstance(l, PkvBatchCacheLayer):
+            raise ValueError(f"layer {i}: beams are reordered in batched caches (join_caches), not in a {type(l).__name__}")
+    backend.cache_reorder([l._reorder_item() for l in batch.layers], num_prompts, num_beams, parent, diverge, step,
+                          step_offset)
 
 
 def layer_is_empty(past_key_values, layer_idx: int) -> bool:

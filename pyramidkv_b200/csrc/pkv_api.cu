@@ -1060,4 +1060,110 @@ int pkv_cache_append(const pkv_decode_desc* d, void* stream) {
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "append launch");
 }
 
+int pkv_beam_candidates(int32_t dtype, int32_t device, int32_t rows, int64_t vocab, const void* logits, int64_t logits_stride,
+                        int32_t top_k, float* m, float* log_z, float* cand_lp, int32_t* cand_id, void* stream) {
+    const char* fn = "pkv_beam_candidates";
+    if (dtype != PKV_BF16 && dtype != PKV_FP16) return fail(PKV_ERR_UNSUPPORTED_DTYPE, "%s: dtype %d: only bf16 (0) and fp16 (1) logits", fn, dtype);
+    if (rows < 1 || rows > (1 << 20)) return fail(PKV_ERR_INVALID_ARG, "%s: rows=%d outside [1, 2^20]", fn, rows);
+    if (vocab < 1 || vocab > (int64_t(1) << 24)) return fail(PKV_ERR_INVALID_ARG, "%s: vocab=%lld outside [1, 2^24]", fn, (long long)vocab);
+    if (logits_stride < vocab) return fail(PKV_ERR_INVALID_ARG, "%s: logits_stride=%lld < vocab", fn, (long long)logits_stride);
+    if (top_k < 1 || top_k > kMaxBeamCandidates) return fail(PKV_ERR_INVALID_ARG, "%s: top_k=%d outside [1, %d]", fn, top_k, kMaxBeamCandidates);
+    auto bad = [](const void* p, uintptr_t align) { return !p || (reinterpret_cast<uintptr_t>(p) & (align - 1)); };
+    if (bad(logits, 2) || bad(m, 4) || bad(log_z, 4) || bad(cand_lp, 4) || bad(cand_id, 4))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned pointer", fn);
+    const DevInfo* di = nullptr;
+    int rc = device_info(device, &di);
+    if (rc) return rc;
+    BeamCandArgs a;
+    a.dtype = dtype; a.rows = rows; a.V = int(vocab); a.K = top_k;
+    a.logits = static_cast<const uint16_t*>(logits); a.ld = logits_stride;
+    a.m = m; a.log_z = log_z; a.cand_lp = cand_lp; a.cand_id = cand_id;
+    DeviceGuard guard(device);
+    const cudaError_t e = launch_beam_candidates(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "beam candidates launch");
+}
+
+int pkv_beam_step(const pkv_beam_step_desc* d, void* stream) {
+    const char* fn = "pkv_beam_step";
+    if (!d) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
+    if (d->struct_bytes != sizeof(pkv_beam_step_desc))
+        return fail(PKV_ERR_INVALID_ARG, "pkv_beam_step_desc.struct_bytes=%u, library expects %zu (ABI mismatch)", d->struct_bytes, sizeof(pkv_beam_step_desc));
+    const int k = d->num_beams;
+    if (d->num_prompts < 1 || d->num_prompts > (1 << 16)) return fail(PKV_ERR_INVALID_ARG, "%s: num_prompts=%d outside [1, 65536]", fn, d->num_prompts);
+    if (k < 2 || k > kMaxBeams) return fail(PKV_ERR_INVALID_ARG, "%s: num_beams=%d outside [2, %d]", fn, k, kMaxBeams);
+    if (d->n_eos < 0 || d->n_eos > 4) return fail(PKV_ERR_INVALID_ARG, "%s: n_eos=%d outside [0, 4]", fn, d->n_eos);
+    const int n_eos = d->n_eos;
+    if (d->top_k != (n_eos + 1 > 2 ? n_eos + 1 : 2) * k) return fail(PKV_ERR_INVALID_ARG, "%s: top_k=%d is not max(2, 1 + n_eos) * num_beams", fn, d->top_k);
+    if (d->cand_rows_per_prompt != 1 && d->cand_rows_per_prompt != k) return fail(PKV_ERR_INVALID_ARG, "%s: cand_rows_per_prompt must be 1 or num_beams", fn);
+    if (d->early_stopping < 0 || d->early_stopping > 2) return fail(PKV_ERR_INVALID_ARG, "%s: early_stopping=%d outside [0, 2]", fn, d->early_stopping);
+    if (d->max_steps < 1) return fail(PKV_ERR_INVALID_ARG, "%s: max_steps=%d < 1", fn, d->max_steps);
+    auto bad = [](const void* p, uintptr_t align) { return !p || (reinterpret_cast<uintptr_t>(p) & (align - 1)); };
+    if (bad(d->step, 4) || bad(d->cand_lp, 4) || bad(d->cand_id, 4) || (n_eos && bad(d->eos, 4)) || bad(d->scale, 4) ||
+        bad(d->running, 4) || bad(d->pool_score, 4) || bad(d->pool_step, 4) || bad(d->pool_parent, 4) || bad(d->pool_token, 4) ||
+        bad(d->pool_done, 1) || bad(d->heuristic, 1) || bad(d->done, 1) || bad(d->bp_token, 4) || bad(d->bp_parent, 4) ||
+        bad(d->cp, 4) || bad(d->next_token, 8) || bad(d->parent, 4) || bad(d->diverge, 4))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned pointer", fn);
+    const DevInfo* di = nullptr;
+    int rc = device_info(d->device, &di);
+    if (rc) return rc;
+    BeamStepArgs a;
+    a.P = d->num_prompts; a.k = k; a.K = d->top_k; a.rows_per_prompt = d->cand_rows_per_prompt; a.n_eos = n_eos;
+    a.early_stopping = d->early_stopping; a.max_steps = d->max_steps; a.step_offset = d->step_offset; a.step = d->step;
+    a.cand_lp = d->cand_lp; a.cand_id = d->cand_id; a.eos = d->eos; a.scale = d->scale; a.running = d->running;
+    a.pool_score = d->pool_score; a.pool_step = d->pool_step; a.pool_parent = d->pool_parent; a.pool_token = d->pool_token;
+    a.pool_done = d->pool_done; a.heur = d->heuristic; a.done = d->done; a.bp_token = d->bp_token; a.bp_parent = d->bp_parent;
+    a.cp = d->cp; a.next_token = d->next_token; a.parent = d->parent; a.diverge = d->diverge;
+    DeviceGuard guard(d->device);
+    const cudaError_t e = launch_beam_step(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "beam step launch");
+}
+
+int pkv_cache_reorder(int32_t num_prompts, int32_t num_beams, int32_t num_heads, int32_t row_bytes, int32_t device,
+                      int32_t num_layers, int32_t window, int32_t heavy, void* const* planes, const int64_t* capacity,
+                      const int32_t* const* base, float* const* heavy_scores, int32_t* const* heavy_gen,
+                      int32_t* const* victim, const int32_t* parent, const int32_t* diverge, const int32_t* step,
+                      int32_t step_offset, void* stream) {
+    const char* fn = "pkv_cache_reorder";
+    if (num_beams < 2 || num_beams > kMaxBeams) return fail(PKV_ERR_INVALID_ARG, "%s: num_beams=%d outside [2, %d]", fn, num_beams, kMaxBeams);
+    if (num_prompts < 1 || num_heads < 1 || num_heads > 4096 || num_layers < 1 || int64_t(num_prompts) * num_heads > (1 << 24))
+        return fail(PKV_ERR_INVALID_ARG, "%s: need num_prompts >= 1, 1 <= num_heads <= 4096, num_layers >= 1", fn);
+    if (row_bytes < 16 || row_bytes > 256 || row_bytes % 16) return fail(PKV_ERR_INVALID_ARG, "%s: row_bytes=%d: a multiple of 16 in [16, 256]", fn, row_bytes);
+    if (window < 0 || (heavy && window == 0)) return fail(PKV_ERR_INVALID_ARG, "%s: window=%d, heavy=%d", fn, window, heavy);
+    auto bad = [](const void* p, uintptr_t align) { return !p || (reinterpret_cast<uintptr_t>(p) & (align - 1)); };
+    if (!planes || !capacity || !base || bad(parent, 4) || bad(diverge, 4) || bad(step, 4))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned table", fn);
+    const bool scaled = planes[2] != nullptr;
+    for (int l = 0; l < num_layers; ++l) {
+        if (bad(planes[4 * l], 16) || bad(planes[4 * l + 1], 16) || bad(base[l], 4) || capacity[l] < 1)
+            return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: null or misaligned rows or row table", fn, l);
+        if (scaled != (planes[4 * l + 2] != nullptr) || (scaled && (bad(planes[4 * l + 2], 4) || bad(planes[4 * l + 3], 4))))
+            return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: scales must be given for every layer or none", fn, l);
+        if (heavy && (!heavy_scores || !heavy_gen || !victim || bad(heavy_scores[l], 4) || bad(heavy_gen[l], 4) || bad(victim[l], 4)))
+            return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: null or misaligned heavy-hitter state", fn, l);
+    }
+    const DevInfo* di = nullptr;
+    int rc = device_info(device, &di);
+    if (rc) return rc;
+    DeviceGuard guard(device);
+    for (int l0 = 0; l0 < num_layers; l0 += kMaxLayerBatch) {
+        ReorderArgs a;
+        a.P = num_prompts; a.k = num_beams; a.H = num_heads; a.row_bytes = row_bytes; a.window = window; a.heavy = heavy != 0;
+        a.n_layers = std::min(kMaxLayerBatch, num_layers - l0); a.step_offset = step_offset;
+        a.parent = parent; a.diverge = diverge; a.step = step;
+        for (int i = 0; i < a.n_layers; ++i) {
+            const int l = l0 + i;
+            ReorderLayer& q = a.layer[i];
+            for (int j = 0; j < 4; ++j) q.plane[j] = planes[4 * l + j];
+            q.cap = capacity[l];
+            q.base = base[l];
+            q.heavy_scores = heavy ? heavy_scores[l] : nullptr;
+            q.heavy_gen = heavy ? heavy_gen[l] : nullptr;
+            q.victim = heavy ? victim[l] : nullptr;
+        }
+        const cudaError_t e = launch_cache_reorder(a, static_cast<cudaStream_t>(stream));
+        if (e != cudaSuccess) return fail_cuda(e, "cache reorder launch");
+    }
+    return PKV_OK;
+}
+
 }  // extern "C"

@@ -262,6 +262,51 @@ struct LogprobsArgs {
 };
 cudaError_t launch_logprobs(const LogprobsArgs& a, cudaStream_t st);
 
+// beam search (pkv_beam.cu, DESIGN.md §4.12)
+constexpr int kMaxBeams = 16;
+constexpr int kMaxBeamCandidates = 80;   // K = max(2, 1 + n_eos) * k with k <= 16 and n_eos <= 4
+struct BeamCandArgs {
+    int dtype, rows, V, K;
+    const uint16_t* logits;
+    int64_t ld;
+    float* m;                   // [rows]
+    float* log_z;               // [rows]
+    float* cand_lp;             // [rows][K]
+    int32_t* cand_id;           // [rows][K]
+};
+cudaError_t launch_beam_candidates(const BeamCandArgs& a, cudaStream_t st);
+struct BeamStepArgs {
+    int P, k, K, rows_per_prompt, n_eos, early_stopping, max_steps, step_offset;
+    const float* cand_lp; const int32_t* cand_id;
+    const int32_t* eos;
+    const float* scale;         // [max_steps][2]
+    const int32_t* step;
+    float* running;
+    float* pool_score; int32_t* pool_step; int32_t* pool_parent; int32_t* pool_token; uint8_t* pool_done;
+    uint8_t* heur; uint8_t* done;
+    int32_t* bp_token; int32_t* bp_parent;
+    int32_t* cp;
+    int64_t* next_token;
+    int32_t* parent; int32_t* diverge;
+};
+cudaError_t launch_beam_step(const BeamStepArgs& a, cudaStream_t st);
+struct ReorderLayer {
+    void* plane[4];             // K, V rows [B][H][cap][row_bytes]; K, V fp32 scales [B][H][cap] (FP8) or null
+    int64_t cap;
+    const int32_t* base;        // [B*H]: the row of generated slot 0
+    float* heavy_scores;        // heavy hitters: [B*H][window]
+    int32_t* heavy_gen;         // [B*H][window]
+    int32_t* victim;            // [B*H]
+};
+struct ReorderArgs {
+    int P, k, H, row_bytes, window, heavy, n_layers, step_offset;
+    const int32_t* parent; const int32_t* diverge;   // [P*k]
+    const int32_t* step;
+    ReorderLayer layer[kMaxLayerBatch];
+};
+size_t reorder_smem_bytes(int k, int row_bytes);
+cudaError_t launch_cache_reorder(const ReorderArgs& a, cudaStream_t st);
+
 // RoPE in place on Q and K (pkv_rope.cu)
 struct RopeArgs {
     int dtype, Hq, Hkv, D;

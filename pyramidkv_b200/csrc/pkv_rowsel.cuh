@@ -1,9 +1,10 @@
 // pkv_rowsel.cuh — block-wide selection over one row of 16-bit logits, one CTA of kThreads per row. Shared by the sampling
-// kernel (pkv_sample.cu) and the log-probability kernel (pkv_logprobs.cu):
+// kernel (pkv_sample.cu), the log-probability kernel (pkv_logprobs.cu) and the beam candidates (pkv_beam.cu):
 //   - the 16-bit order key (okey / key_bits) and per-lane replicated byte histograms walked from the top, which find the
 //     n-th largest logit in two passes over the row;
 //   - expf masses in 64-bit fixed point (2^-40 units), so that every sum is an integer sum, independent of the schedule;
-//   - block reductions (best (value, index), sum) and the index of the n-th element of a predicate in index order.
+//   - block reductions (best (value, index), sum) and the index of the n-th element of a predicate in index order;
+//   - row_top: m, log Z and the row's top N in three passes.
 #pragma once
 
 #include <cmath>
@@ -171,6 +172,114 @@ __device__ int nth_index(Shared& S, int V, long long n, Pred pred) {
         left -= total;
     }
     return S.cut;
+}
+
+template <int MaxN>
+struct Top {
+    uint32_t key[MaxN];
+    int idx[MaxN];
+    int n;
+};
+
+// The three passes over one row of V 16-bit logits lg (every thread of the block calls it): the maximum mx, log_z =
+// logf(Z) with Z = sum expf(x_i - mx) in 64-bit fixed point, and (n_top > 0, n_top <= min(MaxN, V)) the row's n_top
+// largest keys with their indices in top (in no order; ties at the n_top-th key go to the lowest indices). hist is
+// 256 * 32 words of shared memory. False (and log_z NaN, top empty) when the row holds a NaN or +-inf.
+//   1. the maximum, whether any logit is NaN or +-inf, and (n_top > 0) a count histogram of the high byte of the key;
+//   2. Z and (n_top > 0) the low-byte histogram inside the high-byte bin of the n_top-th largest key -> that key k_N,
+//      how many keys lie above it and how many equal it;
+//   3. (n_top > 0) every key above k_N and the lowest-index ties at k_N (when more tie than are needed, the index of the
+//      last one kept comes from one ballot scan in index order, which stops at the chunk that holds it).
+template <typename E, int MaxN>
+__device__ bool row_top(Shared& S, Top<MaxN>& top, uint32_t* hist, const uint16_t* lg, int V, int n_top, float& mx_out,
+                        float& log_z_out) {
+    const int tid = threadIdx.x, lane = tid & 31;
+    const bool vec = (reinterpret_cast<uintptr_t>(lg) & 7u) == 0;
+    if (n_top > 0)
+        for (int b = tid; b < 256 * 32; b += kThreads) hist[b] = 0;
+    if (tid == 0) top.n = 0;
+    __syncthreads();
+
+    // pass 1: the maximum, the non-finite flag, the high-byte histogram
+    float mx = -INFINITY;
+    int bad = 0;
+    for (int g = tid; 4 * g < V; g += kThreads) {
+        uint32_t bb[4];
+        load4(lg, g, V, vec, bb);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (4 * g + j < V) {
+                const float x = DT<E>::to_f32(uint16_t(bb[j]));
+                bad |= !isfinite(x);
+                mx = fmaxf(mx, x);
+                if (n_top > 0) atomicAdd(&hist[(okey(bb[j]) >> 8) * 32 + lane], 1u);
+            }
+        }
+    }
+    int mi = 0;
+    block_best<false>(S, mx, mi);
+    const bool finite = !__syncthreads_or(bad);
+    float log_z = NAN;
+    int hb = 0;
+    if (finite) {
+        if (n_top > 0) {
+            reduce_hist(hist, S.cnt);
+            __syncthreads();
+            walk_top(S, S.cnt, (unsigned long long)n_top);
+            __syncthreads();
+            hb = S.bin;
+        }
+        // pass 2: Z; the low-byte histogram inside bin hb
+        unsigned long long z = 0;
+        for (int g = tid; 4 * g < V; g += kThreads) {
+            uint32_t bb[4];
+            load4(lg, g, V, vec, bb);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                if (4 * g + j < V) {
+                    z += fixed_mass(DT<E>::to_f32(uint16_t(bb[j])), mx);
+                    if (n_top > 0) {
+                        const uint32_t k = okey(bb[j]);
+                        if (int(k >> 8) == hb) atomicAdd(&hist[(k & 255u) * 32 + lane], 1u);
+                    }
+                }
+            }
+        }
+        z = block_sum(S, z);   // >= 2^40: the maximum contributes expf(0) = 1
+        log_z = logf(__ull2float_rn(z) * (1.0f / kFixScale));   // the scaling is exact: log Z in [0, log V]
+    }
+    if (finite && n_top > 0) {
+        const int rest = n_top - int(S.above);
+        __syncthreads();
+        reduce_hist(hist, S.cnt);
+        __syncthreads();
+        walk_top(S, S.cnt, (unsigned long long)rest);
+        __syncthreads();
+        const uint32_t kn = (uint32_t(hb) << 8) | uint32_t(S.bin);
+        const int need = rest - int(S.above);             // ties at k_N to keep, >= 1
+        const int ties = int(S.in_bin);
+        // pass 3: keys above k_N, and the ties at k_N up to the need-th one in index order
+        const int cut = need < ties ? nth_index(S, V, need, [&](int i) { return okey(__ldg(lg + i)) == kn; }) : V - 1;
+        for (int g = tid; 4 * g < V; g += kThreads) {
+            uint32_t bb[4];
+            load4(lg, g, V, vec, bb);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int i = 4 * g + j;
+                if (i < V) {
+                    const uint32_t k = okey(bb[j]);
+                    if (k > kn || (k == kn && i <= cut)) {
+                        const int s = atomicAdd(&top.n, 1);
+                        if (s < MaxN) { top.key[s] = k; top.idx[s] = i; }
+                    }
+                }
+            }
+        }
+        __syncthreads();
+    }
+    mx_out = mx;
+    log_z_out = log_z;
+    return finite;
 }
 
 }  // namespace rowsel

@@ -45,6 +45,10 @@ generated token and the N most likely tokens at each position, under the model's
 logits, whatever the sampling parameters), from one `pkv_token_logprobs` launch per step after the argmax or the draw
 (DESIGN.md §4.8). `score_continuations` forces given continuations through the same step and returns their
 log-probabilities over the compacted cache: the likelihood a cache form gives a fixed text.
+
+`beam_search_generate` is HF's `generate(num_beams=k, do_sample=False)`: each prompt is prefilled once, its cache joined k
+times, and every beam of every prompt decodes in lock-step in `StaticDecoder`, whose beam mode replaces the argmax by three
+launches (`pkv_beam_candidates`, `pkv_beam_step`, `pkv_cache_reorder`: DESIGN.md §4.12).
 """
 from __future__ import annotations
 
@@ -56,7 +60,7 @@ from typing import List, Optional
 
 import torch
 
-from .cache import PkvBatchCacheLayer, PkvCacheLayer, admit_cache, join_caches, park_cache
+from .cache import PkvBatchCacheLayer, PkvCacheLayer, admit_cache, join_caches, park_cache, reorder_caches
 
 
 @dataclass(frozen=True)
@@ -208,6 +212,18 @@ def _rule_tables(p: SamplingParams, eos: set):
 def _seed_i64(seed: int) -> int:
     seed = int(seed)
     return seed - 2 ** 64 if seed >= 2 ** 63 else seed      # the same 64 bits in an int64 tensor
+
+
+EARLY_STOPPING = {False: 0, True: 1, "never": 2}   # pkv_beam_step_desc.early_stopping
+MAX_BEAMS = 16
+
+
+def beam_divisors(max_steps: int, length_penalty: float, early_stopping) -> list:
+    """HF's length-penalty divisors per iteration t, as the Python floats it divides by: the pool's (t + 1)^lp and the
+    heuristic's L^lp (L = max_steps when early_stopping is "never" and lp > 0, else t + 1)."""
+    return [((t + 1) ** length_penalty,
+             (max_steps if early_stopping == "never" and length_penalty > 0.0 else t + 1) ** length_penalty)
+            for t in range(max_steps)]
 
 
 _PENALTY_FIELDS = ("repetition_penalty", "presence_penalty", "frequency_penalty", "min_p")
@@ -393,6 +409,78 @@ def _sampling_list(sampling, n: int, what: str):
     return out
 
 
+class BeamState:
+    """The device state of beam search over P prompts of k beams (include/pkv.h: pkv_beam_step; DESIGN.md §4.12): each
+    beam row's candidates (m, log Z, top K ids and log-probabilities, K = max(2, 1 + n_eos) * k), the running scores,
+    the finished pool (score, (step, parent, token) handle, finished flag), the early-stop heuristic and done flag of each
+    prompt, the backpointers [P*k, max_steps] the host rebuilds hypotheses from, the common-prefix matrix [P, k, k] and
+    the step's outputs: next token, parent slot and divergence row of each beam. Every tensor is written in place, so a
+    captured decode graph keeps its pointers. `scale` [max_steps, 2] holds f32(1 / d) of HF's length-penalty divisors d:
+    torch's CUDA division of an fp32 tensor by a Python float d multiplies by that; `divisors` the Python floats d."""
+
+    def __init__(self, P: int, k: int, max_steps: int, eos, length_penalty: float, early_stopping, device):
+        self.P, self.k, self.max_steps = int(P), int(k), int(max_steps)
+        self.eos = sorted(_eos_set(eos))
+        self.n_eos = len(self.eos)
+        self.K = max(2, 1 + self.n_eos) * self.k
+        self.early_stopping = EARLY_STOPPING[early_stopping]
+        self.divisors = beam_divisors(self.max_steps, float(length_penalty), early_stopping)
+        B, dev = self.P * self.k, device
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.scale = torch.tensor([[1.0 / d for d in row] for row in self.divisors], dtype=torch.float32, device=dev)
+        self.eos_dev = torch.tensor(self.eos or [0], **i32)
+        self.m = torch.zeros(B, dtype=torch.float32, device=dev)
+        self.log_z = torch.zeros(B, dtype=torch.float32, device=dev)
+        self.cand_lp = torch.zeros(B, self.K, dtype=torch.float32, device=dev)
+        self.cand_id = torch.zeros(B, self.K, **i32)
+        self.running = torch.full((self.P, self.k), -1e9, dtype=torch.float32, device=dev)
+        self.running[:, 0] = 0.0
+        self.running = self.running.reshape(B)
+        self.pool_score = torch.full((B,), -1e9, dtype=torch.float32, device=dev)
+        self.pool_step = torch.full((B,), -1, **i32)
+        self.pool_parent = torch.zeros(B, **i32)
+        self.pool_token = torch.zeros(B, **i32)
+        self.pool_done = torch.zeros(B, dtype=torch.uint8, device=dev)
+        self.heuristic = torch.ones(self.P, dtype=torch.uint8, device=dev)
+        self.done = torch.zeros(self.P, dtype=torch.uint8, device=dev)
+        self.bp_token = torch.zeros(B, self.max_steps, **i32)
+        self.bp_parent = torch.zeros(B, self.max_steps, **i32)
+        self.cp = torch.zeros(self.P, self.k, self.k, **i32)
+        self.next_token = torch.zeros(B, dtype=torch.long, device=dev)
+        self.parent = torch.arange(B, **i32) % self.k
+        self.diverge = torch.zeros(B, **i32)
+
+    def state(self) -> list:
+        """The tensors a step reads and advances (restored after the warm-up step of a graph capture)."""
+        return [self.running, self.pool_score, self.pool_step, self.pool_parent, self.pool_token, self.pool_done,
+                self.heuristic, self.done, self.bp_token, self.bp_parent, self.cp]
+
+    def step(self, backend, logits, rows_per_prompt: int, step: torch.Tensor, step_offset: int) -> None:
+        """Candidates of `logits` (one row per beam, or with rows_per_prompt = 1 one per prompt) and one beam step at
+        iteration *step + step_offset: two launches."""
+        backend.beam_candidates(logits, self)
+        backend.beam_step(self, rows_per_prompt, step, step_offset)
+
+    def hypotheses(self, n: int) -> list:
+        """Per prompt, its best n pool entries (best first): (generated tokens, fp32 score)."""
+        tok, par = self.bp_token.cpu().numpy(), self.bp_parent.cpu().numpy()
+        score = self.pool_score.cpu()
+        handles = torch.stack([self.pool_step, self.pool_parent, self.pool_token]).cpu().T.tolist()
+        out = []
+        for p in range(self.P):
+            bk = p * self.k
+            hyps = []
+            for j in range(n):
+                t, r, v = handles[bk + j]
+                seq = [int(v)]
+                for s in range(t - 1, -1, -1):     # back through the slots' backpointers
+                    seq.append(int(tok[bk + r, s]))
+                    r = int(par[bk + r, s])
+                hyps.append((seq[::-1] if t >= 0 else [], score[bk + j].clone()))
+            out.append(hyps)
+        return out
+
+
 @dataclass
 class TokenLogprobs:
     """Log-probabilities of one sequence's tokens (host tensors, n tokens, N = the `logprobs` / `top_n` asked for), under
@@ -461,11 +549,15 @@ class StaticDecoder:
     penalties or min-p, `prompts` gives each sequence's prompt ids (the first token counts as generated).
     logprobs: None, or N: each step also writes the log-probability of its token and the top N into `self.logprobs`
     (`_LogprobBuffers`, column = the step). forced: None, or int64 [B, max_steps]: step n takes forced[:, n] as its token
-    instead of the argmax (teacher forcing; it is then the next step's input, and with `logprobs` the token scored)."""
+    instead of the argmax (teacher forcing; it is then the next step's input, and with `logprobs` the token scored). beam: None, or the
+    `BeamState` of a cache joined num_beams times per prompt: each step's beam step (`pkv_beam_candidates`,
+    `pkv_beam_step`) picks every beam's next token and parent in place of the argmax, and `pkv_cache_reorder` moves each
+    beam's generated rows to its parent's (DESIGN.md §4.12)."""
 
     def __init__(self, model, cache, first_token: torch.Tensor, max_steps: int, use_graph: Optional[bool] = None,
                  eos_token_id=None, pad_token_id: int = 0, sampling: Optional[List[SamplingParams]] = None,
-                 logprobs: Optional[int] = None, forced: Optional[torch.Tensor] = None, prompts=None):
+                 logprobs: Optional[int] = None, forced: Optional[torch.Tensor] = None, prompts=None,
+                 beam: Optional["BeamState"] = None):
         layers = [l for l in cache.layers if isinstance(l, PkvCacheLayer)]
         if len(layers) != model.config.num_hidden_layers:
             raise RuntimeError("StaticDecoder needs a cache prefilled by the patched forward on every layer "
@@ -480,6 +572,9 @@ class StaticDecoder:
             if tuple(forced.shape) != (self.ids.shape[0], self.max_steps):
                 raise ValueError(f"StaticDecoder: forced must be [B={self.ids.shape[0]}, {self.max_steps}], got {tuple(forced.shape)}")
             self.forced = forced.to(device=self.ids.device, dtype=torch.long).contiguous()
+        self.beam = beam
+        if beam is not None and (sampling is not None or forced is not None or logprobs is not None or eos_token_id is not None):
+            raise ValueError("StaticDecoder: beam search excludes sampling, forced tokens, logprobs and eos_token_id")
         self.done = None if self.eos is None else (self.ids == self.eos[None, :]).any(dim=1, keepdim=True)   # [B, 1]
         if self.constrained:
             # a stop sequence completed by the first token; from then on each step ORs in its stop flags
@@ -530,6 +625,7 @@ class StaticDecoder:
                 self.sampling.rules(self.backend)                         # the first step's rule terms and stop flags
         self.constrained = self.sampling is not None and self.sampling.constrained
         self.forced = None
+        self.beam = None
         self.logprobs = None if logprobs is None else _LogprobBuffers(bsz, self.max_steps, int(logprobs), dev)
         cache._pkv_static = self.state
 
@@ -545,7 +641,13 @@ class StaticDecoder:
                       past_key_values=self.cache, use_cache=True)
         h = m.norm(h)
         logits = self.model.lm_head(h[:, -1, :])
-        if self.forced is not None:
+        if self.beam is not None:
+            # this step's row is iteration step + 1 of the beam search (iteration 0 read the prefill's logits)
+            self.beam.step(self.backend, logits, self.beam.k, self.state.step, 1)
+            reorder_caches(self.cache, self.beam.P, self.beam.k, self.beam.parent, self.beam.diverge, self.state.step, 1,
+                           self.backend)
+            tok = self.beam.next_token.view(-1, 1)
+        elif self.forced is not None:
             tok = self.forced.index_select(1, self.cursor)                # [B, 1]
         elif self.sampling is not None:
             self.sampling.draw(self.backend, logits, self.sampled, 0)
@@ -587,11 +689,16 @@ class StaticDecoder:
         # the heavy-hitter state a step updates (knob pkv_decode_heavy): restored so that the captured step starts from it
         heavy = [t for l in self.layers if l.heavy is not None for t in (l.heavy_scores, l.heavy_gen, l.victim)]
         rules = self.sampling.rule_state() if self.sampling is not None else []
+        # beam search: the warm-up step of a capture runs at step 0, where the reorder only touches the row the captured
+        # step rewrites, so restoring the beam state restores everything
+        rules += self.beam.state() if self.beam is not None else []
         return [t for t in (self.ids, self.pos, self.cursor, self.state.step, self.tokens, self.done, idx, counts,
                             self.window_rows) if t is not None] + heavy + rules
 
     def _capture(self) -> None:
         # warm up on a side stream (lazy initialisation, cuBLAS workspaces), restore the counters, then capture
+        if self.beam is not None and self.taken:
+            raise RuntimeError("StaticDecoder: a beam search graph is captured before its first step")
         state = self._counters()
         snap = [t.clone() for t in state]
         s = torch.cuda.Stream(device=self.ids.device)
@@ -1069,3 +1176,68 @@ def score_continuations(model, prompts, continuations, top_n: int = 0, use_graph
             entries[b].append((lp[b, :k], lp_ids[b, :k], lp_top[b, :k]))
         dec.finish(kept)
     return [_join_entries(c, e) for c, e in zip(conts, entries)]
+
+
+@torch.no_grad()
+def beam_search_generate(model, prompts, max_new_tokens: int, num_beams: int, *, length_penalty: float = 1.0,
+                         early_stopping=False, num_return_sequences: int = 1, eos_token_id=None,
+                         use_graph: Optional[bool] = None, check_every: int = 16):
+    """HF's `generate(num_beams=num_beams, do_sample=False, length_penalty=..., early_stopping=...,
+    num_return_sequences=..., max_new_tokens=...)` over the compacted caches (DESIGN.md §4.12). `prompts`: one 1-D (or
+    [1, S]) id tensor, or a list of them of any lengths. Each prompt is prefilled once at batch 1 (its deferred layer batch
+    and FP8 conversion included); its prefill logits row gives the first step's candidates, read for each of its beams;
+    its cache is joined num_beams times and all beams of all prompts decode in lock-step in `StaticDecoder`, one graph
+    replay per step. A prompt is done when HF's loop would stop for it alone; its state is then frozen. The host reads the
+    done flags once per `check_every` steps.
+
+    Returns, per prompt, `num_return_sequences` hypotheses, best first: (1-D tensor of the prompt and its generated ids,
+    ending in the EOS when it ended on one; its fp32 score, HF's `sequences_scores`)."""
+    single = torch.is_tensor(prompts)
+    ids = [p.reshape(1, -1) for p in ([prompts] if single else list(prompts))]
+    if not ids:
+        raise ValueError("beam_search_generate: no prompts")
+    if isinstance(num_beams, bool) or int(num_beams) != num_beams or not 2 <= int(num_beams) <= MAX_BEAMS:
+        raise ValueError(f"beam_search_generate: num_beams must be an integer in [2, {MAX_BEAMS}], got {num_beams!r}")
+    k = int(num_beams)
+    if isinstance(max_new_tokens, bool) or int(max_new_tokens) != max_new_tokens or int(max_new_tokens) < 1:
+        raise ValueError(f"beam_search_generate: max_new_tokens must be an integer >= 1, got {max_new_tokens!r}")
+    T = int(max_new_tokens)
+    if not (early_stopping is True or early_stopping is False or early_stopping == "never"):
+        raise ValueError(f"beam_search_generate: early_stopping must be True, False or 'never', got {early_stopping!r}")
+    if isinstance(num_return_sequences, bool) or int(num_return_sequences) != num_return_sequences \
+            or not 1 <= int(num_return_sequences) <= k:
+        raise ValueError(f"beam_search_generate: num_return_sequences must be in [1, num_beams={k}], got {num_return_sequences!r}")
+    if isinstance(length_penalty, bool) or not math.isfinite(float(length_penalty)):
+        raise ValueError(f"beam_search_generate: length_penalty must be a finite number, got {length_penalty!r}")
+    eos = eos_token_id if isinstance(eos_token_id, (list, tuple)) else ([] if eos_token_id is None else [eos_token_id])
+    V = model.lm_head.weight.shape[0]
+    if len(eos) > 4 or any(isinstance(e, bool) or int(e) != e or not 0 <= int(e) < V for e in eos):
+        raise ValueError(f"beam_search_generate: eos_token_id must be an id in [0, {V}) or a list of at most 4, got {eos_token_id!r}")
+    if len(set(int(e) for e in eos)) != len(eos):
+        raise ValueError(f"beam_search_generate: eos_token_id repeats an id: {eos_token_id!r}")
+    rows, caches = [], []
+    for p in ids:
+        logits, cache = _prefill_logits(model, p)
+        if not all(isinstance(l, PkvCacheLayer) for l in cache.layers):
+            raise RuntimeError("beam_search_generate needs a cache prefilled by the patched forward on every layer "
+                               "(method 'fullkv' and stock caches go through model.generate)")
+        rows.append(logits)
+        caches.append(cache)
+    backend = _backend(model)
+    dev = rows[0].device
+    st = BeamState(len(ids), k, T, [int(e) for e in eos], float(length_penalty), early_stopping, dev)
+    st.step(backend, torch.cat(rows).contiguous(), 1, torch.zeros(1, dtype=torch.int32, device=dev), 0)   # iteration 0
+    del rows
+    if T > 1 and not bool(st.done.all()):
+        cache = join_caches([c for c in caches for _ in range(k)], reserve=T - 1)
+        del caches
+        dec = StaticDecoder(model, cache, st.next_token.clone(), T - 1, use_graph=use_graph, beam=st)
+        while dec.taken < T - 1:
+            dec.run(min(max(1, int(check_every)), T - 1 - dec.taken))
+            if bool(st.done.all()):                                  # one device-to-host read per chunk
+                break
+        dec.finish()
+    out = []
+    for p, hyps in zip(ids, st.hypotheses(int(num_return_sequences))):
+        out.append([(torch.cat([p[0].cpu(), torch.tensor(g, dtype=torch.long)]).to(p.device), score) for g, score in hyps])
+    return out[0] if single else out

@@ -132,6 +132,17 @@ class CudaBackend:
     def token_logprobs(self, logits, tokens, out_lp, out_ids, out_top, col=0, tokens_col=0, cursor=None):
         ops.token_logprobs(logits, tokens, out_lp, out_ids, out_top, col, tokens_col, cursor)
 
+    # -- beam search: candidates per beam row, one step per prompt, the cache reorder of every layer --
+    def beam_candidates(self, logits, st):
+        R = logits.shape[0]
+        ops.beam_candidates(logits, st.m[:R], st.log_z[:R], st.cand_lp[:R], st.cand_id[:R])
+
+    def beam_step(self, st, rows_per_prompt, step, step_offset):
+        ops.beam_step(st, rows_per_prompt, step, step_offset)
+
+    def cache_reorder(self, items, P, k, parent, diverge, step, step_offset):
+        ops.cache_reorder(items, P, k, parent, diverge, step, step_offset)
+
     # -- ragged per-head budgets (AdaKV / HeadKV): scores first, budgets from the host, then select + gather --
     def ragged_begin(self, q, k, v, window_size, kernel_size, pooling):
         """Stages 1-2 (window logits, softmax + pool) into a workspace that stays alive until ragged_finish."""

@@ -981,3 +981,87 @@ def token_logprobs(logits: torch.Tensor, tokens: torch.Tensor, out_lp: torch.Ten
     if N > 0:
         d.top_ids, d.top_logprobs, d.top_stride = out_ids.data_ptr(), out_top.data_ptr(), n * N
     _lib.check(_lib.lib().pkv_token_logprobs(C.byref(d), torch.cuda.current_stream(logits.device).cuda_stream))
+
+
+# ---- beam search (include/pkv.h: pkv_beam_candidates, pkv_beam_step, pkv_cache_reorder; DESIGN.md §4.12) ----
+def beam_candidates(logits: torch.Tensor, m: torch.Tensor, log_z: torch.Tensor, cand_lp: torch.Tensor,
+                    cand_id: torch.Tensor) -> None:
+    """Per row of `logits` [R, V] (bf16 / fp16, contiguous rows): m [R], log_z [R] (float32) and the row's top K =
+    cand_lp.shape[1] tokens (logit descending, index ascending) into cand_id (int32 [R, K]) with their log-probabilities
+    into cand_lp (float32 [R, K]). One launch; it replays in a CUDA graph."""
+    _require_cuda(logits, m, log_z, cand_lp, cand_id)
+    if logits.dim() != 2 or logits.stride(1) != 1:
+        raise ValueError(f"beam_candidates: logits must be [R, V] with contiguous rows, got {tuple(logits.shape)}")
+    R, V = logits.shape
+    K = cand_lp.shape[1] if cand_lp.dim() == 2 else -1
+    if (cand_lp.shape != (R, K) or cand_id.shape != (R, K) or cand_lp.dtype != torch.float32 or cand_id.dtype != torch.int32
+            or not cand_lp.is_contiguous() or not cand_id.is_contiguous()):
+        raise ValueError(f"beam_candidates: cand_lp / cand_id must be contiguous float32 / int32 [R={R}, K] tensors")
+    if m.shape != (R,) or log_z.shape != (R,) or m.dtype != torch.float32 or log_z.dtype != torch.float32:
+        raise ValueError(f"beam_candidates: m / log_z must be float32 [R={R}] tensors")
+    dev = logits.device.index if logits.device.index is not None else torch.cuda.current_device()
+    _lib.check(_lib.lib().pkv_beam_candidates(_dtype_code(logits), dev, R, V, logits.data_ptr(),
+                                              logits.stride(0) if R > 1 else V, K, m.data_ptr(), log_z.data_ptr(),
+                                              cand_lp.data_ptr(), cand_id.data_ptr(),
+                                              torch.cuda.current_stream(logits.device).cuda_stream))
+
+
+_BEAM_FIELDS = ("running", "pool_score", "pool_step", "pool_parent", "pool_token", "pool_done", "heuristic", "done",
+                "bp_token", "bp_parent", "cp", "next_token", "parent", "diverge")
+
+
+def beam_step(st, rows_per_prompt: int, step: torch.Tensor, step_offset: int) -> None:
+    """One `pkv_beam_step` launch over the state `st` (generate.BeamState): its candidates (`rows_per_prompt` rows per
+    prompt: k, or 1 for the prefill's row), iteration *step + step_offset read on the device."""
+    _require_cuda(st.cand_lp, step, *(getattr(st, f) for f in _BEAM_FIELDS))
+    if step.dtype != torch.int32 or step.numel() != 1:
+        raise ValueError("beam_step: step must be a one-element int32 tensor")
+    d = _lib.BeamStepDesc()
+    d.struct_bytes = C.sizeof(_lib.BeamStepDesc)
+    d.device = st.running.device.index if st.running.device.index is not None else torch.cuda.current_device()
+    d.num_prompts, d.num_beams, d.top_k, d.cand_rows_per_prompt = st.P, st.k, st.K, int(rows_per_prompt)
+    d.n_eos, d.early_stopping, d.max_steps, d.step_offset = st.n_eos, st.early_stopping, st.max_steps, int(step_offset)
+    d.step, d.cand_lp, d.cand_id = step.data_ptr(), st.cand_lp.data_ptr(), st.cand_id.data_ptr()
+    d.eos, d.scale = st.eos_dev.data_ptr(), st.scale.data_ptr()
+    for f in _BEAM_FIELDS:
+        setattr(d, f, getattr(st, f).data_ptr())
+    _lib.check(_lib.lib().pkv_beam_step(C.byref(d), torch.cuda.current_stream(st.running.device).cuda_stream))
+
+
+def cache_reorder(items, P: int, k: int, parent: torch.Tensor, diverge: torch.Tensor, step: torch.Tensor,
+                  step_offset: int) -> None:
+    """Every layer's beam reorder in one launch per 32 layers (`pkv_cache_reorder`). items: per layer (k_buf, v_buf,
+    k_scale, v_scale, base, window, heavy_state) as `cache.PkvBatchCacheLayer._reorder_item` gives them: rows [P*k, H,
+    cap, D] (16-bit, or E4M3 with fp32 scales [P*k, H, cap]), base int32 [P*k*H] the row of generated slot 0, window R
+    or None, heavy_state (scores, gen, victim) or None."""
+    if not items:
+        raise ValueError("cache_reorder: no layers")
+    k0 = items[0][0]
+    B, H, _, D = k0.shape
+    fp8 = k0.dtype == torch.float8_e4m3fn
+    if B != P * k:
+        raise ValueError(f"cache_reorder: {B} sequences, expected {P} prompts x {k} beams")
+    window, heavy = items[0][5], items[0][6] is not None
+    _require_cuda(parent, diverge, step)
+    if parent.dtype != torch.int32 or diverge.dtype != torch.int32 or parent.numel() != B or diverge.numel() != B:
+        raise ValueError(f"cache_reorder: parent / diverge must be int32 [{B}]")
+    n = len(items)
+    planes, caps, base, hs, hg, vic = (C.c_void_p * (4 * n))(), (C.c_int64 * n)(), (C.c_void_p * n)(), \
+        (C.c_void_p * n)(), (C.c_void_p * n)(), (C.c_void_p * n)()
+    for i, (kb, vb, ks, vs, rows, win, hstate) in enumerate(items):
+        if kb.shape[:2] != (B, H) or kb.shape[3] != D or vb.shape != kb.shape or kb.dtype != k0.dtype or not kb.is_contiguous() \
+                or not vb.is_contiguous() or win != window or (hstate is not None) != heavy:
+            raise ValueError(f"cache_reorder: layer {i}: every layer must hold the same form and shape")
+        if (ks is not None) != fp8 or rows.dtype != torch.int32 or rows.numel() != B * H:
+            raise ValueError(f"cache_reorder: layer {i}: scales go with E4M3 rows; base must be int32 [{B * H}]")
+        planes[4 * i], planes[4 * i + 1] = kb.data_ptr(), vb.data_ptr()
+        if fp8:
+            planes[4 * i + 2], planes[4 * i + 3] = ks.data_ptr(), vs.data_ptr()
+        caps[i], base[i] = kb.shape[2], rows.data_ptr()
+        if heavy:
+            hs[i], hg[i], vic[i] = (t.data_ptr() for t in hstate)
+    dev = k0.device.index if k0.device.index is not None else torch.cuda.current_device()
+    _lib.check(_lib.lib().pkv_cache_reorder(int(P), int(k), H, D * (1 if fp8 else 2), dev, n, int(window or 0), int(heavy),
+                                            planes, caps, base, hs if heavy else None, hg if heavy else None,
+                                            vic if heavy else None, parent.data_ptr(), diverge.data_ptr(), step.data_ptr(),
+                                            int(step_offset), torch.cuda.current_stream(k0.device).cuda_stream))
