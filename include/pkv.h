@@ -728,6 +728,88 @@ int pkv_cache_reorder(int32_t num_prompts, int32_t num_beams, int32_t num_heads,
                       int32_t* const* victim, const int32_t* parent, const int32_t* diverge, const int32_t* step,
                       int32_t step_offset, void* stream);
 
+/* ---- prompt-lookup speculative decoding, greedy (DESIGN.md §4.13; the rules restated in oracle/spec.py) ----
+ * HF's generate(prompt_lookup_num_tokens=K, max_matching_ngram_size=N) without logits processors, for num_seqs sequences
+ * at once, K in [1, 15], N in [1, 8], Q = K + 1. Per sequence, with history h = prompt + tokens emitted so far (length L)
+ * and remaining budget m (tokens it may still emit):
+ *  1. Draft (PromptLookupCandidateGenerator.get_candidates): for n = min(N, L - 1) down to 1, the lowest start i with
+ *     h[i, i + n) == h[L - n, L) and i + n < L; the draft is h[i + n, min(i + n + K, L)), cut before its first EOS id. No
+ *     n matches: no draft. No draft when m <= 1 or the sequence is done. Draft length d <= K.
+ *  2. Verify: one forward over the Q tokens [last emitted, draft.., padding] at positions L - 1 .. L - 1 + K gives the
+ *     argmaxes t_0 .. t_K (torch.argmax: the first index among ties).
+ *  3. Accept (_assisted_decoding, greedy): a = the number of leading j < d with draft[j] == t_j, then a = min(a, m - 1);
+ *     the sequence emits t_0 .. t_a, stopping after the first EOS id among them. It is done after an EOS or when m reaches
+ *     0; a done sequence emits nothing (pad_token_id) and advances nothing.
+ *  4. Cache: the verify step writes the Q new rows of every layer and cache head at n0 .. n0 + K (n0: the rows held);
+ *     acceptance advances that row count by the tokens emitted. Rejected rows stay in the buffers uncounted and are
+ *     overwritten by the next step. A cache reserves its rows + max_new_tokens + K: a sequence whose budget ran out
+ *     still takes part in the verify steps of the others, writing (uncounted) Q rows behind its last. */
+#define PKV_MAX_SPEC_QUERIES 16
+#define PKV_MAX_NGRAM 8
+/* The verify attention: the batched decode of pkv_decode_attn_batch with Q = num_queries new rows per sequence. `d` gives
+ * dtype, head counts, head_dim, device, length, the caches (cache_stride_h), q, k_new, v_new, out, the workspace and the
+ * softmax scale. Sequence s, token j, query head h reads q at q + (s*Q + j)*q_stride_t + h*q_stride_h (so HF's [b, q, H, D]
+ * projections are read in place), kv head g's new rows at k_new / v_new + (s*Q + j)*kv_stride_t + g*kv_stride_h, and
+ * writes out + (s*Q + j)*out_stride_t + h*out_stride_h. Per (sequence s, cache head c), n0 = d->length (+ *step_dev)
+ * (+ rows[s*H + c]) rows are held (H = num_q_heads, or num_kv_heads when gqa_shared): the launch stores the Q new rows at
+ * n0 .. n0 + Q - 1 (16-bit rows: byte copies; E4M3 rows: the quantisation rule of pkv_decode_attn_batch_fp8, scale
+ * included) and query j of every head of the cache attends rows [0, n0 + j + 1) in fp32 (online softmax; E4M3: the row's
+ * K scale multiplies the fp32 dot, its V scale the softmax weight), the new rows as stored. One CTA per (split, cache head,
+ * sequence) reads each cached row once for all its GH*Q query rows; the split count is pkv_decode_attn_batch's for the
+ * largest attended count n0 + Q. n0 < 0 or n0 + Q > max_length: nothing is read or written, the outputs are NaN. Graph-
+ * replayable: every count is read on the device. Workspace: pkv_decode_workspace_bytes with num_q_heads =
+ * num_seqs*num_q_heads*num_queries. PKV_ERR_INVALID_ARG: m NULL or its struct_bytes wrong, num_queries outside [1, 16],
+ * num_seqs outside [1, 65535], d->length < 0, max_length above the capacity, strides that misalign rows, null or
+ * misaligned pointers; gqa_shared with a group outside {2, 4, 8} is PKV_ERR_UNSUPPORTED. */
+typedef struct pkv_decode_multi {
+    uint32_t struct_bytes;
+    int32_t num_seqs;
+    int32_t num_queries;        /* Q in [1, 16] */
+    int32_t gqa_shared;         /* 0: a cache per query head; 1: one per KV head */
+    int64_t cache_stride_b;     /* elements (E4M3: bytes) between the caches of consecutive sequences */
+    const int32_t* rows;        /* optional DEVICE int32 [num_seqs*H]: rows held */
+    const int32_t* step_dev;    /* optional DEVICE int32 added to every count */
+    int64_t max_length;         /* rows the launch is sized for: cache_stride_h >= max_length*head_dim */
+    float* k_scale;             /* E4M3 rows: fp32 row scales [num_seqs, H, capacity]; NULL for 16-bit rows */
+    float* v_scale;
+    int64_t scale_stride_h, scale_stride_b;
+    int64_t q_stride_t, q_stride_h;      /* elements; multiples of 8 */
+    int64_t kv_stride_t, kv_stride_h;    /* k_new and v_new alike */
+    int64_t out_stride_t, out_stride_h;
+} pkv_decode_multi;
+int pkv_decode_attn_multi(const pkv_decode_desc* d, const pkv_decode_multi* m, void* stream);
+/* The device state of rules 1 and 3, all DEVICE memory, contiguous: hist int64 [num_seqs, hist_cap] (the history; its
+ * length hist_len int32 [num_seqs]), budget int32 [num_seqs] (m), done uint8 [num_seqs], out int64 [num_seqs, out_cap]
+ * (the tokens emitted by the steps; out_len int32 [num_seqs] each sequence's cursor), ids and pos int64 [num_seqs, Q] (the
+ * next verify step's input ids and positions), draft_len int32 [num_seqs], emitted int32 [num_seqs] (the tokens the last
+ * step emitted), tokens int64 [num_seqs, Q] (the verify argmaxes t), eos int64 [n_eos] (n_eos in [0, 4]). rows: a HOST
+ * table of num_layers DEVICE int32 [num_seqs*num_heads] row counts (pkv_spec_step only; may be NULL with num_layers 0). */
+typedef struct pkv_spec_desc {
+    uint32_t struct_bytes;
+    int32_t device;
+    int32_t num_seqs;
+    int32_t num_queries;        /* Q = K + 1 in [2, 16] */
+    int32_t max_ngram;          /* N in [1, 8] */
+    int32_t n_eos;
+    int64_t pad_token_id;       /* the padding of ids past the draft */
+    int64_t hist_cap, out_cap;
+    int64_t* hist; int32_t* hist_len; int32_t* budget; uint8_t* done;
+    int64_t* out; int32_t* out_len;
+    int64_t* ids; int64_t* pos; int32_t* draft_len; int32_t* emitted;
+    const int64_t* tokens; const int64_t* eos;
+    int32_t num_layers, num_heads;
+    int32_t* const* rows;
+} pkv_spec_desc;
+/* Rule 1 for every sequence (one CTA each, a single pass over its history): ids = [h[L - 1], draft.., pad_token_id..],
+ * pos[j] = L - 1 + j, draft_len = d. Runs once before the first verify step. */
+int pkv_prompt_lookup(const pkv_spec_desc* d, void* stream);
+/* Rule 3 for every sequence from `tokens` and the current ids / draft_len: appends the emitted tokens to hist and out at
+ * the sequence's cursors, advances hist_len, out_len, budget, done and every layer's row counts (by emitted), then rule 1
+ * for the next ids / pos / draft_len. One launch per 32 layers; integer logic, no host reads: graph-replayable.
+ * PKV_ERR_INVALID_ARG (both): a wrong struct_bytes, num_seqs outside [1, 65535], Q outside [2, 16], N outside [1, 8],
+ * n_eos outside [0, 4], caps below 1, null or misaligned pointers. */
+int pkv_spec_step(const pkv_spec_desc* d, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

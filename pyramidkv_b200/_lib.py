@@ -26,6 +26,7 @@ EXPORTS = [
     "pkv_decode_attn_heavy", "pkv_decode_heavy_workspace_bytes",
     "pkv_token_logprobs", "pkv_sample_tokens_penalized", "pkv_token_rules", "pkv_sample_tokens_constrained",
     "pkv_beam_candidates", "pkv_beam_step", "pkv_cache_reorder",
+    "pkv_decode_attn_multi", "pkv_prompt_lookup", "pkv_spec_step",
 ]
 RULE_BIAS, RULE_BAN, RULE_BAD, RULE_STOP = 1, 2, 4, 8     # pkv_token_rules_desc.flags[b]
 SEQ_BIAS, SEQ_BAD, SEQ_STOP = 0, 1, 2                     # pkv_token_rules_desc.seq_kind
@@ -74,6 +75,30 @@ class DecodeWindow(C.Structure):
         ("k_scale", C.c_void_p), ("v_scale", C.c_void_p), ("scale_stride_h", C.c_int64), ("scale_stride_b", C.c_int64),
         ("window", C.c_int64),
     ]
+
+
+class DecodeMulti(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("num_seqs", C.c_int32), ("num_queries", C.c_int32), ("gqa_shared", C.c_int32),
+        ("cache_stride_b", C.c_int64), ("rows", C.c_void_p), ("step_dev", C.c_void_p), ("max_length", C.c_int64),
+        ("k_scale", C.c_void_p), ("v_scale", C.c_void_p), ("scale_stride_h", C.c_int64), ("scale_stride_b", C.c_int64),
+        ("q_stride_t", C.c_int64), ("q_stride_h", C.c_int64), ("kv_stride_t", C.c_int64), ("kv_stride_h", C.c_int64),
+        ("out_stride_t", C.c_int64), ("out_stride_h", C.c_int64),
+    ]
+
+
+class SpecDesc(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("device", C.c_int32), ("num_seqs", C.c_int32), ("num_queries", C.c_int32),
+        ("max_ngram", C.c_int32), ("n_eos", C.c_int32), ("pad_token_id", C.c_int64), ("hist_cap", C.c_int64),
+        ("out_cap", C.c_int64), ("hist", C.c_void_p), ("hist_len", C.c_void_p), ("budget", C.c_void_p), ("done", C.c_void_p),
+        ("out", C.c_void_p), ("out_len", C.c_void_p), ("ids", C.c_void_p), ("pos", C.c_void_p), ("draft_len", C.c_void_p),
+        ("emitted", C.c_void_p), ("tokens", C.c_void_p), ("eos", C.c_void_p), ("num_layers", C.c_int32),
+        ("num_heads", C.c_int32), ("rows", C.c_void_p),
+    ]
+
+
+MAX_SPEC_QUERIES, MAX_NGRAM = 16, 8   # PKV_MAX_SPEC_QUERIES, PKV_MAX_NGRAM
 
 
 class DecodeHeavy(C.Structure):
@@ -268,6 +293,12 @@ def lib() -> C.CDLL:
     L.pkv_beam_step.restype = i32
     L.pkv_cache_reorder.argtypes = [C.c_int32] * 8 + [p] * 9 + [C.c_int32, p]
     L.pkv_cache_reorder.restype = i32
+    L.pkv_decode_attn_multi.argtypes = [C.POINTER(DecodeDesc), C.POINTER(DecodeMulti), p]
+    L.pkv_decode_attn_multi.restype = i32
+    for name in ("pkv_prompt_lookup", "pkv_spec_step"):
+        fn = getattr(L, name)
+        fn.argtypes = [C.POINTER(SpecDesc), p]
+        fn.restype = i32
     if L.pkv_version() != 3:
         raise RuntimeError(f"libpkv ABI version {L.pkv_version()} != 3; rebuild with `python -m pyramidkv_b200.build --force`")
     _lib = L

@@ -89,7 +89,15 @@ def make_forward(method: str, modeling, original_forward):
         if getattr(self.config, "pkv_fused_rope", False) and not torch.is_grad_enabled():
             # SURVEY.md §8 f2: one in-place launch (pkv_rope_inplace) instead of HF's ten elementwise launches and four
             # full-size temporaries; bit-identical results. Opt-in knob on the shared config, like the reference's knobs.
-            if q_len == 1 and bsz > 1:
+            static = getattr(past_key_values, "_pkv_static", None)
+            if q_len > 1 and getattr(static, "spec", False):
+                # the verify step of speculative decoding: one launch over the B*Q token rows (q [Hq, B*Q, D], cos / sin
+                # [B*Q, D]: per-sequence positions)
+                cluster.backend.rope_inplace(query_states.transpose(1, 2).view(bsz * q_len, -1, self.head_dim).transpose(0, 1),
+                                             key_states.transpose(1, 2).view(bsz * q_len, -1, self.head_dim).transpose(0, 1),
+                                             cos.expand(bsz, -1, -1).reshape(bsz * q_len, -1),
+                                             sin.expand(bsz, -1, -1).reshape(bsz * q_len, -1))
+            elif q_len == 1 and bsz > 1:
                 # a batched decode step: one launch with the batch axis as the token axis (q [Hq, B, D], cos / sin [B, D])
                 cs = (cos, sin) if cos.shape[0] == bsz else (cos.expand(bsz, -1, -1).contiguous(), sin.expand(bsz, -1, -1).contiguous())
                 cluster.backend.rope_inplace(query_states[:, :, 0, :].transpose(0, 1), key_states[:, :, 0, :].transpose(0, 1),
@@ -182,6 +190,11 @@ def make_forward(method: str, modeling, original_forward):
                 if static is None:
                     layer.advance(1)
                 attn_output = out[:, None]
+            elif static is not None and getattr(static, "spec", False):
+                # the verify step of speculative decoding (generate.SpeculativeDecoder): the Q new rows of every sequence
+                # stored and attended causally in one launch per layer, q / k / v read in their [b, q, H, D] layout
+                attn_output = layer.decode_multi(cluster.backend, query_states.transpose(1, 2), key_states.transpose(1, 2),
+                                                 value_states.transpose(1, 2), static, self.scaling)
             else:
                 # several new tokens after the prefill (not produced by generate()): generic append + library attention
                 keys, values = layer.update(key_states, value_states)

@@ -321,6 +321,18 @@ class PkvBatchCacheLayer(PkvCacheLayer):
         return fn(q, self.k_buf, self.v_buf, 1, k_new, v_new, rows=self.rows, **_devlen_args(self, static),
                   softmax_scale=softmax_scale)
 
+    def decode_multi(self, backend, q, k_new, v_new, static, softmax_scale: float = 0.0) -> torch.Tensor:
+        """The verify step of speculative decoding (generate.SpeculativeDecoder): q [B, Q, Hq, D] and k_new / v_new
+        [B, Q, Hkv, D] (HF's projections as they are laid out). Each (sequence, head) stores its Q new rows at rows[b, h] ..
+        rows[b, h] + Q - 1 and query j attends the first rows[b, h] + j + 1 (`pkv_decode_attn_multi`); the row counts are
+        advanced by the acceptance step, not here. Returns the attention output [B, Q, Hq, D]."""
+        if self.window is not None:
+            raise NotImplementedError("speculative decoding under the decode window (pkv_decode_window / pkv_decode_heavy) is "
+                                      "not built: rejected rows would already have replaced ring rows the cache keeps")
+        return backend.decode_attn_multi(q, self.k_buf, self.v_buf, k_new, v_new, rows=self.rows, max_length=self.capacity,
+                                         scales=self._scales(), gqa=self.group > 1, workspace=static.workspace,
+                                         softmax_scale=softmax_scale)
+
     # -- continuous batching (generate.ContinuousDecoder): one slot rewritten in place while a decode graph holds the buffers --
     def admit(self, slot: int, src_layer, step: torch.Tensor, backend=None) -> None:
         """Copy the single-prompt layer `src_layer` (the form this batch holds: `PkvCacheLayer` / `PkvRaggedCacheLayer`, or,

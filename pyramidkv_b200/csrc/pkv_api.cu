@@ -1166,4 +1166,114 @@ int pkv_cache_reorder(int32_t num_prompts, int32_t num_beams, int32_t num_heads,
     return PKV_OK;
 }
 
+int pkv_decode_attn_multi(const pkv_decode_desc* d, const pkv_decode_multi* m, void* stream) {
+    const char* fn = "pkv_decode_attn_multi";
+    if (!d || !m) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
+    if (d->struct_bytes != sizeof(pkv_decode_desc) || m->struct_bytes != sizeof(pkv_decode_multi))
+        return fail(PKV_ERR_INVALID_ARG, "%s: struct_bytes mismatch (ABI)", fn);
+    if (d->dtype != PKV_BF16 && d->dtype != PKV_FP16) return fail(PKV_ERR_UNSUPPORTED_DTYPE, "%s: dtype %d", fn, d->dtype);
+    if (d->num_q_heads <= 0 || d->num_kv_heads <= 0 || d->num_q_heads % d->num_kv_heads) return fail(PKV_ERR_INVALID_ARG, "%s: bad head counts", fn);
+    if (d->head_dim != 64 && d->head_dim != 128) return fail(PKV_ERR_UNSUPPORTED, "%s: head_dim=%d: only 64 and 128 are built", fn, d->head_dim);
+    const int Q = m->num_queries, G = d->num_q_heads / d->num_kv_heads;
+    if (Q < 1 || Q > PKV_MAX_SPEC_QUERIES) return fail(PKV_ERR_INVALID_ARG, "%s: num_queries=%d outside [1, %d]", fn, Q, PKV_MAX_SPEC_QUERIES);
+    if (m->num_seqs < 1 || m->num_seqs > 65535) return fail(PKV_ERR_INVALID_ARG, "%s: num_seqs=%d outside [1, 65535]", fn, m->num_seqs);
+    if (m->gqa_shared && G != 2 && G != 4 && G != 8)
+        return fail(PKV_ERR_UNSUPPORTED, "%s: group size %d: the grouped form is built for 2, 4 and 8", fn, G);
+    const bool e4m3 = m->k_scale != nullptr;
+    if (e4m3 != (m->v_scale != nullptr)) return fail(PKV_ERR_INVALID_ARG, "%s: k_scale and v_scale go together", fn);
+    const int heads = m->gqa_shared ? d->num_kv_heads : d->num_q_heads;
+    const int64_t align = e4m3 ? 16 : 8;
+    if (d->length < 0 || m->max_length < Q || d->cache_stride_h < m->max_length * d->head_dim || d->cache_stride_h % align ||
+        (m->num_seqs > 1 && (m->cache_stride_b < heads * d->cache_stride_h || m->cache_stride_b % align)))
+        return fail(PKV_ERR_INVALID_ARG, "%s: length, max_length or cache strides out of range (cache capacity exceeded)", fn);
+    if (e4m3 && (m->scale_stride_h < m->max_length || (m->num_seqs > 1 && m->scale_stride_b < heads * m->scale_stride_h)))
+        return fail(PKV_ERR_INVALID_ARG, "%s: scale strides hold fewer than max_length rows", fn);
+    if (m->q_stride_t % 8 || m->q_stride_h % 8 || m->kv_stride_t % 8 || m->kv_stride_h % 8 || m->out_stride_t < 0 || m->out_stride_h < 0)
+        return fail(PKV_ERR_INVALID_ARG, "%s: token / head strides must be multiples of 8 elements", fn);
+    if (!d->q || !d->out || !d->k_new || !d->v_new || !d->k_cache || !d->v_cache || !aligned16(d->q) || !aligned16(d->k_new) ||
+        !aligned16(d->v_new) || !aligned16(d->k_cache) || !aligned16(d->v_cache) || (reinterpret_cast<uintptr_t>(d->out) & 1u) ||
+        (reinterpret_cast<uintptr_t>(m->rows) & 3u) || (reinterpret_cast<uintptr_t>(m->step_dev) & 3u) ||
+        (e4m3 && ((reinterpret_cast<uintptr_t>(m->k_scale) & 3u) || (reinterpret_cast<uintptr_t>(m->v_scale) & 3u))))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned pointer", fn);
+    const DevInfo* di = nullptr;
+    int rc = device_info(d->device, &di);
+    if (rc) return rc;
+    MultiArgs a;
+    a.dtype = d->dtype; a.Hq = d->num_q_heads; a.Hkv = d->num_kv_heads; a.G = G; a.D = d->head_dim; a.Q = Q;
+    a.num_seqs = m->num_seqs; a.heads_per_cache = m->gqa_shared ? G : 1; a.num_sms = di->sms;
+    a.nsplit = decode_num_splits(a.Hq, m->max_length, a.num_sms);
+    a.q = static_cast<const uint16_t*>(d->q); a.k_new = static_cast<const uint16_t*>(d->k_new);
+    a.v_new = static_cast<const uint16_t*>(d->v_new); a.out = static_cast<uint16_t*>(d->out);
+    a.q_st = m->q_stride_t; a.q_sh = m->q_stride_h; a.kv_st = m->kv_stride_t; a.kv_sh = m->kv_stride_h;
+    a.out_st = m->out_stride_t; a.out_sh = m->out_stride_h;
+    a.k_cache = d->k_cache; a.v_cache = d->v_cache; a.cache_sh = d->cache_stride_h;
+    a.cache_sb = m->num_seqs > 1 ? m->cache_stride_b : heads * d->cache_stride_h;
+    a.k_scale = m->k_scale; a.v_scale = m->v_scale; a.scale_sh = m->scale_stride_h;
+    a.scale_sb = m->num_seqs > 1 ? m->scale_stride_b : heads * m->scale_stride_h;
+    a.T = d->length; a.max_rows = m->max_length; a.step_dev = m->step_dev; a.rows = m->rows;
+    a.scale = d->softmax_scale != 0.f ? d->softmax_scale : 1.0f / sqrtf(float(d->head_dim));
+    a.ws = static_cast<float*>(d->workspace);
+    if (a.nsplit > 1) {
+        const uint64_t need = uint64_t(a.num_seqs) * a.Hq * Q * a.nsplit * (2 + a.D) * sizeof(float);
+        if (!d->workspace || d->workspace_bytes < need || (reinterpret_cast<uintptr_t>(d->workspace) & 15u))
+            return fail(PKV_ERR_WORKSPACE, "%s: workspace of %llu bytes required", fn, (unsigned long long)need);
+    }
+    DeviceGuard guard(d->device);
+    const cudaError_t e = launch_decode_multi(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, fn);
+}
+
+static int spec_args(const char* fn, const pkv_spec_desc* d, bool step, SpecArgs* a) {
+    if (!d) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
+    if (d->struct_bytes != sizeof(pkv_spec_desc))
+        return fail(PKV_ERR_INVALID_ARG, "pkv_spec_desc.struct_bytes=%u, library expects %zu (ABI mismatch)", d->struct_bytes, sizeof(pkv_spec_desc));
+    if (d->num_seqs < 1 || d->num_seqs > 65535) return fail(PKV_ERR_INVALID_ARG, "%s: num_seqs=%d outside [1, 65535]", fn, d->num_seqs);
+    if (d->num_queries < 2 || d->num_queries > PKV_MAX_SPEC_QUERIES) return fail(PKV_ERR_INVALID_ARG, "%s: num_queries=%d outside [2, 16]", fn, d->num_queries);
+    if (d->max_ngram < 1 || d->max_ngram > PKV_MAX_NGRAM) return fail(PKV_ERR_INVALID_ARG, "%s: max_ngram=%d outside [1, 8]", fn, d->max_ngram);
+    if (d->n_eos < 0 || d->n_eos > 4) return fail(PKV_ERR_INVALID_ARG, "%s: n_eos=%d outside [0, 4]", fn, d->n_eos);
+    if (d->hist_cap < 1 || d->hist_cap > INT32_MAX || d->out_cap < 1) return fail(PKV_ERR_INVALID_ARG, "%s: hist_cap / out_cap out of range", fn);
+    auto bad = [](const void* p, uintptr_t align) { return !p || (reinterpret_cast<uintptr_t>(p) & (align - 1)); };
+    if (bad(d->hist, 8) || bad(d->hist_len, 4) || bad(d->budget, 4) || bad(d->done, 1) || bad(d->out, 8) || bad(d->out_len, 4) ||
+        bad(d->ids, 8) || bad(d->pos, 8) || bad(d->draft_len, 4) || bad(d->emitted, 4) || (d->n_eos && bad(d->eos, 8)) ||
+        (step && bad(d->tokens, 8)))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned pointer", fn);
+    if (step && (d->num_layers < 0 || (d->num_layers > 0 && (!d->rows || d->num_heads < 1))))
+        return fail(PKV_ERR_INVALID_ARG, "%s: num_layers / num_heads / rows table", fn);
+    for (int l = 0; step && l < d->num_layers; ++l)
+        if (bad(d->rows[l], 4)) return fail(PKV_ERR_INVALID_ARG, "%s: layer %d: null or misaligned row counts", fn, l);
+    const DevInfo* di = nullptr;
+    int rc = device_info(d->device, &di);
+    if (rc) return rc;
+    a->num_seqs = d->num_seqs; a->Q = d->num_queries; a->N = d->max_ngram; a->n_eos = d->n_eos; a->n_layers = 0; a->H = d->num_heads;
+    a->hist_cap = d->hist_cap; a->out_cap = d->out_cap; a->pad = d->pad_token_id;
+    a->hist = d->hist; a->hist_len = d->hist_len; a->budget = d->budget; a->done = d->done; a->out = d->out; a->out_len = d->out_len;
+    a->ids = d->ids; a->pos = d->pos; a->draft_len = d->draft_len; a->emitted = d->emitted; a->tokens = d->tokens; a->eos = d->eos;
+    return PKV_OK;
+}
+
+int pkv_prompt_lookup(const pkv_spec_desc* d, void* stream) {
+    SpecArgs a;
+    int rc = spec_args("pkv_prompt_lookup", d, false, &a);
+    if (rc) return rc;
+    DeviceGuard guard(d->device);
+    const cudaError_t e = launch_prompt_lookup(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "prompt lookup launch");
+}
+
+int pkv_spec_step(const pkv_spec_desc* d, void* stream) {
+    SpecArgs a;
+    int rc = spec_args("pkv_spec_step", d, true, &a);
+    if (rc) return rc;
+    DeviceGuard guard(d->device);
+    int l0 = 0;
+    do {   // the step with the first 32 layers, then the row counts of the next 32 per launch
+        a.n_layers = std::min(kMaxLayerBatch, d->num_layers - l0);
+        for (int i = 0; i < a.n_layers; ++i) a.rows[i] = d->rows[l0 + i];
+        const cudaError_t e = launch_spec_step(a, l0 == 0, static_cast<cudaStream_t>(stream));
+        if (e != cudaSuccess) return fail_cuda(e, "spec step launch");
+        l0 += kMaxLayerBatch;
+    } while (l0 < d->num_layers);
+    return PKV_OK;
+}
+
 }  // extern "C"

@@ -154,6 +154,40 @@ int decode_num_splits(int Hq, int64_t T, int num_sms);
 cudaError_t launch_decode(const DecodeArgs& a, cudaStream_t st);
 cudaError_t launch_append(const DecodeArgs& a, cudaStream_t st);
 
+// ---- speculative decoding (pkv_spec.cu) ----
+// The verify attention: Q new rows per (sequence, cache head) stored at n0 .. n0 + Q - 1, n0 = T (+ *step_dev) (+ rows[..]);
+// query j attends rows [0, n0 + j + 1). n0 < 0 or n0 + Q > max_rows: NaN output, nothing written.
+struct MultiArgs {
+    int dtype, Hq, Hkv, G, D, Q, num_seqs, heads_per_cache, nsplit, num_sms;
+    const uint16_t *q, *k_new, *v_new;   // token s*Q + j, head h at + (s*Q + j)**_st + h*_sh elements
+    uint16_t* out;
+    int64_t q_st, q_sh, kv_st, kv_sh, out_st, out_sh;
+    void *k_cache, *v_cache;
+    int64_t cache_sh, cache_sb;
+    float *k_scale, *v_scale;            // E4M3 rows when set
+    int64_t scale_sh, scale_sb;
+    int64_t T, max_rows;
+    const int32_t* step_dev;
+    const int32_t* rows;
+    float scale;
+    float* ws;                           // [num_seqs*Hq*Q][nsplit][2 + D] when nsplit > 1
+};
+size_t decode_multi_smem_bytes(int heads_per_cache, int Q, int D);
+cudaError_t launch_decode_multi(const MultiArgs& a, cudaStream_t st);
+constexpr int kMaxNgram = 8;
+struct SpecArgs {
+    int num_seqs, Q, N, n_eos, n_layers, H;   // n_layers <= kMaxLayerBatch
+    int64_t hist_cap, out_cap, pad;
+    int64_t* hist; int32_t* hist_len; int32_t* budget; uint8_t* done;
+    int64_t* out; int32_t* out_len;
+    int64_t* ids; int64_t* pos; int32_t* draft_len; int32_t* emitted;
+    const int64_t* tokens; const int64_t* eos;
+    int32_t* rows[kMaxLayerBatch];
+};
+cudaError_t launch_prompt_lookup(const SpecArgs& a, cudaStream_t st);
+// first: the step kernel (rule 3, the rows of a.rows, rule 1); otherwise only the rows of a.rows, by emitted[b]
+cudaError_t launch_spec_step(const SpecArgs& a, bool first, cudaStream_t st);
+
 // ---- conversion of the compacted cache to FP8 (E4M3) rows (pkv_fp8.cu) ----
 struct QuantLayer {
     const uint16_t* src[2];   // K, V: 16-bit [num_seqs][H][src_cap][D]

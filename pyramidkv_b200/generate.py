@@ -535,6 +535,7 @@ class _StaticState:
     step: torch.Tensor        # int32 [1]: decode steps already taken in this static run (read by the decode kernel)
     workspace: torch.Tensor   # split-T partials, shared by all layers (launches are stream-ordered)
     heavy_scratch: Optional[torch.Tensor] = None   # knob pkv_decode_heavy: the per-step logits, shared by all layers
+    spec: bool = False        # the verify step of speculative decoding: q_len > 1 goes through `decode_multi`
 
 
 class StaticDecoder:
@@ -792,17 +793,28 @@ def _eos_set(eos_token_id) -> set:
 @torch.no_grad()
 def greedy_generate(model, input_ids: torch.Tensor, max_new_tokens: int, use_graph: Optional[bool] = None,
                     return_cache: bool = False, eos_token_id=None, check_every: int = 16,
-                    sampling: Optional[SamplingParams] = None, logprobs: Optional[int] = None):
+                    sampling: Optional[SamplingParams] = None, logprobs: Optional[int] = None,
+                    prompt_lookup_num_tokens: Optional[int] = None, max_matching_ngram_size: Optional[int] = None):
     """Prefill (+ eviction in every patched layer) then up to `max_new_tokens - 1` static decode steps. Greedy unless
     `sampling` (a SamplingParams) is given: every token is then drawn with it (DESIGN.md §4.6).
     Returns sequences [1, prompt + generated] like `generate(...).sequences` (and the cache on request).
     `eos_token_id` (int or list, as the reference runner passes it: run_longbench.py:270-272) ends the generation with the first
     such token (kept, like HF); the device never waits for the host, so the tokens are inspected every `check_every` steps
     and the surplus steps are dropped. With `logprobs` = N (0 to 20) the return value gains, as its last element, a list of
-    one `TokenLogprobs` for the generated tokens (DESIGN.md §4.8)."""
+    one `TokenLogprobs` for the generated tokens (DESIGN.md §4.8).
+    `prompt_lookup_num_tokens` = K (1 to 15) decodes by greedy prompt-lookup speculation (HF's argument of that name, with
+    `max_matching_ngram_size` N, 1 to 8, default 2): each step drafts up to K tokens by matching the last N-gram of the
+    prompt and the tokens so far, verifies them in one forward and keeps the accepted ones (`SpeculativeDecoder`, DESIGN.md
+    §4.13). The cache is joined (`cache.join_caches`) first; every cache form but the decode window runs. Greedy only."""
     if input_ids.dim() != 2 or input_ids.shape[0] != 1:
         raise NotImplementedError("batch size 1 (as in the reference: README.md:47); greedy_generate_batch decodes several prompts together")
     eos = _eos_set(eos_token_id)
+    spec = _check_spec(prompt_lookup_num_tokens, max_matching_ngram_size, sampling, logprobs, "greedy_generate")
+    if spec is not None:
+        first, gen, cache = _speculative(model, [input_ids], max_new_tokens, *spec, eos, 0, use_graph, check_every)
+        seq = torch.cat([input_ids, first.to(input_ids.device),
+                         torch.tensor([gen[0]], dtype=torch.long, device=input_ids.device).reshape(1, -1)], dim=1)
+        return (seq, cache) if return_cache else seq
     if sampling is not None and not isinstance(sampling, SamplingParams):
         raise ValueError("greedy_generate: sampling must be a SamplingParams")
     logprobs = _check_logprobs(logprobs, "greedy_generate")
@@ -846,7 +858,8 @@ def greedy_generate(model, input_ids: torch.Tensor, max_new_tokens: int, use_gra
 @torch.no_grad()
 def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None, pad_token_id: int = 0,
                           use_graph: Optional[bool] = None, check_every: int = 16, return_cache: bool = False, sampling=None,
-                          logprobs: Optional[int] = None):
+                          logprobs: Optional[int] = None, prompt_lookup_num_tokens: Optional[int] = None,
+                          max_matching_ngram_size: Optional[int] = None):
     """Greedy generation for several prompts of any lengths (1-D or [1, S] id tensors): each prompt is prefilled alone
     exactly as `greedy_generate` does, the compacted caches are joined, and up to `max_new_tokens - 1` steps decode all of
     them together (`StaticDecoder` over the joined cache). Each sequence stops at its first `eos_token_id` (kept, like HF);
@@ -854,11 +867,18 @@ def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None
     prompt + generated (and the joined cache on request, its per-sequence rows ending at each EOS). Greedy unless `sampling`
     (one SamplingParams for all prompts, or one per prompt) is given: each prompt's tokens are then drawn with its own.
     With `logprobs` = N (0 to 20) the return value gains, as its last element, one `TokenLogprobs` per prompt for its
-    generated tokens (DESIGN.md §4.8)."""
+    generated tokens (DESIGN.md §4.8). `prompt_lookup_num_tokens` / `max_matching_ngram_size`: greedy prompt-lookup
+    speculation as in `greedy_generate`, every prompt drafting from its own history."""
     ids = [p.reshape(1, -1) for p in prompts]
     if not ids:
         raise ValueError("greedy_generate_batch: no prompts")
     eos = _eos_set(eos_token_id)
+    spec = _check_spec(prompt_lookup_num_tokens, max_matching_ngram_size, sampling, logprobs, "greedy_generate_batch")
+    if spec is not None:
+        first, gen, cache = _speculative(model, ids, max_new_tokens, *spec, eos, pad_token_id, use_graph, check_every)
+        seqs = [torch.cat([p[0].cpu(), first[b].cpu(), torch.tensor(gen[b], dtype=torch.long)]).to(p.device)
+                for b, p in enumerate(ids)]
+        return (seqs, cache) if return_cache else seqs
     samp = _sampling_list(sampling, len(ids), "greedy_generate_batch")
     logprobs = _check_logprobs(logprobs, "greedy_generate_batch")
     firsts, caches, entries = [], [], []
@@ -901,6 +921,172 @@ def greedy_generate_batch(model, prompts, max_new_tokens: int, eos_token_id=None
     if logprobs is not None:
         out += ([_join_entries(s[p.shape[1]:].cpu(), e) for s, p, e in zip(seqs, ids, entries)],)
     return out if len(out) > 1 else seqs
+
+
+MAX_PROMPT_LOOKUP_TOKENS, MAX_MATCHING_NGRAM = 15, 8
+
+
+def _check_spec(num_tokens, ngram, sampling, logprobs, what: str):
+    """(K, N) of prompt-lookup speculative decoding, or None when it is off; ValueError for what it excludes."""
+    if num_tokens is None:
+        if ngram is not None:
+            raise ValueError(f"{what}: max_matching_ngram_size goes with prompt_lookup_num_tokens")
+        return None
+    ngram = 2 if ngram is None else ngram
+    for name, v, hi in (("prompt_lookup_num_tokens", num_tokens, MAX_PROMPT_LOOKUP_TOKENS),
+                        ("max_matching_ngram_size", ngram, MAX_MATCHING_NGRAM)):
+        if isinstance(v, bool) or not isinstance(v, int) or not 1 <= v <= hi:
+            raise ValueError(f"{what}: {name} must be an integer in [1, {hi}], got {v!r}")
+    if sampling is not None or logprobs is not None:
+        raise ValueError(f"{what}: prompt_lookup_num_tokens is greedy only: it excludes sampling and logprobs")
+    return int(num_tokens), int(ngram)
+
+
+def _check_spec_cache_form(model) -> None:
+    from .cache import decode_heavy, decode_window
+    for knob, v in (("pkv_decode_heavy", decode_heavy(model.config)), ("pkv_decode_window", decode_window(model.config))):
+        if v is not None:
+            raise NotImplementedError(f"prompt_lookup_num_tokens with {knob} = {v} is not built: the rows a verify step "
+                                      "writes for rejected drafts would already have replaced rows the decode window keeps")
+
+
+class SpecState:
+    """The device state of prompt-lookup speculative decoding (include/pkv.h: pkv_prompt_lookup, pkv_spec_step) over B
+    sequences with Q = K + 1 verify rows: each sequence's history (prompt, then every emitted token; int64 [B, cap] and its
+    length), remaining budget, done flag, the tokens the steps emitted (int64 [B, max_new_tokens - 1], pad_token_id past
+    each sequence's cursor `out_len`), the next verify step's input ids and positions [B, Q], the draft length, the tokens
+    the last step emitted and the verify argmaxes `tokens` [B, Q]. Every tensor is written in place, so a captured step
+    keeps its pointers."""
+
+    def __init__(self, prompts, first: torch.Tensor, max_new_tokens: int, K: int, N: int, eos, pad_token_id: int, device):
+        B, Q, steps = len(prompts), K + 1, max(0, int(max_new_tokens) - 1)
+        lens = [int(p.numel()) for p in prompts]
+        i32, i64 = dict(dtype=torch.int32, device=device), dict(dtype=torch.long, device=device)
+        self.hist = torch.zeros(B, max(lens) + max(1, int(max_new_tokens)), **i64)
+        for b, p in enumerate(prompts):
+            self.hist[b, : lens[b]] = p.reshape(-1).to(device)
+            self.hist[b, lens[b]] = first.reshape(-1)[b]
+        self.prompt_len = torch.tensor(lens, **i32)
+        self.hist_len = self.prompt_len + 1
+        self.budget = torch.full((B,), steps, **i32)
+        self.eos = torch.tensor(sorted(_eos_set(eos)), **i64)
+        if self.eos.numel() > 4:
+            raise ValueError("prompt_lookup_num_tokens: at most 4 EOS ids")
+        self.done = torch.isin(first.reshape(-1).to(device), self.eos) | (self.budget <= 0)
+        self.out = torch.full((B, max(1, steps)), int(pad_token_id), **i64)
+        self.out_len = torch.zeros(B, **i32)
+        self.ids = torch.zeros(B, Q, **i64)
+        self.pos = torch.zeros(B, Q, **i64)
+        self.draft_len = torch.zeros(B, **i32)
+        self.emitted = torch.zeros(B, **i32)
+        self.tokens = torch.zeros(B, Q, **i64)
+        self.max_ngram, self.pad_token_id = int(N), int(pad_token_id)
+
+    def state(self) -> list:
+        """The tensors a step advances (restored after the warm-up step of a graph capture; the history and output rows
+        past the restored cursors are rewritten by the next step)."""
+        return [self.hist_len, self.budget, self.done, self.out_len, self.ids, self.pos, self.draft_len, self.emitted,
+                self.tokens]
+
+
+class SpeculativeDecoder(StaticDecoder):
+    """Greedy prompt-lookup speculative decoding (HF's `generate(prompt_lookup_num_tokens=K, max_matching_ngram_size=N)`)
+    over a joined cache (`cache.join_caches`, any form but the decode window) of the prompts `prompts` whose prefill
+    produced `first_token` [B] or [B, 1]. One step, captured once in a CUDA graph: the embedding of the [B, Q] verify ids
+    (the last emitted token and up to K draft tokens), every layer (the attention stores the Q new rows and attends them
+    causally: `decode_multi`), the LM head on all B*Q rows, their argmax and one `pkv_spec_step` launch that accepts, emits,
+    advances every layer's row counts and drafts the next step's ids by prompt lookup (DESIGN.md §4.13). Each step emits
+    1 .. K + 1 tokens per live sequence, so max_new_tokens - 1 steps finish every sequence. `forced_drafts` (tests and
+    measurements): None, or int64 [B, F] - after every step sequence b drafts forced_drafts[b, E : E + K], E its tokens
+    generated so far (the prefill's included), in place of the lookup."""
+
+    def __init__(self, model, cache, first_token: torch.Tensor, prompts, max_new_tokens: int, num_tokens: int,
+                 max_ngram: int = 2, use_graph: Optional[bool] = None, eos_token_id=None, pad_token_id: int = 0,
+                 forced_drafts: Optional[torch.Tensor] = None):
+        layers = [l for l in cache.layers if isinstance(l, PkvBatchCacheLayer)]
+        if len(layers) != model.config.num_hidden_layers or len(layers) != len(cache.layers):
+            raise RuntimeError("SpeculativeDecoder needs a joined cache (cache.join_caches) on every layer")
+        if layers[0].window is not None:
+            raise NotImplementedError("speculative decoding under the decode window (pkv_decode_window / pkv_decode_heavy) "
+                                      "is not built")
+        K, steps = int(num_tokens), max(0, int(max_new_tokens) - 1)
+        for l in layers:
+            # the rows, the decoded tokens and one verify step's K + 1: a sequence that spent its budget still verifies (and
+            # writes, uncounted) Q rows behind its last one while the others run
+            l.reserve(steps + K + 1)
+        self._setup(model, cache, layers, first_token, max(1, steps), use_graph, None, pad_token_id, None)
+        dev, B = self.ids.device, len(prompts)
+        self.state.workspace = self.backend.decode_workspace(B * layers[0].num_q_heads * (K + 1), layers[0].k_buf.shape[3], dev)
+        self.state.spec = True
+        self.spec = SpecState(prompts, self.ids, max_new_tokens, K, max_ngram, eos_token_id, pad_token_id, dev)
+        self.ids, self.pos, self.done = self.spec.ids, self.spec.pos, self.spec.done
+        self.forced_drafts = None
+        if forced_drafts is not None:
+            self.forced_drafts = forced_drafts.to(device=dev, dtype=torch.long).contiguous()
+            self._offsets = torch.arange(K, device=dev)
+        self.backend.prompt_lookup(self.spec)
+        if self.forced_drafts is not None:
+            self._force_drafts()
+
+    def _force_drafts(self) -> None:
+        st, K = self.spec, self.spec.ids.shape[1] - 1
+        idx = ((st.hist_len - st.prompt_len).long()[:, None] + self._offsets).clamp_(max=self.forced_drafts.shape[1] - 1)
+        st.ids[:, 1:].copy_(self.forced_drafts.gather(1, idx))
+        st.draft_len.copy_(torch.where(st.done | (st.budget <= 1), 0, K))
+
+    def _verify_logits(self) -> torch.Tensor:
+        """The forward of the [B, Q] verify ids at their positions through every layer: logits [B, Q, V]."""
+        m = self.model.model
+        h = m.embed_tokens(self.ids)
+        pos_emb = m.rotary_emb(h, position_ids=self.pos)
+        for layer in m.layers[: self.model.config.num_hidden_layers]:
+            h = layer(h, attention_mask=None, position_embeddings=pos_emb, position_ids=self.pos,
+                      past_key_values=self.cache, use_cache=True)
+        return self.model.lm_head(m.norm(h))
+
+    def _step(self) -> None:
+        self.spec.tokens.copy_(self._verify_logits().argmax(dim=-1))
+        self.backend.spec_step(self.spec, [l.rows for l in self.layers])
+        if self.forced_drafts is not None:
+            self._force_drafts()
+
+    def _counters(self) -> list:
+        return self.spec.state() + [l.rows for l in self.layers]
+
+    def generated(self) -> list:
+        """Per sequence, the tokens the steps emitted (host lists; the prefill's first token not included)."""
+        out, n = self.spec.out.cpu(), self.spec.out_len.cpu().tolist()
+        return [out[b, : n[b]].tolist() for b in range(out.shape[0])]
+
+    def run_to_end(self, check_every: int = 16) -> int:
+        """Replay until every sequence is done (the host reads the done flags every `check_every` replays) or
+        max_new_tokens - 1 replays; returns the replays taken."""
+        while self.taken < self.max_steps and not bool(self.done.all()):
+            self.run(min(max(1, int(check_every)), self.max_steps - self.taken))
+        return self.taken
+
+
+def _speculative(model, ids, max_new_tokens: int, K: int, N: int, eos: set, pad_token_id: int, use_graph, check_every: int):
+    """Prefill each prompt alone, join the caches and decode them by prompt lookup: (first tokens [B, 1], generated host
+    lists per prompt, the joined cache with each sequence's rows ending at its last token)."""
+    _check_spec_cache_form(model)
+    firsts, caches = [], []
+    for p in ids:
+        f, c = _prefill(model, p, None, None, sorted(eos))
+        firsts.append(f)
+        caches.append(c)
+    first = torch.cat(firsts)
+    steps = max(0, max_new_tokens - 1)
+    cache = join_caches(caches, reserve=steps + K + 1)
+    del caches
+    gen = [[] for _ in ids]
+    if steps and not all(int(f) in eos for f in first[:, 0].tolist()):
+        dec = SpeculativeDecoder(model, cache, first, ids, max_new_tokens, K, N, use_graph=use_graph,
+                                 eos_token_id=sorted(eos) if eos else None, pad_token_id=pad_token_id)
+        dec.run_to_end(check_every)
+        gen = dec.generated()
+        dec.finish([len(g) for g in gen])
+    return first, gen, cache
 
 
 class ContinuousDecoder(StaticDecoder):

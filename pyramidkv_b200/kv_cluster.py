@@ -190,6 +190,18 @@ class CudaBackend:
     def decode_workspace(self, num_q_heads, head_dim, device):
         return torch.empty(ops.decode_workspace_bytes(num_q_heads, head_dim), dtype=torch.uint8, device=device)
 
+    # prompt-lookup speculative decoding (generate.SpeculativeDecoder)
+    def decode_attn_multi(self, q, k_buf, v_buf, k_new, v_new, rows=None, length=0, step=None, max_length=0, scales=None,
+                          gqa=False, workspace=None, out=None, softmax_scale=0.0):
+        return ops.decode_attn_multi(q, k_buf, v_buf, k_new, v_new, rows, length, step, max_length, scales, gqa, workspace, out,
+                                     softmax_scale)
+
+    def prompt_lookup(self, st):
+        ops.prompt_lookup(st)
+
+    def spec_step(self, st, rows):
+        ops.spec_step(st, rows)
+
     @staticmethod
     def check_knobs(method: str, window_size: int, max_capacity_prompt=None) -> None:
         """What the sm_90a scoring kernels take, checked when the cluster is built (the reference accepts any window_size;

@@ -10,7 +10,7 @@ from typing import Dict, Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import METHODS, POOLING, SCORE_KERNELS, DecodeDesc, DecodeHeavy, DecodeWindow, EvictDesc, RopeDesc, WsLayout
+from ._lib import METHODS, POOLING, SCORE_KERNELS, DecodeDesc, DecodeHeavy, DecodeMulti, DecodeWindow, EvictDesc, RopeDesc, SpecDesc, WsLayout
 
 _DTYPES = {torch.bfloat16: 0, torch.float16: 1}
 
@@ -1065,3 +1065,135 @@ def cache_reorder(items, P: int, k: int, parent: torch.Tensor, diverge: torch.Te
                                             planes, caps, base, hs if heavy else None, hg if heavy else None,
                                             vic if heavy else None, parent.data_ptr(), diverge.data_ptr(), step.data_ptr(),
                                             int(step_offset), torch.cuda.current_stream(k0.device).cuda_stream))
+
+
+# ---- prompt-lookup speculative decoding (include/pkv.h: pkv_decode_attn_multi, pkv_prompt_lookup, pkv_spec_step) ----
+def _token_rows(t: torch.Tensor) -> torch.Tensor:
+    """t [B, Q, H, D] as the kernel reads it: rows contiguous, token s*Q + j at one stride, strides multiples of 8
+    elements and a 16-byte aligned base (HF's [b, q, H, D] projections are, as they are); otherwise a contiguous copy."""
+    ok = t.stride(3) == 1 and t.stride(0) == t.shape[1] * t.stride(1) and t.stride(1) % 8 == 0 and t.stride(2) % 8 == 0 \
+        and t.data_ptr() % 16 == 0
+    return t if ok else t.contiguous()
+
+
+def decode_attn_multi(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor, k_new: torch.Tensor, v_new: torch.Tensor,
+                      rows: Optional[torch.Tensor] = None, length: int = 0, step: Optional[torch.Tensor] = None,
+                      max_length: int = 0, scales=None, gqa: bool = False, workspace: Optional[torch.Tensor] = None,
+                      out: Optional[torch.Tensor] = None, softmax_scale: float = 0.0) -> torch.Tensor:
+    """The verify attention of speculative decoding (`pkv_decode_attn_multi`): q [B, Q, Hq, D] and k_new / v_new
+    [B, Q, Hkv, D] (HF's projections, read in place), buffers [B, H, capacity, D] (H = Hq, or Hkv with `gqa`; float8_e4m3fn
+    with `scales` = (k_scale, v_scale) [B, H, capacity]). Sequence b, cache head c holds n0 = `length` (+ `*step`) (+
+    `rows[b*H + c]`) rows: the Q new rows are stored at n0 .. n0 + Q - 1 and query j attends rows [0, n0 + j + 1). The
+    launch is sized for `max_length` rows (default: the capacity) and replays in a CUDA graph. Returns out [B, Q, Hq, D]."""
+    what = "decode_attn_multi"
+    _require_cuda(q, k_buf, v_buf, k_new, v_new, rows, step, workspace, out, *(scales or ()))
+    if scales is not None:
+        _check_fp8_buffers(k_buf, v_buf, scales[0], scales[1], what)
+    elif k_buf.dim() != 4 or k_buf.shape != v_buf.shape or k_buf.stride() != v_buf.stride() or k_buf.stride(3) != 1 \
+            or k_buf.stride(2) != k_buf.shape[3]:
+        raise ValueError(f"{what}: k_buf / v_buf must be [B, H, capacity, D] tensors of equal shape and strides, rows contiguous")
+    B, H, cap, D = k_buf.shape
+    if q.dim() != 4 or q.shape[0] != B or q.shape[3] != D or not 1 <= q.shape[1] <= _lib.MAX_SPEC_QUERIES:
+        raise ValueError(f"{what}: q must be [B={B}, Q <= {_lib.MAX_SPEC_QUERIES}, Hq, D={D}], got {tuple(q.shape)}")
+    Q, Hq = q.shape[1], q.shape[2]
+    Hkv = k_new.shape[2] if k_new.dim() == 4 else -1
+    if k_new.shape != (B, Q, Hkv, D) or v_new.shape != k_new.shape or Hkv < 1 or Hq % Hkv \
+            or k_new.dtype != q.dtype or v_new.dtype != q.dtype or (H != (Hkv if gqa else Hq)):
+        raise ValueError(f"{what}: k_new / v_new must be [B, Q, Hkv, D] of q's dtype, and the cache hold "
+                         f"{'Hkv' if gqa else 'Hq'} heads; got {tuple(k_new.shape)}, {tuple(v_new.shape)}, cache heads {H}")
+    q, k_new, v_new = _token_rows(q), _token_rows(k_new), _token_rows(v_new)
+    if k_new.stride() != v_new.stride():
+        k_new, v_new = k_new.contiguous(), v_new.contiguous()
+    if out is None:
+        out = torch.empty(B, Q, Hq, D, dtype=q.dtype, device=q.device)
+    elif out.shape != (B, Q, Hq, D) or not out.is_contiguous() or out.dtype != q.dtype:
+        raise ValueError(f"{what}: out must be a contiguous [B, Q, Hq, D] tensor of q's dtype")
+    max_length = int(max_length) or cap
+    if not Q <= max_length <= cap or int(length) < 0:
+        raise ValueError(f"{what}: cache capacity {cap} exceeded or bad row counts (length {length}, max_length {max_length})")
+    if step is not None and (step.dtype != torch.int32 or step.numel() != 1):
+        raise ValueError("step must be an int32 device tensor with one element")
+    if rows is not None:
+        if rows.dtype != torch.int32 or rows.numel() != B * H or not rows.is_contiguous():
+            raise ValueError(f"{what}: rows must be a contiguous int32 device tensor of B*H = {B * H} elements")
+        if not torch.cuda.is_current_stream_capturing():
+            # (one device read; a captured launch relies on the caller, and the kernel writes no row of a count out of range)
+            most = int(rows.max()) + int(length) + (int(step) if step is not None else 0) + Q
+            if most > max_length:
+                raise ValueError(f"{what}: cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
+    d = DecodeDesc()
+    d.struct_bytes = C.sizeof(DecodeDesc)
+    d.dtype, d.num_q_heads, d.num_kv_heads, d.head_dim = _dtype_code(q), Hq, Hkv, D
+    d.device = q.device.index if q.device.index is not None else torch.cuda.current_device()
+    d.length = int(length)
+    d.q, d.k_new, d.v_new, d.out = q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), out.data_ptr()
+    d.k_cache, d.v_cache, d.cache_stride_h = k_buf.data_ptr(), v_buf.data_ptr(), k_buf.stride(1)
+    if workspace is None:
+        workspace = _workspace(q.device, decode_workspace_bytes(B * Hq * Q, D))
+    d.workspace, d.workspace_bytes = workspace.data_ptr(), workspace.numel() * workspace.element_size()
+    d.softmax_scale = float(softmax_scale)
+    m = DecodeMulti()
+    m.struct_bytes = C.sizeof(DecodeMulti)
+    m.num_seqs, m.num_queries, m.gqa_shared, m.cache_stride_b = B, Q, int(gqa), k_buf.stride(0)
+    m.rows = rows.data_ptr() if rows is not None else None
+    m.step_dev = step.data_ptr() if step is not None else None
+    m.max_length = max_length
+    if scales is not None:
+        m.k_scale, m.v_scale = scales[0].data_ptr(), scales[1].data_ptr()
+        m.scale_stride_h, m.scale_stride_b = scales[0].stride(1), scales[0].stride(0)
+    m.q_stride_t, m.q_stride_h = q.stride(1), q.stride(2)
+    m.kv_stride_t, m.kv_stride_h = k_new.stride(1), k_new.stride(2)
+    m.out_stride_t, m.out_stride_h = out.stride(1), out.stride(2)
+    _lib.check(_lib.lib().pkv_decode_attn_multi(C.byref(d), C.byref(m), torch.cuda.current_stream(q.device).cuda_stream))
+    return out
+
+
+_SPEC_FIELDS = (("hist", torch.int64, 2), ("hist_len", torch.int32, 1), ("budget", torch.int32, 1), ("done", torch.bool, 1),
+                ("out", torch.int64, 2), ("out_len", torch.int32, 1), ("ids", torch.int64, 2), ("pos", torch.int64, 2),
+                ("draft_len", torch.int32, 1), ("emitted", torch.int32, 1), ("tokens", torch.int64, 2))
+
+
+def _spec_desc(fn: str, st, rows=None):
+    """The pkv_spec_desc of a `generate.SpecState` (its device tensors, checked) and the row-count tensors of `rows`."""
+    B, Q = st.ids.shape
+    for name, dt, dim in _SPEC_FIELDS:
+        t = getattr(st, name)
+        _require_cuda(t)
+        if t.dtype != dt or t.dim() != dim or t.shape[0] != B or not t.is_contiguous() or (name in ("pos", "tokens") and t.shape[1] != Q):
+            raise ValueError(f"{fn}: {name} must be a contiguous {dt} device tensor of {B} rows" + (f" x {Q}" if dim == 2 else ""))
+    d = SpecDesc()
+    d.struct_bytes = C.sizeof(SpecDesc)
+    d.device = st.ids.device.index if st.ids.device.index is not None else torch.cuda.current_device()
+    d.num_seqs, d.num_queries, d.max_ngram, d.n_eos = B, Q, int(st.max_ngram), int(st.eos.numel())
+    d.pad_token_id, d.hist_cap, d.out_cap = int(st.pad_token_id), st.hist.shape[1], st.out.shape[1]
+    for name, _, _ in _SPEC_FIELDS:
+        setattr(d, name, getattr(st, name).data_ptr())
+    if st.eos.numel():
+        _require_cuda(st.eos)
+        if st.eos.dtype != torch.int64 or not st.eos.is_contiguous():
+            raise ValueError(f"{fn}: eos must be a contiguous int64 device tensor")
+        d.eos = st.eos.data_ptr()
+    table = None
+    if rows:
+        for r in rows:
+            _require_cuda(r)
+            if r.dtype != torch.int32 or not r.is_contiguous() or r.numel() != rows[0].numel() or r.numel() % B:
+                raise ValueError(f"{fn}: every row-count tensor must be a contiguous int32 device tensor of B*H elements")
+        table = (C.c_void_p * len(rows))(*[r.data_ptr() for r in rows])
+        d.num_layers, d.num_heads, d.rows = len(rows), rows[0].numel() // B, C.cast(table, C.c_void_p)
+    return d, table
+
+
+def prompt_lookup(st) -> None:
+    """Rule 1 of include/pkv.h for every sequence of `st` (`pkv_prompt_lookup`): its next verify ids, positions and draft
+    length from its history."""
+    d, _ = _spec_desc("prompt_lookup", st)
+    _lib.check(_lib.lib().pkv_prompt_lookup(C.byref(d), torch.cuda.current_stream(st.ids.device).cuda_stream))
+
+
+def spec_step(st, rows) -> None:
+    """Rule 3 then rule 1 for every sequence of `st` (`pkv_spec_step`) from its verify argmaxes `st.tokens`; `rows`: the
+    int32 [B*H] row counts of every layer, advanced by each sequence's emitted tokens (one launch per 32 layers)."""
+    d, table = _spec_desc("spec_step", st, list(rows))
+    _lib.check(_lib.lib().pkv_spec_step(C.byref(d), torch.cuda.current_stream(st.ids.device).cuda_stream))
+    del table

@@ -173,11 +173,15 @@ def _sync(device: torch.device) -> None:
         torch.cuda.synchronize(device)
 
 
-def _run_prompt_static(model, ids: torch.Tensor, max_new_tokens: int, use_graph: Optional[bool]) -> PromptResult:
+def _run_prompt_static(model, ids: torch.Tensor, max_new_tokens: int, use_graph: Optional[bool],
+                       prompt_lookup_num_tokens: Optional[int] = None) -> PromptResult:
     """Same record through the static loop (pyramidkv_b200.generate: pre-reserved cache, device-side row counter, one CUDA
-    graph replay per token). Prefill and decode are timed separately — no subtraction of two generate calls is needed."""
+    graph replay per token). Prefill and decode are timed separately — no subtraction of two generate calls is needed.
+    prompt_lookup_num_tokens K: the cache is joined and decoded by greedy prompt-lookup speculation (SpeculativeDecoder,
+    one graph replay per verify step, K draft tokens)."""
     from transformers import DynamicCache
-    from .generate import StaticDecoder
+    from .cache import join_caches
+    from .generate import SpeculativeDecoder, StaticDecoder
     dev = ids.device
 
     def prefill():
@@ -195,7 +199,21 @@ def _run_prompt_static(model, ids: torch.Tensor, max_new_tokens: int, use_graph:
         _sync(dev)
         t1 = time.perf_counter()
         toks, decode_s = [first], 0.0
-        if max_new_tokens > 1:
+        if max_new_tokens > 1 and prompt_lookup_num_tokens:
+            K = int(prompt_lookup_num_tokens)
+            cache = join_caches([cache], reserve=max_new_tokens + K)
+            dec = SpeculativeDecoder(model, cache, first, [ids[0]], max_new_tokens, K, use_graph=use_graph)
+            if dec.use_graph:
+                dec._capture()
+            _sync(dev)
+            t2 = time.perf_counter()
+            dec.run_to_end(max_new_tokens)
+            gen = dec.generated()
+            _sync(dev)
+            decode_s = time.perf_counter() - t2
+            toks.append(torch.tensor([gen[0]], dtype=torch.long, device=dev).reshape(1, -1))
+            dec.finish([len(gen[0])])
+        elif max_new_tokens > 1:
             dec = StaticDecoder(model, cache, first, max_new_tokens - 1, use_graph=use_graph)
             if dec.use_graph:
                 dec._capture()                       # graph capture is a one-off cost per prompt shape, not decode time
@@ -276,15 +294,19 @@ def _run_continuous(model, prompts: List[torch.Tensor], max_new_tokens: List[int
     return res, block
 
 
-def run_prompt(model, ids: torch.Tensor, max_new_tokens: int, decode_loop: str = "hf") -> PromptResult:
+def run_prompt(model, ids: torch.Tensor, max_new_tokens: int, decode_loop: str = "hf",
+               prompt_lookup_num_tokens: Optional[int] = None) -> PromptResult:
     """Greedy generate exactly as the reference runner does. One untimed warm-up call at this prompt length (allocator,
     cuBLAS heuristics, lazy module init), then two timed calls: one new token (prefill + eviction of all layers) and the
     full length; decode tok/s is taken over the difference. decode_loop = "static" / "static-eager" replaces HF's loop by
-    the static one (SURVEY.md §8 f3)."""
+    the static one (SURVEY.md §8 f3); with it, prompt_lookup_num_tokens K decodes by prompt-lookup speculation."""
     if decode_loop != "hf":
         if decode_loop not in ("static", "static-eager"):
             raise ValueError(f"decode_loop must be hf, static or static-eager, got {decode_loop!r}")
-        return _run_prompt_static(model, ids, max_new_tokens, None if decode_loop == "static" else False)
+        return _run_prompt_static(model, ids, max_new_tokens, None if decode_loop == "static" else False,
+                                  prompt_lookup_num_tokens)
+    if prompt_lookup_num_tokens:
+        raise NotImplementedError("prompt_lookup_num_tokens runs in the static loop (decode_loop static or static-eager)")
     dev = ids.device
     kw = dict(attention_mask=torch.ones_like(ids), num_beams=1, do_sample=False, pad_token_id=0, return_dict_in_generate=True)
     with torch.no_grad():
@@ -316,7 +338,8 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
               backend_factory: Optional[Callable] = None, out_path: Optional[str] = None, tag: Optional[dict] = None,
               decode_loop: str = "hf", floor: float = 0.2, head_beta: float = 1.01, head_path: str = "",
               capacity_ratio: float = -1, eval_batch_size: int = 1, kv_cache_dtype: str = "auto",
-              gqa_shared: bool = False, decode_window: Optional[int] = None, decode_heavy: Optional[int] = None) -> List[dict]:
+              gqa_shared: bool = False, decode_window: Optional[int] = None, decode_heavy: Optional[int] = None,
+              prompt_lookup_num_tokens: Optional[int] = None) -> List[dict]:
     """prompts: iterable of (name, prompt_tokens, max_new_tokens). One JSON record per prompt (also appended to out_path).
     eval_batch_size N > 1: consecutive prompts with the same max_new_tokens are decoded N at a time (static loops only;
     each prompt is still prefilled alone, so its prefill_ms, cache rows and tokens are its own).
@@ -330,7 +353,9 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
     with the most accumulated attention (model.config.pkv_decode_heavy); the records then carry "decode_heavy".
     decode_loop "continuous": every prompt goes through one greedy_generate_continuous with eval_batch_size slots, whatever
     its max_new_tokens; each record keeps its own prefill_ms, cache rows and tokens and carries the run's "continuous" block
-    (slots, decode_steps, occupancy, aggregate_tok_per_s) instead of a per-prompt decode rate."""
+    (slots, decode_steps, occupancy, aggregate_tok_per_s) instead of a per-prompt decode rate.
+    prompt_lookup_num_tokens K (static loops, eval_batch_size 1, an eviction method): greedy prompt-lookup speculative
+    decoding with K draft tokens per step; the records then carry "prompt_lookup_num_tokens"."""
     if kv_cache_dtype not in ("auto", "fp8_e4m3"):
         raise ValueError(f"kv_cache_dtype must be auto or fp8_e4m3, got {kv_cache_dtype!r}")
     if kv_cache_dtype != "auto" and canonical_method(method) == "fullkv":
@@ -351,6 +376,10 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
                                   "use --decode_loop static or static-eager with an eviction method (padded HF batches are not supported)")
     if decode_loop not in ("hf", "static", "static-eager", "continuous"):
         raise ValueError(f"decode_loop must be hf, static, static-eager or continuous, got {decode_loop!r}")
+    if prompt_lookup_num_tokens is not None and (decode_loop not in ("static", "static-eager") or eval_batch_size > 1
+                                                 or canonical_method(method) == "fullkv"):
+        raise NotImplementedError("--prompt_lookup_num_tokens runs in the static loop with eval_batch_size 1 and an eviction "
+                                  "method")
     if device is None:
         if not torch.cuda.is_available():
             raise RuntimeError("the runners need a CUDA device (H100, sm_90a); there is no CPU fallback")
@@ -390,6 +419,7 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
                        **({"gqa_shared": True} if gqa_shared else {}),
                        **({"decode_window": int(decode_window)} if decode_window is not None else {}),
                        **({"decode_heavy": int(decode_heavy)} if decode_heavy is not None else {}),
+                       **({"prompt_lookup_num_tokens": int(prompt_lookup_num_tokens)} if prompt_lookup_num_tokens else {}),
                        "dtype": str(dtype).replace("torch.", ""), "data": "synthetic token ids, random-init weights", **(tag or {}),
                        "prompt_tokens": r.prompt_tokens, "new_tokens": r.new_tokens, "prefill_ms": r.prefill_ms,
                        **({} if continuous else {"decode_tok_per_s": r.decode_tok_per_s}), **extra,
@@ -424,7 +454,7 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
                 rs, agg = _run_batch_static(model, ids, prompts[i][2], None if decode_loop == "static" else False)
                 batch = {"eval_batch_size": eval_batch_size, "batch_size": len(group), "batch_decode_tok_per_s_aggregate": agg}
             else:
-                rs = [run_prompt(model, ids[0], prompts[i][2], decode_loop if method != "fullkv" else "hf")]
+                rs = [run_prompt(model, ids[0], prompts[i][2], decode_loop if method != "fullkv" else "hf", prompt_lookup_num_tokens)]
             emit(group, rs, batch)
             i = group[-1] + 1
         return records

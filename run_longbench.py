@@ -56,6 +56,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--decode_loop", type=str, default="hf", choices=["hf", "static", "static-eager", "continuous"],
                    help="hf: model.generate as in the reference; static: pyramidkv_b200.generate (CUDA-graph replay per token); "
                         "continuous: every prompt through --eval_batch_size slots, a finished sequence's slot taking the next prompt")
+    p.add_argument("--prompt_lookup_num_tokens", type=int, default=None,
+                   help="--decode_loop static: greedy prompt-lookup speculative decoding with K (1..15) draft tokens per step "
+                        "(HF's generate argument of that name; DESIGN.md §4.13)")
     p.add_argument("--kv_cache_dtype", type=str, default="auto", choices=["auto", "fp8_e4m3"],
                    help="auto: the compacted cache in the model dtype; fp8_e4m3: FP8 bytes + one fp32 scale per row (half the KV bytes)")
     p.add_argument("--gqa_shared", action="store_true",
@@ -102,7 +105,8 @@ def main(argv=None, backend_factory=None, device=None):
                             floor=args.floor, head_beta=args.head_beta, head_path=args.head_path,
                             capacity_ratio=args.max_capacity_prompts_ratio, eval_batch_size=args.eval_batch_size,
                             kv_cache_dtype=args.kv_cache_dtype, gqa_shared=args.gqa_shared,
-                            decode_window=args.decode_window, decode_heavy=args.decode_heavy)
+                            decode_window=args.decode_window, decode_heavy=args.decode_heavy,
+                            prompt_lookup_num_tokens=args.prompt_lookup_num_tokens)
     n = len(recs)
     print(json.dumps({"summary": True, "arch": arch, "method": method, "max_capacity_prompts": capacity, "examples": n,
                       "mean_prefill_ms": sum(r["prefill_ms"] for r in recs) / n,
