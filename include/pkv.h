@@ -810,6 +810,51 @@ int pkv_prompt_lookup(const pkv_spec_desc* d, void* stream);
  * n_eos outside [0, 4], caps below 1, null or misaligned pointers. */
 int pkv_spec_step(const pkv_spec_desc* d, void* stream);
 
+/* ---- prompt-lookup speculation in the continuous loop: packed verify rows (DESIGN.md §4.14) ----
+ * A step verifies M = B + D token rows: one per slot and a budget of D draft tokens shared by the B slots. Rules 1, 3 and
+ * 4 above hold unchanged; rule 2' (pack) runs at the start of every step, before the verify forward:
+ *  2'. Slots take their draft tokens in turn, from slot r0 = step mod B (step: the decoder's step counter) wrapping
+ *      around. A done slot gets 0 rows. A live slot b gets 1 + d' rows, d' = min(d_b, m_b - 1, the budget left), d_b the
+ *      draft length of rule 1 and m_b the slot's remaining budget; draft_len[b] becomes d' (rule 3 accepts against the
+ *      truncated draft). The rows of each slot are contiguous and in slot order: row_start[b] = the rows of slots 0 .. b - 1;
+ *      packed row row_start[b] + j holds ids[b][j] at pos[b][j]. Rows no slot owns hold pad_token_id at position 0.
+ * Truncation changes no emitted token. A step writes at most m_b cache rows for slot b, so a slot needs the rows of the
+ * plain continuous loop (prompt rows + max_new_tokens), not the static loop's + K. */
+/* The packed layout of pkv_decode_attn_packed: sequence s owns the token rows [row_start[s], row_start[s] + row_count[s])
+ * of the M = total_rows rows q, k_new, v_new and out hold (DEVICE int32 [num_seqs] each; counts in [0, num_queries]).
+ * The ranges must ascend with s and not overlap (row_start[s] + row_count[s] <= row_start[s + 1]). */
+typedef struct pkv_decode_packed {
+    uint32_t struct_bytes;
+    int32_t total_rows;         /* M >= 1 */
+    const int32_t* row_start;
+    const int32_t* row_count;
+} pkv_decode_packed;
+/* pkv_decode_attn_multi over packed rows: query j < row_count[s] of sequence s reads q, k_new and v_new at token row
+ * row_start[s] + j (the strides of `m` are per token row), stores that row at n0 + j and attends rows [0, n0 + j + 1),
+ * as the dense launch does; its output lands in token row row_start[s] + j. A sequence whose count is 0 reads and writes
+ * nothing of its own, and the split count follows n0 + row_count[s]. Rows no sequence owns get a zero output (the rows
+ * between a sequence's last and the next one's first, before the first and after the last). A sequence whose range leaves
+ * [0, M) or whose count exceeds num_queries reads and writes nothing. The dense launch is this one with row_start[s] =
+ * s*Q and row_count[s] = Q (bit for bit). Workspace and errors as pkv_decode_attn_multi; also PKV_ERR_INVALID_ARG for a
+ * wrong p->struct_bytes, total_rows < 1, or a null or misaligned row_start / row_count. Graph-replayable. */
+int pkv_decode_attn_packed(const pkv_decode_desc* d, const pkv_decode_multi* m, const pkv_decode_packed* p, void* stream);
+/* Rule 2' for the B = d->num_seqs sequences of `d` (reads done, budget, ids, pos; truncates draft_len in place) into
+ * M = total_rows packed rows: ids / pos DEVICE int64 [M], row_start / row_count DEVICE int32 [B]. `step`: DEVICE int32,
+ * the step counter. `totals`: optional DEVICE int64 [2], advanced by the draft tokens granted and the live slots. One
+ * CTA, one scan over B; integer logic, graph-replayable. PKV_ERR_INVALID_ARG: the errors of pkv_prompt_lookup, a wrong
+ * struct_bytes, max_draft_tokens outside [1, B*(Q - 1)], total_rows below B + max_draft_tokens, null or misaligned
+ * pointers. */
+typedef struct pkv_spec_pack_desc {
+    uint32_t struct_bytes;
+    int32_t max_draft_tokens;   /* D */
+    int32_t total_rows;         /* M */
+    const int32_t* step;
+    int64_t* ids; int64_t* pos;
+    int32_t* row_start; int32_t* row_count;
+    int64_t* totals;
+} pkv_spec_pack_desc;
+int pkv_spec_pack(const pkv_spec_desc* d, const pkv_spec_pack_desc* k, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

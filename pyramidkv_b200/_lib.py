@@ -26,7 +26,7 @@ EXPORTS = [
     "pkv_decode_attn_heavy", "pkv_decode_heavy_workspace_bytes",
     "pkv_token_logprobs", "pkv_sample_tokens_penalized", "pkv_token_rules", "pkv_sample_tokens_constrained",
     "pkv_beam_candidates", "pkv_beam_step", "pkv_cache_reorder",
-    "pkv_decode_attn_multi", "pkv_prompt_lookup", "pkv_spec_step",
+    "pkv_decode_attn_multi", "pkv_prompt_lookup", "pkv_spec_step", "pkv_decode_attn_packed", "pkv_spec_pack",
 ]
 RULE_BIAS, RULE_BAN, RULE_BAD, RULE_STOP = 1, 2, 4, 8     # pkv_token_rules_desc.flags[b]
 SEQ_BIAS, SEQ_BAD, SEQ_STOP = 0, 1, 2                     # pkv_token_rules_desc.seq_kind
@@ -95,6 +95,17 @@ class SpecDesc(C.Structure):
         ("out", C.c_void_p), ("out_len", C.c_void_p), ("ids", C.c_void_p), ("pos", C.c_void_p), ("draft_len", C.c_void_p),
         ("emitted", C.c_void_p), ("tokens", C.c_void_p), ("eos", C.c_void_p), ("num_layers", C.c_int32),
         ("num_heads", C.c_int32), ("rows", C.c_void_p),
+    ]
+
+
+class DecodePacked(C.Structure):
+    _fields_ = [("struct_bytes", C.c_uint32), ("total_rows", C.c_int32), ("row_start", C.c_void_p), ("row_count", C.c_void_p)]
+
+
+class SpecPackDesc(C.Structure):
+    _fields_ = [
+        ("struct_bytes", C.c_uint32), ("max_draft_tokens", C.c_int32), ("total_rows", C.c_int32), ("step", C.c_void_p),
+        ("ids", C.c_void_p), ("pos", C.c_void_p), ("row_start", C.c_void_p), ("row_count", C.c_void_p), ("totals", C.c_void_p),
     ]
 
 
@@ -295,6 +306,10 @@ def lib() -> C.CDLL:
     L.pkv_cache_reorder.restype = i32
     L.pkv_decode_attn_multi.argtypes = [C.POINTER(DecodeDesc), C.POINTER(DecodeMulti), p]
     L.pkv_decode_attn_multi.restype = i32
+    L.pkv_decode_attn_packed.argtypes = [C.POINTER(DecodeDesc), C.POINTER(DecodeMulti), C.POINTER(DecodePacked), p]
+    L.pkv_decode_attn_packed.restype = i32
+    L.pkv_spec_pack.argtypes = [C.POINTER(SpecDesc), C.POINTER(SpecPackDesc), p]
+    L.pkv_spec_pack.restype = i32
     for name in ("pkv_prompt_lookup", "pkv_spec_step"):
         fn = getattr(L, name)
         fn.argtypes = [C.POINTER(SpecDesc), p]

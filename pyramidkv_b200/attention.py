@@ -193,8 +193,10 @@ def make_forward(method: str, modeling, original_forward):
             elif static is not None and getattr(static, "spec", False):
                 # the verify step of speculative decoding (generate.SpeculativeDecoder): the Q new rows of every sequence
                 # stored and attended causally in one launch per layer, q / k / v read in their [b, q, H, D] layout
-                attn_output = layer.decode_multi(cluster.backend, query_states.transpose(1, 2), key_states.transpose(1, 2),
-                                                 value_states.transpose(1, 2), static, self.scaling)
+                # (the continuous loop's packed rows: `decode_packed`, one [1, M] forward over every slot's rows)
+                fn = layer.decode_multi if static.pack is None else layer.decode_packed
+                attn_output = fn(cluster.backend, query_states.transpose(1, 2), key_states.transpose(1, 2),
+                                 value_states.transpose(1, 2), static, self.scaling)
             else:
                 # several new tokens after the prefill (not produced by generate()): generic append + library attention
                 keys, values = layer.update(key_states, value_states)

@@ -333,6 +333,19 @@ class PkvBatchCacheLayer(PkvCacheLayer):
                                          scales=self._scales(), gqa=self.group > 1, workspace=static.workspace,
                                          softmax_scale=softmax_scale)
 
+    def decode_packed(self, backend, q, k_new, v_new, static, softmax_scale: float = 0.0) -> torch.Tensor:
+        """The verify step of speculation in the continuous loop (generate.ContinuousSpecDecoder): q [1, M, Hq, D] and
+        k_new / v_new [1, M, Hkv, D], the projections of the packed token rows; `static.pack` (generate.PackState) gives
+        each sequence's rows. Sequence b stores its row_count[b] new rows at rows[b, h] .. and attends them causally
+        (`pkv_decode_attn_packed`); the row counts are advanced by the acceptance step. Returns out [1, M, Hq, D]."""
+        if self.window is not None:
+            raise NotImplementedError("speculative decoding under the decode window (pkv_decode_window / pkv_decode_heavy) is "
+                                      "not built: rejected rows would already have replaced ring rows the cache keeps")
+        pk = static.pack
+        return backend.decode_attn_packed(q, self.k_buf, self.v_buf, k_new, v_new, pk.row_start, pk.row_count, pk.num_queries,
+                                          rows=self.rows, max_length=self.capacity, scales=self._scales(),
+                                          gqa=self.group > 1, workspace=static.workspace, softmax_scale=softmax_scale)
+
     # -- continuous batching (generate.ContinuousDecoder): one slot rewritten in place while a decode graph holds the buffers --
     def admit(self, slot: int, src_layer, step: torch.Tensor, backend=None) -> None:
         """Copy the single-prompt layer `src_layer` (the form this batch holds: `PkvCacheLayer` / `PkvRaggedCacheLayer`, or,

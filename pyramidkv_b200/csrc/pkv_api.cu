@@ -1166,8 +1166,9 @@ int pkv_cache_reorder(int32_t num_prompts, int32_t num_beams, int32_t num_heads,
     return PKV_OK;
 }
 
-int pkv_decode_attn_multi(const pkv_decode_desc* d, const pkv_decode_multi* m, void* stream) {
-    const char* fn = "pkv_decode_attn_multi";
+// pkv_decode_attn_multi (pk NULL) and pkv_decode_attn_packed: one launch of the verify kernel.
+static int decode_multi_run(const char* fn, const pkv_decode_desc* d, const pkv_decode_multi* m, const pkv_decode_packed* pk,
+                            void* stream) {
     if (!d || !m) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
     if (d->struct_bytes != sizeof(pkv_decode_desc) || m->struct_bytes != sizeof(pkv_decode_multi))
         return fail(PKV_ERR_INVALID_ARG, "%s: struct_bytes mismatch (ABI)", fn);
@@ -1213,6 +1214,9 @@ int pkv_decode_attn_multi(const pkv_decode_desc* d, const pkv_decode_multi* m, v
     a.T = d->length; a.max_rows = m->max_length; a.step_dev = m->step_dev; a.rows = m->rows;
     a.scale = d->softmax_scale != 0.f ? d->softmax_scale : 1.0f / sqrtf(float(d->head_dim));
     a.ws = static_cast<float*>(d->workspace);
+    a.row_start = pk ? pk->row_start : nullptr;
+    a.row_count = pk ? pk->row_count : nullptr;
+    a.M = pk ? pk->total_rows : int64_t(m->num_seqs) * Q;
     if (a.nsplit > 1) {
         const uint64_t need = uint64_t(a.num_seqs) * a.Hq * Q * a.nsplit * (2 + a.D) * sizeof(float);
         if (!d->workspace || d->workspace_bytes < need || (reinterpret_cast<uintptr_t>(d->workspace) & 15u))
@@ -1221,6 +1225,21 @@ int pkv_decode_attn_multi(const pkv_decode_desc* d, const pkv_decode_multi* m, v
     DeviceGuard guard(d->device);
     const cudaError_t e = launch_decode_multi(a, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, fn);
+}
+
+int pkv_decode_attn_multi(const pkv_decode_desc* d, const pkv_decode_multi* m, void* stream) {
+    return decode_multi_run("pkv_decode_attn_multi", d, m, nullptr, stream);
+}
+
+int pkv_decode_attn_packed(const pkv_decode_desc* d, const pkv_decode_multi* m, const pkv_decode_packed* p, void* stream) {
+    const char* fn = "pkv_decode_attn_packed";
+    if (!p) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
+    if (p->struct_bytes != sizeof(pkv_decode_packed)) return fail(PKV_ERR_INVALID_ARG, "%s: struct_bytes mismatch (ABI)", fn);
+    if (p->total_rows < 1) return fail(PKV_ERR_INVALID_ARG, "%s: total_rows=%d below 1", fn, p->total_rows);
+    if (!p->row_start || !p->row_count || (reinterpret_cast<uintptr_t>(p->row_start) & 3u) ||
+        (reinterpret_cast<uintptr_t>(p->row_count) & 3u))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned row_start / row_count", fn);
+    return decode_multi_run(fn, d, m, p, stream);
 }
 
 static int spec_args(const char* fn, const pkv_spec_desc* d, bool step, SpecArgs* a) {
@@ -1258,6 +1277,31 @@ int pkv_prompt_lookup(const pkv_spec_desc* d, void* stream) {
     DeviceGuard guard(d->device);
     const cudaError_t e = launch_prompt_lookup(a, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? PKV_OK : fail_cuda(e, "prompt lookup launch");
+}
+
+int pkv_spec_pack(const pkv_spec_desc* d, const pkv_spec_pack_desc* k, void* stream) {
+    const char* fn = "pkv_spec_pack";
+    SpecArgs a;
+    int rc = spec_args(fn, d, false, &a);
+    if (rc) return rc;
+    if (!k) return fail(PKV_ERR_INVALID_ARG, "%s: null descriptor", fn);
+    if (k->struct_bytes != sizeof(pkv_spec_pack_desc))
+        return fail(PKV_ERR_INVALID_ARG, "pkv_spec_pack_desc.struct_bytes=%u, library expects %zu (ABI mismatch)", k->struct_bytes, sizeof(pkv_spec_pack_desc));
+    const int64_t most = int64_t(d->num_seqs) * (d->num_queries - 1);
+    if (k->max_draft_tokens < 1 || k->max_draft_tokens > most)
+        return fail(PKV_ERR_INVALID_ARG, "%s: max_draft_tokens=%d outside [1, %lld]", fn, k->max_draft_tokens, (long long)most);
+    if (int64_t(k->total_rows) < int64_t(d->num_seqs) + k->max_draft_tokens)
+        return fail(PKV_ERR_INVALID_ARG, "%s: total_rows=%d below num_seqs + max_draft_tokens", fn, k->total_rows);
+    auto bad = [](const void* p, uintptr_t align) { return !p || (reinterpret_cast<uintptr_t>(p) & (align - 1)); };
+    if (bad(k->step, 4) || bad(k->ids, 8) || bad(k->pos, 8) || bad(k->row_start, 4) || bad(k->row_count, 4) ||
+        (k->totals && bad(k->totals, 8)))
+        return fail(PKV_ERR_INVALID_ARG, "%s: null or misaligned pointer", fn);
+    PackArgs p;
+    p.D = k->max_draft_tokens; p.M = k->total_rows; p.step = k->step; p.ids = k->ids; p.pos = k->pos;
+    p.row_start = k->row_start; p.row_count = k->row_count; p.totals = k->totals;
+    DeviceGuard guard(d->device);
+    const cudaError_t e = launch_spec_pack(a, p, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PKV_OK : fail_cuda(e, "spec pack launch");
 }
 
 int pkv_spec_step(const pkv_spec_desc* d, void* stream) {

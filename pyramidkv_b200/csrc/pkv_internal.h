@@ -156,7 +156,8 @@ cudaError_t launch_append(const DecodeArgs& a, cudaStream_t st);
 
 // ---- speculative decoding (pkv_spec.cu) ----
 // The verify attention: Q new rows per (sequence, cache head) stored at n0 .. n0 + Q - 1, n0 = T (+ *step_dev) (+ rows[..]);
-// query j attends rows [0, n0 + j + 1). n0 < 0 or n0 + Q > max_rows: NaN output, nothing written.
+// query j attends rows [0, n0 + j + 1). n0 < 0 or n0 + Q > max_rows: NaN output, nothing written. Packed (row_count set):
+// sequence s has row_count[s] new rows at token rows row_start[s] + j of M; split 0 zeroes the output rows no sequence owns.
 struct MultiArgs {
     int dtype, Hq, Hkv, G, D, Q, num_seqs, heads_per_cache, nsplit, num_sms;
     const uint16_t *q, *k_new, *v_new;   // token s*Q + j, head h at + (s*Q + j)**_st + h*_sh elements
@@ -171,6 +172,9 @@ struct MultiArgs {
     const int32_t* rows;
     float scale;
     float* ws;                           // [num_seqs*Hq*Q][nsplit][2 + D] when nsplit > 1
+    const int32_t* row_start;            // packed rows (pkv_decode_attn_packed); NULL: the dense layout start s*Q, count Q
+    const int32_t* row_count;
+    int64_t M;                           // packed token rows
 };
 size_t decode_multi_smem_bytes(int heads_per_cache, int Q, int D);
 cudaError_t launch_decode_multi(const MultiArgs& a, cudaStream_t st);
@@ -187,6 +191,14 @@ struct SpecArgs {
 cudaError_t launch_prompt_lookup(const SpecArgs& a, cudaStream_t st);
 // first: the step kernel (rule 3, the rows of a.rows, rule 1); otherwise only the rows of a.rows, by emitted[b]
 cudaError_t launch_spec_step(const SpecArgs& a, bool first, cudaStream_t st);
+struct PackArgs {   // rule 2' (pkv_spec_pack)
+    int D, M;
+    const int32_t* step;
+    int64_t *ids, *pos;
+    int32_t *row_start, *row_count;
+    int64_t* totals;
+};
+cudaError_t launch_spec_pack(const SpecArgs& a, const PackArgs& k, cudaStream_t st);
 
 // ---- conversion of the compacted cache to FP8 (E4M3) rows (pkv_fp8.cu) ----
 struct QuantLayer {

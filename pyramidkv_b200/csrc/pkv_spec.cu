@@ -10,6 +10,8 @@
 // rows [0, n0 + j + 1). Per (query row, tile): lane r computes the dot with row r (K tile padded to D + 1 floats per row, so
 // the 32 lanes hit 32 banks), one warp max / sum gives the online softmax step, and the lanes then own D / 32 output dims
 // each. Accumulators live in shared memory, so the register count does not grow with Q or the group.
+// The packed launch (pkv_decode_attn_packed) runs the same body with a per-sequence row count c <= Q read on the device:
+// the CTA works on GH * c query rows, and a count of 0 returns before anything of the sequence is read or written.
 #include "pkv_common.cuh"
 #include "pkv_internal.h"
 #include "pkv_rows.cuh"
@@ -41,13 +43,43 @@ __host__ __device__ inline MultiSmem multi_smem(int M, int Q, int D) {
     return s;
 }
 
+// The token rows of sequence s: [*base, *base + *cnt). Dense: s*Q and Q. Packed: row_start / row_count; false when the range
+// leaves [0, M) or the count exceeds Q (the sequence is then skipped).
+__device__ __forceinline__ bool seq_rows(const MultiArgs& p, int s, int64_t* base, int* cnt) {
+    if (!p.row_count) {
+        *base = int64_t(s) * p.Q;
+        *cnt = p.Q;
+        return true;
+    }
+    *base = __ldg(p.row_start + s);
+    *cnt = __ldg(p.row_count + s);
+    return *cnt >= 0 && *cnt <= p.Q && *base >= 0 && *base + *cnt <= p.M;
+}
+
+// Packed: zero the output rows of heads [h0, h0 + GH) between sequence s's last row and the next sequence's first (the
+// last sequence: up to M; sequence 0 also those before its first).
+__device__ void zero_gaps(const MultiArgs& p, int s, int h0, int GH, int D) {
+    const int64_t start = __ldg(p.row_start + s);
+    const int64_t end = max(int64_t(0), start + max(0, __ldg(p.row_count + s)));
+    const int64_t next = s + 1 < p.num_seqs ? int64_t(__ldg(p.row_start + s + 1)) : p.M;
+    const uint16_t zero = 0;
+    for (int part = 0; part < 2; ++part) {
+        const int64_t lo = part ? end : 0, hi = min(p.M, part ? next : (s == 0 ? start : 0));
+        for (int64_t x = threadIdx.x; x < (hi - lo) * GH * D; x += kMultiThreads) {
+            const int64_t r = lo + x / (int64_t(GH) * D);
+            const int hi_ = int(x / D % GH), d = int(x % D);
+            p.out[r * p.out_st + int64_t(h0 + hi_) * p.out_sh + d] = zero;
+        }
+    }
+}
+
 template <typename T, int D, bool kE4M3>
 __global__ void __launch_bounds__(kMultiThreads) decode_multi_kernel(const MultiArgs p) {
     using Elem = typename std::conditional<kE4M3, uint8_t, uint16_t>::type;
     constexpr int DPL = D / 32;   // output dims per lane
     extern __shared__ float smem[];
-    const int Q = p.Q, GH = p.heads_per_cache, M = GH * Q;
-    const MultiSmem L = multi_smem(M, Q, D);
+    const int Q = p.Q, GH = p.heads_per_cache;
+    const MultiSmem L = multi_smem(GH * Q, Q, D);
     float* s_q = smem + L.q;
     float* s_acc = smem + L.acc;
     float* s_ml = smem + L.ml;
@@ -65,6 +97,11 @@ __global__ void __launch_bounds__(kMultiThreads) decode_multi_kernel(const Multi
     const int64_t sc = int64_t(s) * heads + c;                         // (sequence, cache head)
     const int kvh = GH > 1 ? c : c / p.G;                              // the kv head whose new rows this cache head takes
     const int h0 = GH > 1 ? c * GH : c;                                // first query head
+    if (p.row_count && split == 0) zero_gaps(p, s, h0, GH, D);
+    int64_t base;                                                      // token row of the sequence's query 0
+    int cnt;                                                           // its new rows (queries per head)
+    if (!seq_rows(p, s, &base, &cnt) || cnt == 0) return;
+    const int M = GH * cnt;
     Elem* kc = static_cast<Elem*>(p.k_cache) + int64_t(s) * p.cache_sb + int64_t(c) * p.cache_sh;
     Elem* vc = static_cast<Elem*>(p.v_cache) + int64_t(s) * p.cache_sb + int64_t(c) * p.cache_sh;
     const int64_t scale_off = int64_t(s) * p.scale_sb + int64_t(c) * p.scale_sh;
@@ -72,8 +109,8 @@ __global__ void __launch_bounds__(kMultiThreads) decode_multi_kernel(const Multi
     int64_t n0 = p.T;   // rows held before this step's Q rows
     if (p.step_dev) n0 += int64_t(__ldg(p.step_dev));
     if (p.rows) n0 += int64_t(__ldg(p.rows + sc));
-    const bool valid = n0 >= 0 && n0 + Q <= p.max_rows;
-    const int64_t rows = valid ? n0 + Q : 0;                           // the largest attended count
+    const bool valid = n0 >= 0 && n0 + cnt <= p.max_rows;
+    const int64_t rows = valid ? n0 + cnt : 0;                         // the largest attended count
     const int64_t ns = min(int64_t(p.nsplit), decode_splits_for(p.Hq, rows, p.num_sms));
     const int64_t chunk = (rows + ns - 1) / ns;
     const int64_t r_begin = int64_t(split) * chunk;
@@ -81,8 +118,8 @@ __global__ void __launch_bounds__(kMultiThreads) decode_multi_kernel(const Multi
 
     // queries (fp32) and fresh accumulators
     for (int x = tid; x < M * D; x += kMultiThreads) {
-        const int i = x / D, d = x % D, hi = i / Q, j = i % Q;
-        const uint16_t* src = p.q + (int64_t(s) * Q + j) * p.q_st + int64_t(h0 + hi) * p.q_sh;
+        const int i = x / D, d = x % D, hi = i / cnt, j = i % cnt;
+        const uint16_t* src = p.q + (base + j) * p.q_st + int64_t(h0 + hi) * p.q_sh;
         s_q[x] = DT<T>::to_f32(src[d]);
         s_acc[x] = 0.f;
     }
@@ -91,9 +128,9 @@ __global__ void __launch_bounds__(kMultiThreads) decode_multi_kernel(const Multi
         s_ml[2 * i + 1] = 0.f;
     }
     // the Q new rows: warp w builds rows w, w + 8, ... of K and V (lane l holds dims l*DPL .. l*DPL + DPL - 1)
-    for (int x = warp; x < 2 * Q; x += kMultiWarps) {
+    for (int x = warp; x < 2 * cnt; x += kMultiWarps) {
         const int j = x >> 1, which = x & 1;
-        const uint16_t* src = (which ? p.v_new : p.k_new) + (int64_t(s) * Q + j) * p.kv_st + int64_t(kvh) * p.kv_sh + lane * DPL;
+        const uint16_t* src = (which ? p.v_new : p.k_new) + (base + j) * p.kv_st + int64_t(kvh) * p.kv_sh + lane * DPL;
         float v[DPL];
 #pragma unroll
         for (int e = 0; e < DPL; ++e) v[e] = DT<T>::to_f32(src[e]);
@@ -205,7 +242,7 @@ __global__ void __launch_bounds__(kMultiThreads) decode_multi_kernel(const Multi
         const int64_t row = t0 + lane;
         const float* krow = s_k + lane * (D + 1);
         for (int i = warp; i < M; i += kMultiWarps) {
-            const int j = i % Q;
+            const int j = i % cnt;
             const float* qrow = s_q + i * D;
             float dot = 0.f;
 #pragma unroll 16
@@ -246,11 +283,11 @@ __global__ void __launch_bounds__(kMultiThreads) decode_multi_kernel(const Multi
     }
 
     for (int x = tid; x < M * D; x += kMultiThreads) {
-        const int i = x / D, d = x % D, hi = i / Q, j = i % Q;
+        const int i = x / D, d = x % D, hi = i / cnt, j = i % cnt;
         const float m = s_ml[2 * i], l = s_ml[2 * i + 1], a = s_acc[x];
         const int64_t h = h0 + hi;
         if (p.nsplit == 1) {
-            p.out[(int64_t(s) * Q + j) * p.out_st + h * p.out_sh + d] = DT<T>::from_f32(a / l);
+            p.out[(base + j) * p.out_st + h * p.out_sh + d] = DT<T>::from_f32(a / l);
         } else {
             float* w = p.ws + (((int64_t(s) * p.Hq + h) * Q + j) * p.nsplit + split) * (2 + D);
             if (d == 0) { w[0] = m; w[1] = l; }
@@ -264,6 +301,9 @@ __global__ void decode_multi_combine_kernel(const MultiArgs p) {   // one CTA pe
     const int64_t x = blockIdx.x;
     const int d = threadIdx.x;
     const int64_t j = x % p.Q, h = (x / p.Q) % p.Hq, s = x / (int64_t(p.Q) * p.Hq);
+    int64_t base;
+    int cnt;
+    if (!seq_rows(p, int(s), &base, &cnt) || j >= cnt) return;   // a row no query of s owns (zeroed by split 0)
     const float* w = p.ws + x * p.nsplit * (2 + D);
     float mn = -INFINITY;
     for (int k = 0; k < p.nsplit; ++k) mn = fmaxf(mn, w[k * (2 + D)]);
@@ -274,7 +314,7 @@ __global__ void decode_multi_combine_kernel(const MultiArgs p) {   // one CTA pe
         lt += w[k * (2 + D) + 1] * c;
         at += w[k * (2 + D) + 2 + d] * c;
     }
-    p.out[(s * p.Q + j) * p.out_st + h * p.out_sh + d] = DT<T>::from_f32(at / lt);
+    p.out[(base + j) * p.out_st + h * p.out_sh + d] = DT<T>::from_f32(at / lt);
 }
 
 template <typename T, int D, bool kE4M3>
@@ -421,7 +461,96 @@ __global__ void spec_rows_kernel(const SpecArgs p) {   // the row counts of laye
     for (int x = threadIdx.x; x < p.n_layers * p.H; x += blockDim.x) p.rows[x / p.H][int64_t(b) * p.H + x % p.H] += n;
 }
 
+// ---- rule 2' (pack): one CTA; one scan over the slots in rotation order, then each slot's rows ----
+constexpr int kPackThreads = 1024;
+
+// Exclusive block scan of v (all threads take part); *total gets the sum over the block.
+__device__ long long block_exclusive_scan(long long v, long long* total) {
+    __shared__ long long s_warp[kPackThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    long long x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const long long y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        long long w = s_warp[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const long long y = __shfl_up_sync(0xffffffffu, w, o);
+            if (lane >= o) w += y;
+        }
+        s_warp[lane] = w;   // inclusive over warps
+    }
+    __syncthreads();
+    const long long before = (warp ? s_warp[warp - 1] : 0) + x - v;
+    *total = s_warp[kPackThreads / 32 - 1];
+    __syncthreads();        // s_warp is reused by the next call
+    return before;
+}
+
+// Slot b at rotation position k = (b - r0) mod B. The scan runs over k and carries (draft tokens wanted, live slots) in one
+// 64-bit value: the budget granted before position k is min(P_k, D), so d' = min(want, max(0, D - P_k)), and the rows of
+// the positions before k are R_k = L_k + min(P_k, D). Slot order then shifts every start by the rows of slots 0 .. r0 - 1.
+__global__ void __launch_bounds__(kPackThreads) spec_pack_kernel(const SpecArgs p, const PackArgs k) {
+    __shared__ long long s_r0;   // R of slot 0
+    const int B = p.num_seqs, Q = p.Q;
+    const int r0 = int(((int64_t(__ldg(k.step)) % B) + B) % B);
+    long long carry = 0;         // (wanted << 0) + (live << 32), summed over the positions already scanned
+    for (int k0 = 0; k0 < B; k0 += kPackThreads) {
+        const int pos = k0 + int(threadIdx.x);
+        const int b = pos < B ? (r0 + pos) % B : 0;
+        long long want = 0, live = 0;
+        if (pos < B && !p.done[b]) {
+            live = 1;
+            want = max(0, min(p.draft_len[b], p.budget[b] - 1));
+        }
+        long long total;
+        const long long before = carry + block_exclusive_scan(want + (live << 32), &total);
+        if (pos < B) {
+            const long long P = before & 0xffffffffll, L = before >> 32;
+            const int granted = int(min(want, max(0ll, k.D - P)));
+            p.draft_len[b] = granted;
+            k.row_count[b] = int(live) + granted;
+            const long long R = L + min(P, (long long)k.D);
+            k.row_start[b] = int(R);   // rotation order for now
+            if (b == 0) s_r0 = R;
+        }
+        carry += total;
+    }
+    __syncthreads();
+    const long long Ptot = carry & 0xffffffffll, Ltot = carry >> 32;
+    const long long rows = Ltot + min(Ptot, (long long)k.D);
+    const long long shift = r0 ? rows - s_r0 : 0;   // the rows of slots 0 .. r0 - 1
+    if (threadIdx.x == 0 && k.totals) {
+        k.totals[0] += min(Ptot, (long long)k.D);
+        k.totals[1] += Ltot;
+    }
+    for (int b = threadIdx.x; b < B; b += kPackThreads) {
+        const long long R = k.row_start[b];
+        const int start = int(b >= r0 ? R + shift : R - s_r0);
+        k.row_start[b] = start;
+        for (int j = 0; j < k.row_count[b]; ++j) {
+            k.ids[start + j] = p.ids[int64_t(b) * Q + j];
+            k.pos[start + j] = p.pos[int64_t(b) * Q + j];
+        }
+    }
+    for (long long r = rows + threadIdx.x; r < k.M; r += kPackThreads) {
+        k.ids[r] = p.pad;
+        k.pos[r] = 0;
+    }
+}
+
 }  // namespace
+
+cudaError_t launch_spec_pack(const SpecArgs& a, const PackArgs& k, cudaStream_t st) {
+    spec_pack_kernel<<<1, kPackThreads, 0, st>>>(a, k);
+    count_launch();
+    return cudaGetLastError();
+}
 
 size_t decode_multi_smem_bytes(int heads_per_cache, int Q, int D) {
     return size_t(multi_smem(heads_per_cache * Q, Q, D).total) * sizeof(float);

@@ -536,6 +536,7 @@ class _StaticState:
     workspace: torch.Tensor   # split-T partials, shared by all layers (launches are stream-ordered)
     heavy_scratch: Optional[torch.Tensor] = None   # knob pkv_decode_heavy: the per-step logits, shared by all layers
     spec: bool = False        # the verify step of speculative decoding: q_len > 1 goes through `decode_multi`
+    pack: Optional["PackState"] = None   # ... or, in the continuous loop, over packed rows through `decode_packed`
 
 
 class StaticDecoder:
@@ -956,9 +957,11 @@ class SpecState:
     length), remaining budget, done flag, the tokens the steps emitted (int64 [B, max_new_tokens - 1], pad_token_id past
     each sequence's cursor `out_len`), the next verify step's input ids and positions [B, Q], the draft length, the tokens
     the last step emitted and the verify argmaxes `tokens` [B, Q]. Every tensor is written in place, so a captured step
-    keeps its pointers."""
+    keeps its pointers. `budgets` (one per sequence, in place of max_new_tokens - 1 for all) and `out_cap` (the width of
+    `out`) serve the continuous loop, whose slots come and go."""
 
-    def __init__(self, prompts, first: torch.Tensor, max_new_tokens: int, K: int, N: int, eos, pad_token_id: int, device):
+    def __init__(self, prompts, first: torch.Tensor, max_new_tokens: int, K: int, N: int, eos, pad_token_id: int, device,
+                 budgets=None, out_cap: Optional[int] = None):
         B, Q, steps = len(prompts), K + 1, max(0, int(max_new_tokens) - 1)
         lens = [int(p.numel()) for p in prompts]
         i32, i64 = dict(dtype=torch.int32, device=device), dict(dtype=torch.long, device=device)
@@ -968,12 +971,12 @@ class SpecState:
             self.hist[b, lens[b]] = first.reshape(-1)[b]
         self.prompt_len = torch.tensor(lens, **i32)
         self.hist_len = self.prompt_len + 1
-        self.budget = torch.full((B,), steps, **i32)
+        self.budget = torch.full((B,), steps, **i32) if budgets is None else torch.tensor([int(n) for n in budgets], **i32)
         self.eos = torch.tensor(sorted(_eos_set(eos)), **i64)
         if self.eos.numel() > 4:
             raise ValueError("prompt_lookup_num_tokens: at most 4 EOS ids")
         self.done = torch.isin(first.reshape(-1).to(device), self.eos) | (self.budget <= 0)
-        self.out = torch.full((B, max(1, steps)), int(pad_token_id), **i64)
+        self.out = torch.full((B, max(1, steps) if out_cap is None else int(out_cap)), int(pad_token_id), **i64)
         self.out_len = torch.zeros(B, **i32)
         self.ids = torch.zeros(B, Q, **i64)
         self.pos = torch.zeros(B, Q, **i64)
@@ -987,6 +990,43 @@ class SpecState:
         past the restored cursors are rewritten by the next step)."""
         return [self.hist_len, self.budget, self.done, self.out_len, self.ids, self.pos, self.draft_len, self.emitted,
                 self.tokens]
+
+    def set_row(self, b: int, prompt: torch.Tensor, first: torch.Tensor, budget: int) -> bool:
+        """Sequence b starts over with `prompt` (1-D ids), its first token and `budget` tokens to emit, in place. True when
+        the history had to grow (a new tensor: a captured step must be captured again)."""
+        prompt = prompt.reshape(-1)
+        n = int(prompt.numel())
+        grew = n + 1 + max(0, int(budget)) > self.hist.shape[1]
+        if grew:
+            hist = torch.zeros(self.hist.shape[0], n + 1 + int(budget), dtype=self.hist.dtype, device=self.hist.device)
+            hist[:, : self.hist.shape[1]] = self.hist
+            self.hist = hist
+        first = first.reshape(-1)[:1].to(self.hist.device)
+        self.hist[b, :n] = prompt.to(self.hist.device)
+        self.hist[b, n] = first[0]
+        self.prompt_len[b] = n
+        self.hist_len[b] = n + 1
+        self.budget[b] = int(budget)
+        self.done[b] = bool(torch.isin(first, self.eos).any()) or int(budget) <= 0
+        self.out_len[b] = 0
+        return grew
+
+
+class PackState:
+    """The packed verify rows of a continuous speculative step (include/pkv.h: pkv_spec_pack, pkv_decode_attn_packed):
+    M = B + max_draft_tokens token rows, their ids and positions (int64 [1, M]), each slot's first row and row count (int32
+    [B]), the step counter `step` the budget rotation starts from, and `totals` int64 [2]: the draft tokens granted and
+    the live slot-steps, summed over the steps."""
+
+    def __init__(self, B: int, K: int, max_draft_tokens: int, step: torch.Tensor, device):
+        M = B + int(max_draft_tokens)
+        self.num_queries, self.max_draft_tokens = K + 1, int(max_draft_tokens)
+        self.ids = torch.zeros(1, M, dtype=torch.long, device=device)
+        self.pos = torch.zeros(1, M, dtype=torch.long, device=device)
+        self.row_start = torch.zeros(B, dtype=torch.int32, device=device)
+        self.row_count = torch.zeros(B, dtype=torch.int32, device=device)
+        self.step = step
+        self.totals = torch.zeros(2, dtype=torch.long, device=device)
 
 
 class SpeculativeDecoder(StaticDecoder):
@@ -1036,13 +1076,7 @@ class SpeculativeDecoder(StaticDecoder):
 
     def _verify_logits(self) -> torch.Tensor:
         """The forward of the [B, Q] verify ids at their positions through every layer: logits [B, Q, V]."""
-        m = self.model.model
-        h = m.embed_tokens(self.ids)
-        pos_emb = m.rotary_emb(h, position_ids=self.pos)
-        for layer in m.layers[: self.model.config.num_hidden_layers]:
-            h = layer(h, attention_mask=None, position_embeddings=pos_emb, position_ids=self.pos,
-                      past_key_values=self.cache, use_cache=True)
-        return self.model.lm_head(m.norm(h))
+        return _forward_rows(self.model, self.cache, self.ids, self.pos)
 
     def _step(self) -> None:
         self.spec.tokens.copy_(self._verify_logits().argmax(dim=-1))
@@ -1064,6 +1098,16 @@ class SpeculativeDecoder(StaticDecoder):
         while self.taken < self.max_steps and not bool(self.done.all()):
             self.run(min(max(1, int(check_every)), self.max_steps - self.taken))
         return self.taken
+
+
+def _forward_rows(model, cache, ids: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
+    """The forward of token rows `ids` at positions `pos` (both [b, q]) through every layer over `cache`: logits [b, q, V]."""
+    m = model.model
+    h = m.embed_tokens(ids)
+    pos_emb = m.rotary_emb(h, position_ids=pos)
+    for layer in m.layers[: model.config.num_hidden_layers]:
+        h = layer(h, attention_mask=None, position_embeddings=pos_emb, position_ids=pos, past_key_values=cache, use_cache=True)
+    return model.lm_head(m.norm(h))
 
 
 def _speculative(model, ids, max_new_tokens: int, K: int, N: int, eos: set, pad_token_id: int, use_graph, check_every: int):
@@ -1201,6 +1245,104 @@ class ContinuousDecoder(StaticDecoder):
         self.taken = 0
 
 
+class ContinuousSpecDecoder(SpeculativeDecoder, ContinuousDecoder):
+    """Greedy prompt-lookup speculation in the continuous loop (DESIGN.md §4.14): the slots of `ContinuousDecoder`, each
+    step a verify step of `SpeculativeDecoder` over M = B + max_draft_tokens packed token rows instead of a dense [B, K + 1]
+    block. One step, captured once in a CUDA graph: `pkv_spec_pack` (rule 2': every live slot gets its last token and a
+    share of the max_draft_tokens draft tokens, in turn from slot step mod B; a done slot gets no row), the forward of the
+    [1, M] rows (the attention stores and attends each slot's rows: `decode_packed`), the LM head and argmax on the M rows,
+    a gather of each slot's argmaxes into `spec.tokens` and `pkv_spec_step`. `prompts` and `first_token` [B] as in
+    `SpeculativeDecoder`; left[b] the tokens slot b may still emit; `chunk` the steps between host reads (`run_chunk`).
+    Between chunks `admit` rewrites a slot in place and `park` leaves one done. `history`: the longest budget a later
+    admission brings (the history is sized for it). `forced_drafts` (tests and measurements): None, or int64 [B, F] per
+    slot, as in `SpeculativeDecoder`; `admit` takes the new request's row."""
+
+    def __init__(self, model, cache, first_token: torch.Tensor, prompts, left, chunk: int, num_tokens: int, max_ngram: int = 2,
+                 max_draft_tokens: Optional[int] = None, use_graph: Optional[bool] = None, eos_token_id=None,
+                 pad_token_id: int = 0, history: int = 0, forced_drafts: Optional[torch.Tensor] = None):
+        layers = [l for l in cache.layers if isinstance(l, PkvBatchCacheLayer)]
+        if len(layers) != model.config.num_hidden_layers or len(layers) != len(cache.layers):
+            raise RuntimeError("ContinuousSpecDecoder needs a batched cache (cache.join_caches) on every layer")
+        if layers[0].window is not None:
+            raise NotImplementedError("speculative decoding under the decode window (pkv_decode_window / pkv_decode_heavy) "
+                                      "is not built")
+        B, K, chunk = len(prompts), int(num_tokens), max(1, int(chunk))
+        D = B * K if max_draft_tokens is None else int(max_draft_tokens)
+        if not 1 <= D <= B * K:
+            raise ValueError(f"max_draft_tokens must be in [1, {B * K}], got {D}")
+        left = [int(n) for n in left]
+        self._setup(model, cache, layers, first_token, chunk, use_graph, None, pad_token_id, None)
+        dev = self.ids.device
+        self.state.workspace = self.backend.decode_workspace(B * layers[0].num_q_heads * (K + 1), layers[0].k_buf.shape[3], dev)
+        self.state.spec = True
+        self.spec = SpecState(prompts, self.ids, max(left + [int(history)]) + 1, K, max_ngram, eos_token_id, pad_token_id, dev,
+                              budgets=left, out_cap=chunk * (K + 1))
+        self.state.pack = PackState(B, K, D, self.state.step, dev)
+        self.ids, self.pos, self.done = self.spec.ids, self.spec.pos, self.spec.done
+        self._cols = torch.arange(K + 1, device=dev)
+        self._no_offset = torch.zeros(1, dtype=torch.int32, device=dev)   # admissions install absolute row counts
+        self.captures = 0
+        self.parked = set()
+        self.forced_drafts = None
+        if forced_drafts is not None:
+            self.forced_drafts = forced_drafts.to(device=dev, dtype=torch.long).contiguous()
+            self._offsets = torch.arange(K, device=dev)
+        self.backend.prompt_lookup(self.spec)
+        if self.forced_drafts is not None:
+            self._force_drafts()
+
+    def _verify_logits(self) -> torch.Tensor:
+        """The forward of the packed rows: logits [1, M, V]."""
+        return _forward_rows(self.model, self.cache, self.state.pack.ids, self.state.pack.pos)
+
+    def _step(self) -> None:
+        st, pk = self.spec, self.state.pack
+        self.backend.spec_pack(st, pk)
+        am = self._verify_logits().argmax(dim=-1)[0]                           # [M]
+        # slot b's argmaxes t_j sit at rows row_start[b] + j, j < row_count[b]; the rest are never read by the step
+        st.tokens.copy_(am[(pk.row_start.long()[:, None] + self._cols).clamp_(max=am.numel() - 1)])
+        self.backend.spec_step(st, [l.rows for l in self.layers])
+        if self.forced_drafts is not None:
+            self._force_drafts()
+        self.state.step.add_(1)
+
+    def _counters(self) -> list:
+        return super()._counters() + [self.state.step, self.state.pack.totals]
+
+    def run_chunk(self, steps: int) -> list:
+        """Take `steps` (<= chunk) steps; per slot, the tokens they emitted (host lists, one device-to-host read)."""
+        self.run(steps)
+        st = self.spec
+        host = torch.cat([st.out, st.out_len.long()[:, None]], dim=1).cpu()
+        st.out_len.zero_()
+        self.taken = 0
+        return [host[b, : int(host[b, -1])].tolist() for b in range(host.shape[0])]
+
+    def admit(self, slot: int, src_cache, first_token: torch.Tensor, left: int, sampling: Optional[SamplingParams] = None,
+              prompt=None, forced: Optional[torch.Tensor] = None) -> None:
+        """Slot `slot` continues the prefilled prompt `prompt` (its cache `src_cache`, first token `first_token`, `left`
+        tokens to emit): its history row and cache rows are rewritten in place (the rows at their absolute counts), and
+        the lookup drafts again (unchanged for the other slots). `forced`: the request's forced drafts, with
+        `forced_drafts`."""
+        if sampling is not None:
+            raise ValueError("admit: prompt-lookup speculation is greedy only")
+        if self.spec.set_row(slot, prompt, first_token, left):
+            self.graph = None
+        admit_cache(self.cache, slot, src_cache, self._no_offset, self.backend)
+        if self.forced_drafts is not None:
+            self.forced_drafts[slot].fill_(self.pad_token_id)
+            f = forced.reshape(-1)[: self.forced_drafts.shape[1]]
+            self.forced_drafts[slot, : f.numel()] = f.to(self.forced_drafts.device)
+        self.backend.prompt_lookup(self.spec)
+        if self.forced_drafts is not None:
+            self._force_drafts()
+        self.parked.discard(slot)
+
+    def park(self, slot: int) -> None:
+        self.done[slot] = True
+        self.parked.add(slot)
+
+
 def _sync(device: torch.device) -> None:
     if device.type == "cuda":
         torch.cuda.synchronize(device)
@@ -1209,7 +1351,9 @@ def _sync(device: torch.device) -> None:
 @torch.no_grad()
 def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, eos_token_id=None, pad_token_id: int = 0,
                                use_graph: Optional[bool] = None, check_every: int = 16, return_stats: bool = False,
-                               sampling=None, logprobs: Optional[int] = None):
+                               sampling=None, logprobs: Optional[int] = None, prompt_lookup_num_tokens: Optional[int] = None,
+                               max_matching_ngram_size: Optional[int] = None, max_draft_tokens: Optional[int] = None,
+                               _forced_drafts=None):
     """Greedy generation for any number of prompts (1-D or [1, S] id tensors) through `num_slots` sequences decoded together
     (continuous batching). `max_new_tokens`: an int, or one per prompt. The first `num_slots` prompts are prefilled one at a
     time and joined exactly as in `greedy_generate_batch`; decoding then runs in chunks of `check_every` steps. After each
@@ -1223,7 +1367,14 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     SamplingParams for all prompts, or one per prompt) is given: each request's tokens are then drawn with its own, and
     equal those it gets from `greedy_generate_batch` with the same parameters wherever its logits are equal there. With
     `logprobs` = N (0 to 20) the return value gains, as its last element, one `TokenLogprobs` per prompt for its generated
-    tokens, read with the tokens once per chunk (DESIGN.md §4.8)."""
+    tokens, read with the tokens once per chunk (DESIGN.md §4.8).
+    `prompt_lookup_num_tokens` = K / `max_matching_ngram_size` = N: greedy prompt-lookup speculation as in
+    `greedy_generate` (`ContinuousSpecDecoder`, DESIGN.md §4.14): each step verifies one token per live slot plus at most
+    `max_draft_tokens` = D draft tokens shared by the slots (1 to num_slots * K, default num_slots * K), packed into
+    num_slots + D rows. The stats then gain `granted_drafts` and `accepted_drafts` (run totals), and live_slot_steps counts
+    verify steps of live slots. Every cache form but the decode window runs; greedy only. `_forced_drafts` (tests and
+    measurements): one 1-D id tensor per prompt; after every step its slot drafts from it at the index of its tokens so far
+    (the first included), in place of the lookup."""
     ids = [p.reshape(1, -1) for p in prompts]
     if not ids:
         raise ValueError("greedy_generate_continuous: no prompts")
@@ -1233,6 +1384,16 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     if int(num_slots) < 1:
         raise ValueError(f"greedy_generate_continuous: num_slots must be >= 1, got {num_slots}")
     eos = _eos_set(eos_token_id)
+    spec = _check_spec(prompt_lookup_num_tokens, max_matching_ngram_size, sampling, logprobs, "greedy_generate_continuous")
+    if spec is None and max_draft_tokens is not None:
+        raise ValueError("greedy_generate_continuous: max_draft_tokens goes with prompt_lookup_num_tokens")
+    if spec is not None:
+        _check_spec_cache_form(model)
+        hi = int(num_slots) * spec[0]
+        if max_draft_tokens is not None and (isinstance(max_draft_tokens, bool) or not isinstance(max_draft_tokens, int)
+                                             or not 1 <= max_draft_tokens <= hi):
+            raise ValueError(f"greedy_generate_continuous: max_draft_tokens must be an integer in [1, {hi}] "
+                             f"(num_slots * prompt_lookup_num_tokens), got {max_draft_tokens!r}")
     samp = _sampling_list(sampling, len(ids), "greedy_generate_continuous")
     logprobs = _check_logprobs(logprobs, "greedy_generate_continuous")
     chunk = max(1, int(check_every))
@@ -1270,11 +1431,28 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
     cache = join_caches(list(caches), reserve=max(caps))
     del caches
     slot_req = list(range(B))
-    dec = ContinuousDecoder(model, cache, torch.cat(firsts), [0 if finished(b) else caps[b] - 1 for b in range(B)], chunk,
-                            use_graph=use_graph, eos_token_id=sorted(eos) if eos else None, pad_token_id=pad_token_id,
-                            sampling=None if samp is None else samp[:B], logprobs=logprobs, prompts=ids[:B],
-                            penalties=samp is not None and any(p.penalized for p in samp),
-                            constraints=samp is not None and any(p.constrained for p in samp), history=max(caps))
+    left = [0 if finished(b) else caps[b] - 1 for b in range(B)]
+    forced = None
+    if spec is None:
+        dec = ContinuousDecoder(model, cache, torch.cat(firsts), left, chunk,
+                                use_graph=use_graph, eos_token_id=sorted(eos) if eos else None, pad_token_id=pad_token_id,
+                                sampling=None if samp is None else samp[:B], logprobs=logprobs, prompts=ids[:B],
+                                penalties=samp is not None and any(p.penalized for p in samp),
+                                constraints=samp is not None and any(p.constrained for p in samp), history=max(caps))
+    else:
+        K, N = spec
+        if _forced_drafts is not None:
+            width = max(caps) + K
+            forced = [torch.full((width,), int(pad_token_id), dtype=torch.long) for _ in ids]
+            for f, src in zip(forced, _forced_drafts):
+                src = torch.as_tensor(src, dtype=torch.long).reshape(-1)[:width].cpu()
+                f[: src.numel()] = src
+        D = min(B * K, max_draft_tokens if max_draft_tokens is not None else int(num_slots) * K)
+        dec = ContinuousSpecDecoder(model, cache, torch.cat(firsts), [p.reshape(-1) for p in ids[:B]], left, chunk, K, N, D,
+                                    use_graph=use_graph, eos_token_id=sorted(eos) if eos else None,
+                                    pad_token_id=pad_token_id, history=max(caps),
+                                    forced_drafts=None if forced is None else torch.stack(forced[:B]))
+    decoded = 0                                    # tokens the decode steps emitted
     waiting = B
     while True:
         for s in range(B):
@@ -1288,7 +1466,8 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
                 if finished(i):
                     continue
                 stats["regrowths"] += int(dec.grow_for(single, caps[i]))
-                dec.admit(s, single, first, caps[i] - 1, None if samp is None else samp[i], ids[i])
+                dec.admit(s, single, first, caps[i] - 1, None if samp is None else samp[i], ids[i],
+                          **({} if forced is None else {"forced": forced[i]}))
                 stats["admissions"] += 1
                 slot_req[s] = i
             if slot_req[s] is None:
@@ -1301,13 +1480,17 @@ def greedy_generate_continuous(model, prompts, max_new_tokens, num_slots: int, e
         stats["decode_steps"] += n
         for s in live:
             r = slot_req[s]
-            for j, t in enumerate(toks[s].tolist()):
+            for j, t in enumerate(toks[s] if spec is not None else toks[s].tolist()):
                 push(r, t)
-                stats["live_slot_steps"] += 1
+                decoded += 1
                 if finished(r):
                     break
             if logprobs is not None:
                 lps[r].append(tuple(x[s, : j + 1] for x in dec.chunk_logprobs))
+    stats["live_slot_steps"] = decoded
+    if spec is not None:
+        granted, live_steps = dec.state.pack.totals.tolist()
+        stats.update(live_slot_steps=live_steps, granted_drafts=granted, accepted_drafts=decoded - live_steps)
     dec.finish()
     stats["graph_captures"] = dec.captures
     stats["decode_s"] = time.perf_counter() - t_start - stats["prefill_s"]

@@ -202,6 +202,15 @@ class CudaBackend:
     def spec_step(self, st, rows):
         ops.spec_step(st, rows)
 
+    # prompt-lookup speculation in the continuous loop (generate.ContinuousSpecDecoder)
+    def decode_attn_packed(self, q, k_buf, v_buf, k_new, v_new, row_start, row_count, num_queries, rows=None, max_length=0,
+                           scales=None, gqa=False, workspace=None, out=None, softmax_scale=0.0):
+        return ops.decode_attn_packed(q, k_buf, v_buf, k_new, v_new, row_start, row_count, num_queries, rows, max_length,
+                                      scales, gqa, workspace, out, softmax_scale)
+
+    def spec_pack(self, st, pk):
+        ops.spec_pack(st, pk)
+
     @staticmethod
     def check_knobs(method: str, window_size: int, max_capacity_prompt=None) -> None:
         """What the sm_90a scoring kernels take, checked when the cluster is built (the reference accepts any window_size;

@@ -10,7 +10,7 @@ from typing import Dict, Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import METHODS, POOLING, SCORE_KERNELS, DecodeDesc, DecodeHeavy, DecodeMulti, DecodeWindow, EvictDesc, RopeDesc, SpecDesc, WsLayout
+from ._lib import METHODS, POOLING, SCORE_KERNELS, DecodeDesc, DecodeHeavy, DecodeMulti, DecodePacked, DecodeWindow, EvictDesc, RopeDesc, SpecDesc, SpecPackDesc, WsLayout
 
 _DTYPES = {torch.bfloat16: 0, torch.float16: 1}
 
@@ -1121,6 +1121,17 @@ def decode_attn_multi(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor,
             most = int(rows.max()) + int(length) + (int(step) if step is not None else 0) + Q
             if most > max_length:
                 raise ValueError(f"{what}: cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
+    d, m = _multi_descs(q, k_buf, v_buf, k_new, v_new, rows, length, step, max_length, scales, gqa, workspace, out,
+                        softmax_scale, B, Q)
+    _lib.check(_lib.lib().pkv_decode_attn_multi(C.byref(d), C.byref(m), torch.cuda.current_stream(q.device).cuda_stream))
+    return out
+
+
+def _multi_descs(q, k_buf, v_buf, k_new, v_new, rows, length, step, max_length, scales, gqa, workspace, out, softmax_scale,
+                 B: int, Q: int):
+    """The pkv_decode_desc and pkv_decode_multi of a verify launch over B sequences of up to Q new rows; q, k_new, v_new and
+    out are [.., tokens, H, D] with the token stride at dim 1."""
+    Hq, Hkv, D = q.shape[2], k_new.shape[2], q.shape[3]
     d = DecodeDesc()
     d.struct_bytes = C.sizeof(DecodeDesc)
     d.dtype, d.num_q_heads, d.num_kv_heads, d.head_dim = _dtype_code(q), Hq, Hkv, D
@@ -1144,7 +1155,66 @@ def decode_attn_multi(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor,
     m.q_stride_t, m.q_stride_h = q.stride(1), q.stride(2)
     m.kv_stride_t, m.kv_stride_h = k_new.stride(1), k_new.stride(2)
     m.out_stride_t, m.out_stride_h = out.stride(1), out.stride(2)
-    _lib.check(_lib.lib().pkv_decode_attn_multi(C.byref(d), C.byref(m), torch.cuda.current_stream(q.device).cuda_stream))
+    return d, m
+
+
+def decode_attn_packed(q: torch.Tensor, k_buf: torch.Tensor, v_buf: torch.Tensor, k_new: torch.Tensor, v_new: torch.Tensor,
+                       row_start: torch.Tensor, row_count: torch.Tensor, num_queries: int, rows: Optional[torch.Tensor] = None,
+                       max_length: int = 0, scales=None, gqa: bool = False, workspace: Optional[torch.Tensor] = None,
+                       out: Optional[torch.Tensor] = None, softmax_scale: float = 0.0) -> torch.Tensor:
+    """`decode_attn_multi` over packed token rows (`pkv_decode_attn_packed`): q [1, M, Hq, D] and k_new / v_new
+    [1, M, Hkv, D] (the projections of a [1, M] forward, read in place); sequence b owns the rows [row_start[b],
+    row_start[b] + row_count[b]) (int32 device [B], counts in [0, num_queries], ranges ascending). Its query j stores its
+    new row at rows[b*H + c] + j and attends the rows up to it. Rows no sequence owns get a zero output. Returns out
+    [1, M, Hq, D]."""
+    what = "decode_attn_packed"
+    _require_cuda(q, k_buf, v_buf, k_new, v_new, row_start, row_count, rows, workspace, out, *(scales or ()))
+    if scales is not None:
+        _check_fp8_buffers(k_buf, v_buf, scales[0], scales[1], what)
+    elif k_buf.dim() != 4 or k_buf.shape != v_buf.shape or k_buf.stride() != v_buf.stride() or k_buf.stride(3) != 1 \
+            or k_buf.stride(2) != k_buf.shape[3]:
+        raise ValueError(f"{what}: k_buf / v_buf must be [B, H, capacity, D] tensors of equal shape and strides, rows contiguous")
+    B, H, cap, D = k_buf.shape
+    Q = int(num_queries)
+    if not 1 <= Q <= _lib.MAX_SPEC_QUERIES:
+        raise ValueError(f"{what}: num_queries must be in [1, {_lib.MAX_SPEC_QUERIES}], got {Q}")
+    if q.dim() != 4 or q.shape[0] != 1 or q.shape[3] != D or not 1 <= q.shape[1] < 2 ** 31:
+        raise ValueError(f"{what}: q must be [1, M, Hq, D={D}], got {tuple(q.shape)}")
+    M, Hq = q.shape[1], q.shape[2]
+    Hkv = k_new.shape[2] if k_new.dim() == 4 else -1
+    if k_new.shape != (1, M, Hkv, D) or v_new.shape != k_new.shape or Hkv < 1 or Hq % Hkv \
+            or k_new.dtype != q.dtype or v_new.dtype != q.dtype or (H != (Hkv if gqa else Hq)):
+        raise ValueError(f"{what}: k_new / v_new must be [1, M, Hkv, D] of q's dtype, and the cache hold "
+                         f"{'Hkv' if gqa else 'Hq'} heads; got {tuple(k_new.shape)}, {tuple(v_new.shape)}, cache heads {H}")
+    for name, t in (("row_start", row_start), ("row_count", row_count)):
+        if t.dtype != torch.int32 or t.numel() != B or not t.is_contiguous():
+            raise ValueError(f"{what}: {name} must be a contiguous int32 device tensor of B = {B} elements")
+    q, k_new, v_new = _token_rows(q), _token_rows(k_new), _token_rows(v_new)
+    if k_new.stride() != v_new.stride():
+        k_new, v_new = k_new.contiguous(), v_new.contiguous()
+    if out is None:
+        out = torch.empty(1, M, Hq, D, dtype=q.dtype, device=q.device)
+    elif out.shape != (1, M, Hq, D) or not out.is_contiguous() or out.dtype != q.dtype:
+        raise ValueError(f"{what}: out must be a contiguous [1, M, Hq, D] tensor of q's dtype")
+    max_length = int(max_length) or cap
+    if not Q <= max_length <= cap:
+        raise ValueError(f"{what}: cache capacity {cap} exceeded (max_length {max_length})")
+    if rows is not None:
+        if rows.dtype != torch.int32 or rows.numel() != B * H or not rows.is_contiguous():
+            raise ValueError(f"{what}: rows must be a contiguous int32 device tensor of B*H = {B * H} elements")
+        if not torch.cuda.is_current_stream_capturing():
+            # (one device read; a captured launch relies on the caller, and the kernel writes no row of a count out of range)
+            end = rows.view(B, H) + row_count.view(B, 1)
+            most = int(end[row_count > 0].max()) if bool((row_count > 0).any()) else 0
+            if most > max_length:
+                raise ValueError(f"{what}: cache capacity exceeded: {most} rows for max_length {max_length} (capacity {cap})")
+    d, m = _multi_descs(q, k_buf, v_buf, k_new, v_new, rows, 0, None, max_length, scales, gqa, workspace, out, softmax_scale,
+                        B, Q)
+    p = DecodePacked()
+    p.struct_bytes, p.total_rows = C.sizeof(DecodePacked), M
+    p.row_start, p.row_count = row_start.data_ptr(), row_count.data_ptr()
+    _lib.check(_lib.lib().pkv_decode_attn_packed(C.byref(d), C.byref(m), C.byref(p),
+                                                 torch.cuda.current_stream(q.device).cuda_stream))
     return out
 
 
@@ -1189,6 +1259,27 @@ def prompt_lookup(st) -> None:
     length from its history."""
     d, _ = _spec_desc("prompt_lookup", st)
     _lib.check(_lib.lib().pkv_prompt_lookup(C.byref(d), torch.cuda.current_stream(st.ids.device).cuda_stream))
+
+
+def spec_pack(st, pk) -> None:
+    """Rule 2' of include/pkv.h (`pkv_spec_pack`) for the SpecState `st` into the packed state `pk`
+    (`generate.PackState`: max_draft_tokens, ids / pos int64 [1, M], row_start / row_count int32 [B], step int32 [1],
+    totals int64 [2]); truncates st.draft_len in place."""
+    d, _ = _spec_desc("spec_pack", st)
+    B = st.ids.shape[0]
+    for name, dt, n in (("ids", torch.int64, None), ("pos", torch.int64, None), ("row_start", torch.int32, B),
+                        ("row_count", torch.int32, B), ("step", torch.int32, 1), ("totals", torch.int64, 2)):
+        t = getattr(pk, name)
+        _require_cuda(t)
+        if t.dtype != dt or not t.is_contiguous() or (n is not None and t.numel() != n) or t.numel() > 2 ** 31 - 1:
+            raise ValueError(f"spec_pack: {name} must be a contiguous {dt} device tensor" + (f" of {n} elements" if n else ""))
+    if pk.pos.numel() != pk.ids.numel():
+        raise ValueError("spec_pack: ids and pos must hold M elements each")
+    k = SpecPackDesc()
+    k.struct_bytes, k.max_draft_tokens, k.total_rows = C.sizeof(SpecPackDesc), int(pk.max_draft_tokens), pk.ids.numel()
+    k.step, k.ids, k.pos = pk.step.data_ptr(), pk.ids.data_ptr(), pk.pos.data_ptr()
+    k.row_start, k.row_count, k.totals = pk.row_start.data_ptr(), pk.row_count.data_ptr(), pk.totals.data_ptr()
+    _lib.check(_lib.lib().pkv_spec_pack(C.byref(d), C.byref(k), torch.cuda.current_stream(st.ids.device).cuda_stream))
 
 
 def spec_step(st, rows) -> None:

@@ -271,21 +271,27 @@ def _run_batch_static(model, prompts: List[torch.Tensor], max_new_tokens: int, u
     return res, per_seq * len(prompts)
 
 
-def _run_continuous(model, prompts: List[torch.Tensor], max_new_tokens: List[int], slots: int):
+def _run_continuous(model, prompts: List[torch.Tensor], max_new_tokens: List[int], slots: int,
+                    prompt_lookup_num_tokens: Optional[int] = None):
     """All prompts through one greedy_generate_continuous with `slots` slots (graph replay), after an untimed warm-up prefill
-    per prompt length. Returns (one PromptResult per prompt, the run's `continuous` record block)."""
+    per prompt length. Returns (one PromptResult per prompt, the run's `continuous` record block). prompt_lookup_num_tokens
+    K: greedy prompt-lookup speculation in the loop (ContinuousSpecDecoder); the block then carries granted_drafts and
+    accepted_drafts."""
     from .generate import _prefill, greedy_generate_continuous
     dev = prompts[0].device
     with torch.no_grad():
         for n in sorted({int(p.shape[1]) for p in prompts}):
             _prefill(model, next(p for p in prompts if p.shape[1] == n))
         _sync(dev)
-        seqs, st = greedy_generate_continuous(model, prompts, max_new_tokens, slots, return_stats=True)
+        seqs, st = greedy_generate_continuous(model, prompts, max_new_tokens, slots, return_stats=True,
+                                              prompt_lookup_num_tokens=prompt_lookup_num_tokens)
     steps = st["decode_steps"]
     block = {"slots": min(slots, len(prompts)), "decode_steps": steps,
              "occupancy": st["live_slot_steps"] / max(1, min(slots, len(prompts)) * steps),
-             "aggregate_tok_per_s": st["live_slot_steps"] / max(st["decode_s"], 1e-9),
-             "admissions": st["admissions"], "regrowths": st["regrowths"], "graph_captures": st["graph_captures"]}
+             # (with speculation a live slot-step emits 1 + its accepted drafts)
+             "aggregate_tok_per_s": (st["live_slot_steps"] + st.get("accepted_drafts", 0)) / max(st["decode_s"], 1e-9),
+             "admissions": st["admissions"], "regrowths": st["regrowths"], "graph_captures": st["graph_captures"],
+             **{k: st[k] for k in ("granted_drafts", "accepted_drafts") if k in st}}
     res = []
     for i, (p, n, s) in enumerate(zip(prompts, max_new_tokens, seqs)):
         pred = s[p.shape[1]:].tolist()
@@ -354,8 +360,8 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
     decode_loop "continuous": every prompt goes through one greedy_generate_continuous with eval_batch_size slots, whatever
     its max_new_tokens; each record keeps its own prefill_ms, cache rows and tokens and carries the run's "continuous" block
     (slots, decode_steps, occupancy, aggregate_tok_per_s) instead of a per-prompt decode rate.
-    prompt_lookup_num_tokens K (static loops, eval_batch_size 1, an eviction method): greedy prompt-lookup speculative
-    decoding with K draft tokens per step; the records then carry "prompt_lookup_num_tokens"."""
+    prompt_lookup_num_tokens K (an eviction method; the static loops with eval_batch_size 1, or the continuous loop): greedy
+    prompt-lookup speculative decoding with K draft tokens per step; the records then carry "prompt_lookup_num_tokens"."""
     if kv_cache_dtype not in ("auto", "fp8_e4m3"):
         raise ValueError(f"kv_cache_dtype must be auto or fp8_e4m3, got {kv_cache_dtype!r}")
     if kv_cache_dtype != "auto" and canonical_method(method) == "fullkv":
@@ -376,10 +382,10 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
                                   "use --decode_loop static or static-eager with an eviction method (padded HF batches are not supported)")
     if decode_loop not in ("hf", "static", "static-eager", "continuous"):
         raise ValueError(f"decode_loop must be hf, static, static-eager or continuous, got {decode_loop!r}")
-    if prompt_lookup_num_tokens is not None and (decode_loop not in ("static", "static-eager") or eval_batch_size > 1
-                                                 or canonical_method(method) == "fullkv"):
-        raise NotImplementedError("--prompt_lookup_num_tokens runs in the static loop with eval_batch_size 1 and an eviction "
-                                  "method")
+    if prompt_lookup_num_tokens is not None and (decode_loop == "hf" or canonical_method(method) == "fullkv"
+                                                 or (not continuous and eval_batch_size > 1)):
+        raise NotImplementedError("--prompt_lookup_num_tokens runs with an eviction method in the static loop with "
+                                  "eval_batch_size 1, or in the continuous loop")
     if device is None:
         if not torch.cuda.is_available():
             raise RuntimeError("the runners need a CUDA device (H100, sm_90a); there is no CPU fallback")
@@ -436,7 +442,7 @@ def run_suite(arch: str, method: str, max_capacity_prompt: int, prompts: Iterabl
                 window = set_knobs(model, method, round(prompts[0][1] * capacity_ratio), merge, backend_factory, floor, head_beta, head_path)
             ids = [synthetic_prompt(model.config.vocab_size, p[1], seed + j, device) for j, p in enumerate(prompts)]
             if ids:
-                rs, block = _run_continuous(model, ids, [p[2] for p in prompts], eval_batch_size)
+                rs, block = _run_continuous(model, ids, [p[2] for p in prompts], eval_batch_size, prompt_lookup_num_tokens)
                 emit(range(len(prompts)), rs, {"continuous": block})
             return records
         i = 0

@@ -57,8 +57,8 @@ def build_parser() -> argparse.ArgumentParser:
                    help="hf: model.generate as in the reference; static: pyramidkv_b200.generate (CUDA-graph replay per token); "
                         "continuous: every prompt through --eval_batch_size slots, a finished sequence's slot taking the next prompt")
     p.add_argument("--prompt_lookup_num_tokens", type=int, default=None,
-                   help="--decode_loop static: greedy prompt-lookup speculative decoding with K (1..15) draft tokens per step "
-                        "(HF's generate argument of that name; DESIGN.md §4.13)")
+                   help="--decode_loop static or continuous: greedy prompt-lookup speculative decoding with K (1..15) draft "
+                        "tokens per step (HF's generate argument of that name; DESIGN.md §4.13, §4.14)")
     p.add_argument("--kv_cache_dtype", type=str, default="auto", choices=["auto", "fp8_e4m3"],
                    help="auto: the compacted cache in the model dtype; fp8_e4m3: FP8 bytes + one fp32 scale per row (half the KV bytes)")
     p.add_argument("--gqa_shared", action="store_true",
